@@ -6,10 +6,15 @@ backward -> single gradient all-reduce -> Adam) of the speech Transformer, BASEL
     python bench.py --gpus N --steps K --warmup W                 # ours  (torchrun launches N>1)
     python bench.py --impl reference --gpus N --steps K --warmup W    # the reference algorithm on the host CPU
 
-Prints ONE JSON line (see the task contract): `value` = whole-job utt/s with inputs resident in HBM, `e2e` = the same
+Prints ONE JSON line: `value` = whole-job utt/s with inputs resident in HBM, `e2e` = the same
 step through the public API with pinned-host inputs copied in and the loss read back every step, `roofline` for the
 dominant kernel group (CUDA-event timed on the launching stream inside the timed region), `cpu_baseline` = the oracle
 port on the host cores (rank 0, N=1).  Data are synthetic, weights random-init (no network for corpora/checkpoints).
+
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR
+
+also writes what the last timed step computed (see dump_outputs) as DIR/<name>.npy; with the same arguments the inputs,
+weights and dropout streams are the same from run to run, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -29,17 +34,13 @@ METRIC = "utterances/sec (fwd+bwd) dim512/4L/8H T_src=800"
 
 
 def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
-                    source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    """H100 SXM data-sheet peaks (dense, 700 W card): 3.35 TB/s HBM3, 989 TFLOP/s BF16.  Data-sheet figures, not measured;
+    a card run at a lower power limit or clock reaches less."""
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -193,8 +194,8 @@ def reference_flags(cfg, cuda=False):
 
 
 def build_reference(cfg, cuda=False):
-    """The UNMODIFIED reference model + its own optimizer (utils/functions.py:101-152), imported from /root/reference or the
-    staged oracle/_ref (oracle/make_ref.py).  Returns (namespace, model, opt) or None when the checkout is absent."""
+    """The UNMODIFIED reference model + its own optimizer (utils/functions.py:101-152), imported from the reference checkout
+    staged in oracle/_ref (oracle/make_ref.py).  Returns (namespace, model, opt) or None when the checkout is absent."""
     from oracle import ref_shim
     if not ref_shim.available():
         return None
@@ -248,7 +249,7 @@ def cpu_reference_throughput(batch, steps, warmup, threads=None):
 
 
 def gpu_reference_throughput(dev, batch, steps=5, warmup=3):
-    """The unmodified reference, eager, ON THE SAME B200 (SURVEY.md 8d: "the kernel-for-kernel bar"): same step as
+    """The unmodified reference, eager, ON THE SAME GPU (SURVEY.md 8d: "the kernel-for-kernel bar"): same step as
     reference_step, inputs resident on the device, CUDA-event timed; once with PyTorch's default flags (cuDNN convolutions
     may use TF32, matmuls are fp32) and once with allow_tf32 everywhere.  None when the checkout is not staged."""
     import b200asr
@@ -306,6 +307,30 @@ def run_reference(args, rank, world):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU arm
+def dump_outputs(out_dir, step_out, dp):
+    """What the last timed step handed back to its caller, as float32 / float64 .npy files (< 64 MB in all): the logits
+    (a fixed, seeded sample of 2^20 of them), the greedy ids, [sum of row losses, tokens, correct] and the mean loss of the
+    step, and fixed, seeded samples of the parameters after the optimizer step and of the gradients it applied."""
+    import numpy as np
+    pred, hyp, stats = step_out
+    os.makedirs(out_dir, exist_ok=True)
+    g = torch.Generator().manual_seed(20260901)
+
+    def sample(t, n=1 << 20):
+        flat = t.detach().reshape(-1)
+        if flat.numel() <= n:
+            return flat.float()
+        idx = torch.randperm(flat.numel(), generator=g)[:n].sort().values
+        return flat[idx.to(flat.device)].float()
+
+    n = dp.flat.numel
+    arrays = {"logits_sample": sample(pred), "hyp": hyp.double(), "stats": stats.double(),
+              "loss": dp.global_loss().reshape(1).double(), "params_sample": sample(dp.flat.flat[:n]),
+              "grads_sample": sample(dp.flat.flat_grad[:n])}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.cpu().numpy())
+
+
 def run_b200(args, rank, local_rank, world):
     import torch.distributed as dist
     import b200asr
@@ -358,10 +383,12 @@ def run_b200(args, rank, local_rank, world):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        dp.step(src_d, lens_d, tgt_d)
+        last = dp.step(src_d, lens_d, tgt_d)
     e1.record()
     barrier()
     launches = (lib.b200asr_launch_count() - launches0) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, dp)
     ms_dev = max_over_ranks(e0.elapsed_time(e1)) / args.steps
     # ---- forward + loss + backward alone (BASELINE.json's metric names fwd+bwd; `value` above is the whole step incl. the
     #      all-reduce and Adam): single GPU only, the weights do not change so the operand cache stays valid
@@ -440,25 +467,13 @@ def run_b200(args, rank, local_rank, world):
     peaks = load_peaks()
     groups = summarize_profile(report, prof_steps, peaks)
     top = next((g for g in groups if g["gflop_per_step"] > 0), groups[0])
-    tf32_peak = peaks["bf16_tflops_sustained"] / 2.0       # kind::tf32 runs at half the bf16 rate
-    # DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the dominant group come from the tracked ncu
-    # summary profiles/ncu_traffic.json (written by tools/ncu_traffic.py from an `ncu --set full` capture of this very
-    # command; it records the git revision it was taken at) -- null when that file has no entry for the group
-    traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            tj = json.load(f)
-        ent = tj.get("groups", {}).get(top["kernel"])
-        if ent:
-            traffic, traffic_src = ent["dram_bytes_per_launch"], f"profiles/ncu_traffic.json (git {tj.get('git', '?')}, {ent.get('launches', '?')} launches)"
-    except Exception:
-        pass
+    tf32_peak = peaks["bf16_tflops_sustained"] / 2.0       # tf32 MMAs run at half the bf16 rate
     roof = {"bound": "tensor", "kernel": top["kernel"], "achieved": top["tflops"], "peak": tf32_peak, "unit": "TFLOP/s",
-            "frac": top["tflops"] / tf32_peak, "traffic": traffic, "traffic_source": traffic_src,
+            "frac": top["tflops"] / tf32_peak,
             "peak_source": f"{peaks['source']} bf16_tflops_sustained/2 (TF32 = half the bf16 tensor rate)",
             "share_of_step": top["share"],
             # 3xTF32 issues three tf32 MMAs per algorithmic product, so `frac` tops out at 1/3 for precision-3 kernels;
-            # the tensor-pipe occupancy is frac * mma_per_product (ncu: sm__pipe_tensor_cycles_active, profiles/)
+            # the tensor-pipe occupancy is frac * mma_per_product
             "mma_per_product": 3 if ops.config.conv_wgrad == 3 else 1,
             "tensor_pipe_frac": top["tflops"] / tf32_peak * (3 if ops.config.conv_wgrad == 3 else 1)}
     # BASELINE.json asks for the achieved fraction of the attention-matmul roofline next to the headline number
@@ -468,8 +483,8 @@ def run_b200(args, rank, local_rank, world):
     attention = {"ms_per_step": att_ms, "gflop_per_step": att_gf, "achieved": att_gf / att_ms if att_ms else 0.0, "unit": "TFLOP/s",
                  "peak": tf32_peak, "frac": (att_gf / att_ms / tf32_peak) if att_ms else 0.0, "mma_per_product": mult,
                  "tensor_pipe_frac": (att_gf / att_ms / tf32_peak * mult) if att_ms else 0.0,
-                 "note": ("fused kind::f16 (bf16x3) kernels: QK^T / PV (+ the four backward products, scores recomputed) with masks, "
-                          "softmax and dropout on the accumulator in tensor memory; includes the bf16 operand pre-pass")
+                 "note": ("fused bf16x3 kernels: QK^T / PV (+ the four backward products, scores recomputed) with masks, "
+                          "softmax and dropout on the score fragments in registers")
                  if any(g["kernel"].startswith("sdpa_fused") for g in att) else
                  ("materialised path: batched per-head 3xTF32 GEMMs on the tile engine (QK^T, PV and the four backward products) "
                   "around fp32 softmax / dropout kernels; scores and probabilities stay L2-resident")}
@@ -480,9 +495,9 @@ def run_b200(args, rank, local_rank, world):
                       "dropout": cfg.dropout, "label_smoothing": cfg.label_smoothing,
                       "precision": {"linear": ops.config.linear, "conv": ops.config.conv, "conv_wgrad": ops.config.conv_wgrad,
                                     "attn": ops.config.attn, "attn_bwd": ops.config.attn_bwd,
-                                    "legend": "0 = fp32 CUDA cores, 1 = tcgen05 TF32 (RN), 3 = tcgen05 3xTF32 (fp32-grade)"},
+                                    "legend": "0 = fp32 CUDA cores, 1 = TF32 (RN), 3 = 3xTF32 (fp32-grade), 2 = bf16, 6 = bf16x3 (2-term bf16 split)"},
                       "step": "zero_grad+fwd+CE+bwd+allreduce+adam", "parallelism": f"dp{world}",
-                      "l2": "per-step working set (GBs of activations) >> 126 MB L2; no explicit flush"},
+                      "l2": "per-step working set (GBs of activations) >> 50 MB L2; no explicit flush"},
            "e2e": {"value": world * B / (ms_e2e / 1e3), "unit": "utt/s", "h2d_bytes_per_step": world * (src_h.numel() * 4 + tgt_h.numel() * 8),
                    "d2h_bytes_per_step": world * 4, "ms_per_step": ms_e2e, "wall_ms_per_step": wall_ms,
                    "how": "b200asr.HostBatchPrefetcher (pinned host batch copied on a side stream one step ahead, every step) -> "
@@ -519,6 +534,7 @@ def main():
     ap.add_argument("--precision", default="", help="linear,conv,attn[,conv_wgrad[,attn_bwd]] in {fp32,tf32,tf32x3} (default: package default)")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-ref-gpu", action="store_true", help="skip timing the unmodified reference eager on this GPU")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

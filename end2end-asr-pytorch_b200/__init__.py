@@ -1,8 +1,8 @@
-"""b200asr -- B200-native hot path of gentaiscool/end2end-asr-pytorch (teacher-forced Transformer-ASR fwd+bwd).
+"""b200asr -- H100-native hot path of gentaiscool/end2end-asr-pytorch (teacher-forced Transformer-ASR fwd+bwd).
 
-Everything computes in hand-written sm_100a CUDA kernels behind the C ABI of include/b200asr.h
+Everything computes in hand-written sm_90a CUDA kernels behind the C ABI of include/b200asr.h
 (libb200asr.so, built in-tree).  There is no CPU or stock-PyTorch fallback: importing is fine anywhere, running
-needs the built library and a B200.
+needs the built library and an H100.
 """
 from . import _lib
 from .config import ASRConfig, BASELINE_CONFIGS

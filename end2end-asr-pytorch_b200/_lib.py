@@ -1,7 +1,7 @@
 """ctypes binding of libb200asr.so (the C ABI declared in include/b200asr.h).
 
 The library is built in-tree by ``__graft_entry__.build()`` / ``build.sh``.  There is no fallback of any
-kind: if the shared object is missing, or the device is not an sm_100 part, importing callers get a
+kind: if the shared object is missing, or the device is not an sm_90 part (H100), importing callers get a
 RuntimeError that says so.
 """
 from __future__ import annotations
@@ -17,7 +17,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "b200asr.h")
 _lib = None
 
 PREC_FP32, PREC_TF32, PREC_TF32X3 = 0, 1, 3
-PREC_BF16, PREC_BF16X3 = 2, 6          # kind::f16 modes (include/b200asr.h)
+PREC_BF16, PREC_BF16X3 = 2, 6          # bf16 modes (include/b200asr.h)
 
 _vp, _i, _f, _u64, _ll, _sz = C.c_void_p, C.c_int, C.c_float, C.c_uint64, C.c_longlong, C.c_size_t
 

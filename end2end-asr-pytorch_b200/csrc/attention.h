@@ -1,4 +1,4 @@
-// Attention parameter block shared by the CUDA-core and tcgen05 kernels.
+// Attention parameter block shared by the CUDA-core and tensor-core kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -21,8 +21,10 @@ struct AttnP {
 
 int sdpa_fwd_simt(const AttnP& p, cudaStream_t st);
 int sdpa_bwd_simt(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st);
-// tcgen05 + TMA kernels (tc_attention.cu)
+// tensor-core kernels (tc_flash.cu): TF32 and the bf16x3 "fused" variant
 int sdpa_fwd_tc(const AttnP& p, cudaStream_t st);
 int sdpa_bwd_tc(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st);
+int sdpa_fused_fwd_tc(const AttnP& p, cudaStream_t st);
+int sdpa_fused_bwd_tc(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st);
 
 }  // namespace b200asr

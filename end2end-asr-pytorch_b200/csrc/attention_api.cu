@@ -1,4 +1,4 @@
-// b200asr_sdpa_fwd / b200asr_sdpa_bwd: argument checking and precision dispatch.
+// b200asr_sdpa_fwd / _bwd and b200asr_sdpa_fused_fwd / _bwd: argument checking and precision dispatch.
 #include "../../include/b200asr.h"
 #include "attention.h"
 #include "common.cuh"
@@ -43,7 +43,7 @@ int b200asr_sdpa_fwd(const float* q, const float* k, const float* v, long long q
   if (rc) return rc;
   if (precision == B200ASR_PREC_FP32) return sdpa_fwd_simt(p, (cudaStream_t)stream);
   if (precision == B200ASR_PREC_TF32) return sdpa_fwd_tc(p, (cudaStream_t)stream);
-  set_error("sdpa_fwd: precision %d unsupported (0 = fp32 CUDA cores, 1 = tcgen05 TF32)", precision);
+  set_error("sdpa_fwd: precision %d unsupported (0 = fp32 CUDA cores, 1 = TF32 tensor cores)", precision);
   return B200ASR_BAD_ARG;
 }
 
@@ -63,6 +63,45 @@ int b200asr_sdpa_bwd(const float* dout, const float* q, const float* k, const fl
   if (precision == B200ASR_PREC_TF32) return sdpa_bwd_tc(p, dout, dq, dk_out, dv_out, delta_ws, (cudaStream_t)stream);
   set_error("sdpa_bwd: precision %d unsupported", precision);
   return B200ASR_BAD_ARG;
+}
+
+// the fused workspaces keep their sizes: ws16 is reserved, ws_bwd = [2][B*H*Tq*64 rounded up to 64] bf16 slots, then delta
+static size_t ws16_elems(int B, int H, int T) { return ((size_t)B * H * T * 64 + 63) / 64 * 64; }
+
+size_t b200asr_sdpa_fused_ws_bytes(int B, int H, int Tq, int Tk) {
+  return 2 * (2 * ws16_elems(B, H, Tq) + 4 * ws16_elems(B, H, Tk));
+}
+
+size_t b200asr_sdpa_fused_bwd_ws_bytes(int B, int H, int Tq) {
+  return 2 * 2 * ws16_elems(B, H, Tq) + sizeof(float) * (((size_t)B * H * Tq + 3) / 4 * 4);
+}
+
+int b200asr_sdpa_fused_fwd(const float* q, const float* k, const float* v, long long q_bs, long long q_hs, long long q_rs,
+                           long long k_bs, long long k_hs, long long k_rs, long long v_bs, long long v_hs, long long v_rs,
+                           const uint8_t* key_pad, const uint8_t* dense_mask, int causal, float* out, long long o_bs,
+                           long long o_hs, long long o_rs, float* lse, void* ws16, int B, int H, int Tq, int Tk, int dk, int dv,
+                           float scale, float p_drop, uint64_t seed, uint64_t offset, b200asr_stream_t stream) {
+  B200_REQUIRE(ws16 && aligned16(ws16), B200ASR_BAD_ARG, "sdpa_fused_fwd: workspace");
+  AttnP p;
+  int rc = fill(p, q, k, v, out, lse, q_bs, q_hs, q_rs, k_bs, k_hs, k_rs, v_bs, v_hs, v_rs, o_bs, o_hs, o_rs, key_pad,
+                dense_mask, causal, B, H, Tq, Tk, dk, dv, scale, p_drop, seed, offset);
+  return rc ? rc : sdpa_fused_fwd_tc(p, (cudaStream_t)stream);
+}
+
+int b200asr_sdpa_fused_bwd(const float* dout, const float* q, const float* k, const float* v, const float* out, const float* lse,
+                           long long q_bs, long long q_hs, long long q_rs, long long k_bs, long long k_hs, long long k_rs,
+                           long long v_bs, long long v_hs, long long v_rs, long long o_bs, long long o_hs, long long o_rs,
+                           const uint8_t* key_pad, const uint8_t* dense_mask, int causal, float* dq, float* dk_out, float* dv_out,
+                           const void* ws16, void* ws_bwd, int B, int H, int Tq, int Tk, int dk, int dv, float scale, float p_drop,
+                           uint64_t seed, uint64_t offset, b200asr_stream_t stream) {
+  B200_REQUIRE(dout && dq && dk_out && dv_out && ws16 && ws_bwd, B200ASR_BAD_ARG, "sdpa_fused_bwd: null pointer");
+  B200_REQUIRE(aligned16(dout) && aligned16(dq) && aligned16(dk_out) && aligned16(dv_out) && aligned16(ws_bwd), B200ASR_BAD_ALIGN, "sdpa_fused_bwd: alignment");
+  AttnP p;
+  int rc = fill(p, q, k, v, const_cast<float*>(out), const_cast<float*>(lse), q_bs, q_hs, q_rs, k_bs, k_hs, k_rs, v_bs,
+                v_hs, v_rs, o_bs, o_hs, o_rs, key_pad, dense_mask, causal, B, H, Tq, Tk, dk, dv, scale, p_drop, seed, offset);
+  if (rc) return rc;
+  float* delta = (float*)((uint16_t*)ws_bwd + 2 * ws16_elems(B, H, Tq));
+  return sdpa_fused_bwd_tc(p, dout, dq, dk_out, dv_out, delta, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 // "Materialised" scaled-dot-product attention (precision 3 = 3xTF32, precision 1 = TF32): the contractions run as batched
-// tcgen05 GEMMs (tc_bgemm.cu) and the masked softmax / dropout and its backward are exact fp32 row kernels in between.
+// tensor-core GEMMs (tc_bgemm.cu) and the masked softmax / dropout and its backward are exact fp32 row kernels in between.
 //
 //   fwd:  S = Q K^T                  (bgemm, per head, written into `probs`)
 //         P = softmax(mask(S * scale)); Pd = dropout(P)      (softmax_fwd_kernel; P kept for backward, Pd only if p > 0)

@@ -1,7 +1,7 @@
 // Fused scaled-dot-product attention on CUDA cores (precision 0): flash-style online softmax, scores never
 // leave the SM.  64x64 (query x key) tiles, 256 threads, each thread owns a 4x4 strided micro-tile
 // (rows ty+16i, cols tx+16j) so that shared-memory reads are conflict free with 128-bit accesses.
-// This is the exact-fp32 path and the on-device cross-check of the tcgen05 attention kernel.
+// This is the exact-fp32 path and the on-device cross-check of the tensor-core attention kernels.
 #include <math.h>
 
 #include "../../include/b200asr.h"

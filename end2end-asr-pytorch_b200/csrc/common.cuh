@@ -1,4 +1,4 @@
-// Shared device/host helpers for libb200asr (sm_100a only).
+// Shared device/host helpers for libb200asr (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -22,7 +22,16 @@ int device_sm_count();
 // reference's nn.DataParallel drives several devices from one process.  `done` is the caller's per-kernel flag array.
 constexpr int kMaxDevices = 64;
 int ensure_dynamic_smem(const void* kernel, int bytes, bool (&done)[kMaxDevices], const char* what);
-int ensure_sm100();                   // B200ASR_OK iff current device is compute capability 10.x
+int ensure_sm90();                    // B200ASR_OK iff current device is compute capability 9.0
+
+// Fixed-order reductions.  Where many CTAs contribute to the same outputs they write partial results to separate slots and
+// reduce_parts() sums the slots in a fixed order: floating-point atomics would make the rounding of every such sum -- and
+// so the whole training step -- change from run to run.  stream_scratch() is the library's own device buffer for those
+// partials, one per (device, stream), valid for work enqueued on `st`; a larger request reallocates it (cudaFree
+// synchronises the device, so that happens during the first steps only).  nullptr (with the error set) on failure.
+void* stream_scratch(size_t bytes, cudaStream_t st);
+// out[i] = (accumulate ? out[i] : 0) + sum over z = 0 .. parts-1 of part[z * stride + i], for i < n
+int reduce_parts(const float* part, int parts, long long stride, long long n, float* out, int accumulate, cudaStream_t st);
 
 #define B200_REQUIRE(cond, code, ...)            \
   do {                                           \
@@ -34,7 +43,7 @@ int ensure_sm100();                   // B200ASR_OK iff current device is comput
 
 // Programmatic dependent launch.  A kernel launched through launch_pdl() may begin while its predecessor in the stream is
 // still draining (the predecessor calls griddep_launch() early; the hardware starts the dependent grid once every CTA of the
-// predecessor has done so or exited): its prologue -- barrier init, TMEM allocation, descriptor prefetch -- and the launch
+// predecessor has done so or exited): its prologue -- barrier init, descriptor prefetch -- and the launch
 // latency then overlap the predecessor's tail.  Contract: EVERY kernel launched this way executes griddep_wait() before its
 // first global-memory access; griddep_wait() returns when the predecessor grid has completed and its writes are visible, so
 // ordering stays transitive along the stream.  Kernels launched the ordinary way are unaffected (both instructions are no-ops

@@ -59,9 +59,9 @@ __global__ void __launch_bounds__(256) conv3x3_c1_fwd_kernel(const float* __rest
 }
 
 // dw[Co][9] += sum_p dy[p][co] * x[p + tap]; dbias[co] += sum_p dy[p][co]; same tiling, grid-stride over tiles
+// part[block][10 * Co]: this block's [9 * Co] weight-gradient sums (co * 9 + tap) followed by its [Co] bias sums
 __global__ void __launch_bounds__(256) conv3x3_c1_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy,
-                                                               float* __restrict__ dw, float* __restrict__ dbias, int B,
-                                                               int F, int T, int Co) {
+                                                               float* __restrict__ part, int B, int F, int T, int Co) {
   extern __shared__ float red[];   // [slots][Co*10] (also reused for nothing else)
   __shared__ float patch[C1_TF + 2][C1_TT + 2 + 1];
   const int cqs = Co >> 2;
@@ -127,8 +127,7 @@ __global__ void __launch_bounds__(256) conv3x3_c1_wgrad_kernel(const float* __re
     float s = 0.f;
     for (int sl = 0; sl < slots; sl++) s += red[(size_t)sl * Co * 10 + i];
     int co = i / 10, k = i % 10;
-    if (k < 9) atomicAdd(dw + co * 9 + k, s);
-    else atomicAdd(dbias + co, s);
+    part[(size_t)blockIdx.x * Co * 10 + (k < 9 ? co * 9 + k : 9 * Co + co)] = s;
   }
 }
 
@@ -147,7 +146,7 @@ __global__ void conv_repack_kernel(const float* __restrict__ w, float* __restric
     wr[i] = w[((size_t)co * Ci + ci) * 9 + (8 - tap)];
   }
 }
-// K-major repacks for the tcgen05 path (contraction channel contiguous):
+// K-major repacks for the tensor-core path (contraction channel contiguous):
 // fwd:   wk[tap][co][ci] = w[co][ci][tap]
 // dgrad: wk[tap'][ci][co] = w[co][ci][8 - tap']
 // split != 0 additionally writes the 3xTF32 halves: wk[i] = rna_tf32(w), wk[total + i] = rna_tf32(w - hi)
@@ -445,7 +444,7 @@ __global__ void maxpool2x2_fwd_kernel(const float* __restrict__ x, float* __rest
 
 // one thread = one 2x2 window x 4 channels; writes all four dx positions (and zeroes are written for the odd tails
 // by the tail kernel below).  ATen scans the window freq-major (h = freq outer, w = time inner) and keeps the first max.
-// fp32 value -> (bf16 hi, bf16 lo) with hi + lo ~ x to 16 significant bits (the operand split of the kind::f16 kernels)
+// fp32 value -> (bf16 hi, bf16 lo) with hi + lo ~ x to 16 significant bits (the operand split of the bf16 kernels)
 __device__ __forceinline__ void pair_of(float x, uint16_t& h, uint16_t& l) {
   const uint32_t r = __float_as_uint(x) + 0x8000u;
   h = (uint16_t)(r >> 16);
@@ -627,19 +626,25 @@ int b200asr_conv3x3_c1_bwd_weight(const float* x, const float* dy, float* dw, fl
   B200_REQUIRE(x && dy && dw && dbias, B200ASR_BAD_ARG, "conv3x3_c1_bwd_weight: null pointer");
   B200_REQUIRE(Co % 4 == 0 && 256 % (Co / 4) == 0, B200ASR_BAD_SHAPE, "conv3x3_c1_bwd_weight: Co=%d unsupported", Co);
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(dw, 0, sizeof(float) * 9 * (size_t)Co, st);
-  cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)Co, st);
   long long P = (long long)B * T * F;
-  if (P <= 0) return B200ASR_OK;
+  if (P <= 0) {
+    cudaMemsetAsync(dw, 0, sizeof(float) * 9 * (size_t)Co, st);
+    cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)Co, st);
+    return B200ASR_OK;
+  }
   int slots = 256 / (Co / 4);
   size_t smem = sizeof(float) * (size_t)slots * Co * 10;
   B200_REQUIRE(smem <= 44 * 1024, B200ASR_BAD_SHAPE, "conv3x3_c1_bwd_weight: Co=%d too large", Co);
   int blocks = device_sm_count() * 4;
-  conv3x3_c1_wgrad_kernel<<<blocks, 256, smem, st>>>(x, dy, dw, dbias, B, F, T, Co);
-  return check_launch("conv3x3_c1_wgrad");
+  float* part = (float*)stream_scratch(sizeof(float) * (size_t)blocks * 10 * Co, st);
+  if (!part) return B200ASR_CUDA_ERROR;
+  conv3x3_c1_wgrad_kernel<<<blocks, 256, smem, st>>>(x, dy, part, B, F, T, Co);
+  int rc = check_launch("conv3x3_c1_wgrad");
+  if (rc || (rc = reduce_parts(part, blocks, 10LL * Co, 9LL * Co, dw, 0, st))) return rc;
+  return reduce_parts(part + 9 * Co, blocks, 10LL * Co, Co, dbias, 0, st);
 }
 
-// bf16 variant of conv_repack_k_kernel for the kind::f16 modes: wk16[i] = bf16(w), and (terms == 2) wk16[total + i] =
+// bf16 variant of conv_repack_k_kernel for the bf16 modes: wk16[i] = bf16(w), and (terms == 2) wk16[total + i] =
 // bf16(w - hi); same K-major [tap][n][c] order (fwd) / flipped taps (dgrad)
 __global__ void conv_repack_k_bf16_kernel(const float* __restrict__ w, uint16_t* __restrict__ wk, int Ci, int Co, int dgrad, int terms) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -139,7 +139,7 @@ struct BnIdx {
 };
 
 // Grid = (BN_SPLITS x C): the B*H rows of a channel are cut into BN_SPLITS contiguous ranges, one block each (32 channels
-// alone would leave 116 of the 148 SMs idle).  Pass 1 writes one partial per block -- (count, mean, M2) of its range, each
+// alone would leave all but 32 SMs idle).  Pass 1 writes one partial per block -- (count, mean, M2) of its range, each
 // from a two-pass sum inside the block; pass 2 merges the partials of its channel (Chan et al.'s pairwise update, fixed
 // order => deterministic), and applies.  ws: [C][BN_SPLITS][4] floats.
 constexpr int BN_SPLITS = 32;

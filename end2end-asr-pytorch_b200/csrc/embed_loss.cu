@@ -70,27 +70,40 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ tokens, const float
   }
 }
 
+// One block per row; the FIRST row holding a token adds, in row order, the gradients of every row holding it into that
+// token's table row -- no atomics, so a token that occurs many times gets the same sum in every run.
 __global__ void embed_bwd_kernel(const int64_t* __restrict__ tokens, const float* __restrict__ dout,
                                  float* __restrict__ dtable, int rows, int d, int V, float scale, uint32_t thresh,
                                  float inv_keep, uint64_t key, int pad_idx) {
-  int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  int64_t tok = tokens[row];
+  const int row = blockIdx.x;
+  const int64_t tok = tokens[row];
   if (tok == pad_idx || tok < 0 || tok >= V) return;
-  float* g = dtable + (size_t)tok * d;
-  const size_t base = (size_t)row * d;
-  for (int c = lane * 4; c < d; c += 128) {
-    float4 a = *reinterpret_cast<const float4*>(dout + base + c);
-    float k0 = scale, k1 = scale, k2 = scale, k3 = scale;
-    if (thresh) {
-      uint64_t r = dropout_bits4(key, (base + c) >> 2);
-      k0 = ((uint32_t)(r) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
-      k1 = ((uint32_t)(r >> 16) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
-      k2 = ((uint32_t)(r >> 32) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
-      k3 = ((uint32_t)(r >> 48) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
+  __shared__ int earlier;
+  if (threadIdx.x == 0) earlier = 0;
+  __syncthreads();
+  for (int j = threadIdx.x; j < row; j += blockDim.x)
+    if (tokens[j] == tok) earlier = 1;
+  __syncthreads();
+  if (earlier) return;
+  for (int c = threadIdx.x * 4; c < d; c += blockDim.x * 4) {
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j = row; j < rows; j++) {
+      if (__ldg(tokens + j) != tok) continue;
+      const size_t base = (size_t)j * d;
+      const float4 a = *reinterpret_cast<const float4*>(dout + base + c);
+      float k0 = scale, k1 = scale, k2 = scale, k3 = scale;
+      if (thresh) {
+        uint64_t r = dropout_bits4(key, (base + c) >> 2);
+        k0 = ((uint32_t)(r) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
+        k1 = ((uint32_t)(r >> 16) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
+        k2 = ((uint32_t)(r >> 32) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
+        k3 = ((uint32_t)(r >> 48) & 0xFFFFu) >= thresh ? scale * inv_keep : 0.f;
+      }
+      s.x += a.x * k0; s.y += a.y * k1; s.z += a.z * k2; s.w += a.w * k3;
     }
-    atomicAdd(g + c + 0, a.x * k0); atomicAdd(g + c + 1, a.y * k1);
-    atomicAdd(g + c + 2, a.z * k2); atomicAdd(g + c + 3, a.w * k3);
+    float4* g = reinterpret_cast<float4*>(dtable + (size_t)tok * d + c);
+    const float4 o = *g;
+    *g = make_float4(o.x + s.x, o.y + s.y, o.z + s.z, o.w + s.w);
   }
 }
 
@@ -145,7 +158,7 @@ constexpr int CE_THREADS = 256;
 
 __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restrict__ logits,
                                                             const int64_t* __restrict__ gold, float* __restrict__ row_lse,
-                                                            float* __restrict__ stats, int rows, int V, float eps) {
+                                                            float* __restrict__ part, int rows, int V, float eps) {
   __shared__ float sv[CE_THREADS / 32];
   __shared__ int si[CE_THREADS / 32];
   __shared__ float ss[CE_THREADS / 32];
@@ -188,6 +201,8 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restr
     const float lse = mx + logf(t);
     row_lse[row] = lse;
     const int64_t g = gold[row];
+    float* pr = part + (size_t)row * 3;            // (loss, 1, correct) of this row; zeros for PAD rows
+    pr[0] = pr[1] = pr[2] = 0.f;
     if (g != TOK_PAD) {
       const float xg = x[g];
       float loss;
@@ -198,9 +213,9 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restr
       } else {
         loss = lse - xg;
       }
-      atomicAdd(stats + 0, loss);
-      atomicAdd(stats + 1, 1.f);
-      if ((int64_t)amax == g) atomicAdd(stats + 2, 1.f);
+      pr[0] = loss;
+      pr[1] = 1.f;
+      pr[2] = (int64_t)amax == g ? 1.f : 0.f;
     }
   }
 }
@@ -253,7 +268,8 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
   p[i] -= (lr / bc1) * mi / denom;
 }
 
-__global__ void sumsq_kernel(const float* __restrict__ g, long long n, float* __restrict__ out) {
+// part[block] = the block's sum of squares (reduce_parts adds the blocks in order)
+__global__ void sumsq_kernel(const float* __restrict__ g, long long n, float* __restrict__ part) {
   __shared__ float red[8];
   float s = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -266,7 +282,7 @@ __global__ void sumsq_kernel(const float* __restrict__ g, long long n, float* __
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += red[w];
-    atomicAdd(out, t);
+    part[blockIdx.x] = t;
   }
 }
 
@@ -335,7 +351,7 @@ int b200asr_embed_bwd(const int64_t* tokens, const float* dout, float* dtable, i
   B200_REQUIRE(tokens && dout && dtable, B200ASR_BAD_ARG, "embed_bwd: null pointer");
   B200_REQUIRE(d % 4 == 0, B200ASR_BAD_SHAPE, "embed_bwd: d=%d", d);
   if (rows <= 0) return B200ASR_OK;
-  embed_bwd_kernel<<<ceil_div(rows, 8), 256, 0, (cudaStream_t)stream>>>(tokens, dout, dtable, rows, d, V, scale,
+  embed_bwd_kernel<<<rows, 128, 0, (cudaStream_t)stream>>>(tokens, dout, dtable, rows, d, V, scale,
                                                                         p_drop > 0.f ? dropout_thresh16(p_drop) : 0u,
                                                                         dropout_inv_keep(p_drop), dropout_key(seed, offset), pad_idx);
   return check_launch("embed_bwd");
@@ -360,10 +376,15 @@ int b200asr_ce_fwd(const float* logits, const int64_t* gold, float* row_lse, flo
                    b200asr_stream_t stream) {
   B200_REQUIRE(logits && gold && row_lse && stats && V > 0, B200ASR_BAD_ARG, "ce_fwd: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(stats, 0, 3 * sizeof(float), st);
-  if (rows <= 0) return B200ASR_OK;
-  ce_fwd_kernel<<<rows, CE_THREADS, 0, st>>>(logits, gold, row_lse, stats, rows, V, smoothing);
-  return check_launch("ce_fwd");
+  if (rows <= 0) {
+    cudaMemsetAsync(stats, 0, 3 * sizeof(float), st);
+    return B200ASR_OK;
+  }
+  float* part = (float*)stream_scratch(sizeof(float) * 3 * (size_t)rows, st);
+  if (!part) return B200ASR_CUDA_ERROR;
+  ce_fwd_kernel<<<rows, CE_THREADS, 0, st>>>(logits, gold, row_lse, part, rows, V, smoothing);
+  int rc = check_launch("ce_fwd");
+  return rc ? rc : reduce_parts(part, rows, 3, 3, stats, 0, st);
 }
 
 int b200asr_ce_finalize(float* stats, float* loss_out, int mean, b200asr_stream_t stream) {
@@ -396,8 +417,13 @@ int b200asr_sumsq(const float* g, long long n, float* out, b200asr_stream_t stre
   if (n <= 0) return B200ASR_OK;
   long long blocks = ceil_div_ll(n, 256 * 8);
   int cap = device_sm_count() * 8;
-  sumsq_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(g, n, out);
-  return check_launch("sumsq");
+  const int nb = (int)(blocks < cap ? blocks : cap);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* part = (float*)stream_scratch(sizeof(float) * nb, st);
+  if (!part) return B200ASR_CUDA_ERROR;
+  sumsq_kernel<<<nb, 256, 0, st>>>(g, n, part);
+  int rc = check_launch("sumsq");
+  return rc ? rc : reduce_parts(part, nb, 1, 1, out, 1, st);
 }
 
 int b200asr_grad_scale(const float* g, long long n, const float* n_tokens, float max_norm, float* scratch, float* out,

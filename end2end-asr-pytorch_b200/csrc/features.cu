@@ -6,7 +6,7 @@
 // The STFT is a GEMM: frame t of an utterance is the n_fft samples starting at t*hop of its reflect-padded signal, so with
 // every padded signal placed at a multiple of `hop` in one buffer ALL frames of the batch are the rows of one matrix with
 // row stride hop (rows overlap; TMA only needs a 16-byte-multiple stride), multiplied by the windowed DFT basis
-// [2*(n_fft/2+1) x n_fft] (cos rows, then -sin rows).  It runs on the 3xTF32 tcgen05 GEMM of the training path (or the
+// [2*(n_fft/2+1) x n_fft] (cos rows, then -sin rows).  It runs on the 3xTF32 tensor-core GEMM of the training path (or the
 // fp32 CUDA-core GEMM), then two bandwidth-bound kernels do |.|, log1p, the statistics and the transposed, zero-padded
 // store.  Rows that straddle two utterances are computed and ignored.
 #include <math.h>

@@ -1,6 +1,6 @@
 // fp32 CUDA-core GEMM (precision 0): 128x128x16 tiles, 8x8 register micro-tiles, double-buffered smem,
 // 128-bit coalesced global loads on whichever axis is contiguous.  C[m,n] = sum_k A(m,k) * B(k,n).
-// This is the exact-fp32 path and the on-device cross-check for the tcgen05 kernels.
+// This is the exact-fp32 path and the on-device cross-check for the tensor-core kernels.
 #include "../../include/b200asr.h"
 #include "common.cuh"
 #include "kernels.h"
@@ -153,8 +153,8 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmP p) {
   }
 }
 
-// column sums: out[n] (+)= sum_m X[m, n]
-__global__ void colsum_kernel(const float* __restrict__ X, float* __restrict__ out, int M, int N, int rows_per_cta) {
+// column sums: part[row slice][n] = sum over the slice's rows of X[m, n] (reduce_parts adds the slices in order)
+__global__ void colsum_kernel(const float* __restrict__ X, float* __restrict__ part, int M, int N, int rows_per_cta) {
   __shared__ float red[8][33];
   int c = blockIdx.x * 32 + (threadIdx.x & 31);
   int rl = threadIdx.x >> 5;
@@ -168,17 +168,23 @@ __global__ void colsum_kernel(const float* __restrict__ X, float* __restrict__ o
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; i++) t += red[i][threadIdx.x & 31];
-    atomicAdd(out + c, t);
+    part[(size_t)blockIdx.y * N + c] = t;
   }
 }
 
 int launch_colsum(const float* X, float* out, int M, int N, int accumulate, cudaStream_t st) {
-  if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * (size_t)N, st);
-  // enough CTAs to hide the load latency of a skinny reduction (51 of these run per step); atomics per column = M / rows
+  if (M <= 0) {
+    if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * (size_t)N, st);
+    return B200ASR_OK;
+  }
+  // enough CTAs to hide the load latency of a skinny reduction; one partial row per slice of rows
   int rows_per_cta = M >= (1 << 20) ? 2048 : 128;
   dim3 grid(ceil_div(N, 32), ceil_div(M, rows_per_cta));
-  colsum_kernel<<<grid, 256, 0, st>>>(X, out, M, N, rows_per_cta);
-  return check_launch("colsum");
+  float* part = (float*)stream_scratch(sizeof(float) * (size_t)grid.y * N, st);
+  if (!part) return B200ASR_CUDA_ERROR;
+  colsum_kernel<<<grid, 256, 0, st>>>(X, part, M, N, rows_per_cta);
+  int rc = check_launch("colsum");
+  return rc ? rc : reduce_parts(part, (int)grid.y, N, N, out, accumulate, st);
 }
 
 // Generic entry: C[M,N] = A(m,k) B(k,n) with per-operand major flags.

@@ -10,7 +10,7 @@ int gemm_simt(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj,
               cudaStream_t st);
 int launch_colsum(const float* X, float* out, int M, int N, int accumulate, cudaStream_t st);
 
-// tcgen05 GEMM (tc_gemm.cu).  nsplit = 1 (TF32) or 3 (3xTF32).  Returns B200ASR_BAD_SHAPE when the
+// Tensor-core GEMM (tc_gemm.cu).  nsplit = 1 (TF32) or 3 (3xTF32).  Returns B200ASR_BAD_SHAPE when the
 // shape/alignment cannot be expressed as TMA tiles (callers turn that into an error, never a fallback).
 int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, int ldb, float* C, int ldc, int M,
             int N, int K, const float* bias, int relu, const float* relu_mask, int accumulate, int nsplit,
@@ -22,7 +22,7 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
 bool gemm_tc_fuses_rowsum(bool a_kmaj, bool b_kmaj, int nsplit);
 // b_split: B operand pre-split as [2][b_rows][ldb] (hi | lo), 3xTF32 only -- the kernel then skips its own B split.
 
-// Batched tcgen05 GEMM (tc_bgemm.cu): C_z[M,N] = alpha * A_z B_z for z = (batch, head), operands addressed in place.
+// Batched tensor-core GEMM (tc_bgemm.cu): C_z[M,N] = alpha * A_z B_z for z = (batch, head), operands addressed in place.
 // An operand is a logical [rows x cols] matrix per z, contiguous along cols; element (b, h, r, c) lives at
 // p + b*bs + h*hs + r*rs + c when heads != 0, and at p + z*bs + r*rs + c (z = b*H + h) when heads == 0.
 // K-major use: cols = contraction; MN-major use: rows = contraction.
@@ -30,7 +30,7 @@ struct BOperand { const float* p; long long bs, hs, rs; int heads, rows, cols; }
 int bgemm_tc(const BOperand& A, bool a_kmaj, const BOperand& B, bool b_kmaj, float* C, long long c_bs, long long c_hs, int ldc,
              int M, int N, int K, int Bsz, int H, float alpha, int nsplit, cudaStream_t st);
 
-// tcgen05 implicit-GEMM convolution (tc_conv.cu); takes K-major repacked weights wk[9][Cout][Cin]
+// Tensor-core implicit-GEMM convolution (tc_conv.cu); takes K-major repacked weights wk[9][Cout][Cin]
 // (conv_repack_k_kernel); the weight-gradient variant takes/produces dwr[9][Ci][Co].
 int conv3x3_tc(const float* in, const float* wr, const float* bias, const float* mask, float* out, int B, int T, int F,
                int Cin, int Cout, int relu, int precision, cudaStream_t st);

@@ -165,11 +165,11 @@ add_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ z, con
 }
 
 // dgamma/dbeta = column sums of the per-CTA partials: grid (d/32, row slices); 32 columns x 8 row lanes per CTA, smem tree,
-// one atomicAdd per column and slice into the zeroed outputs (a single-slice version was latency-bound: 16 CTAs walking
-// 1600 partial rows took longer than the main kernel)
+// one sum per column and slice into `slices` [LN_FIN_SLICES][2d], which reduce_parts adds up in slice order (a single-slice
+// version was latency-bound: 16 CTAs walking 1600 partial rows took longer than the main kernel)
 constexpr int LN_FIN_SLICES = 16;
 __global__ void __launch_bounds__(256) ln_bwd_finalize_kernel(const float* __restrict__ partial, int nblk, int d,
-                                                              float* __restrict__ dgamma, float* __restrict__ dbeta) {
+                                                              float* __restrict__ slices) {
   __shared__ float ra[8][33], rb[8][33];
   griddep_launch();      // programmatic dependent launch (common.cuh)
   griddep_wait();
@@ -189,8 +189,8 @@ __global__ void __launch_bounds__(256) ln_bwd_finalize_kernel(const float* __res
     float sa = 0.f, sb = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; i++) { sa += ra[i][cl]; sb += rb[i][cl]; }
-    atomicAdd(dgamma + c, sa);
-    atomicAdd(dbeta + c, sb);
+    slices[(size_t)blockIdx.y * 2 * d + c] = sa;
+    slices[(size_t)blockIdx.y * 2 * d + d + c] = sb;
   }
 }
 
@@ -248,12 +248,12 @@ int b200asr_add_ln_bwd(const float* dy, const float* z, const float* gamma, cons
 #undef LN_BWD
   int rc = check_launch("add_ln_bwd");
   if (rc) return rc;
-  if (!accumulate) {          // the finalize kernel adds its slices atomically: into zeros, or into the existing gradients
-    cudaMemsetAsync(dgamma, 0, sizeof(float) * d, st);
-    cudaMemsetAsync(dbeta, 0, sizeof(float) * d, st);
-  }
-  launch_pdl(ln_bwd_finalize_kernel, dim3(ceil_div(d, 32), LN_FIN_SLICES), dim3(256), 0, st, (const float*)partial_ws, nblk, d, dgamma, dbeta);
-  return check_launch("ln_bwd_finalize");
+  float* slices = (float*)stream_scratch(sizeof(float) * 2 * (size_t)d * LN_FIN_SLICES, st);
+  if (!slices) return B200ASR_CUDA_ERROR;
+  launch_pdl(ln_bwd_finalize_kernel, dim3(ceil_div(d, 32), LN_FIN_SLICES), dim3(256), 0, st, (const float*)partial_ws, nblk, d, slices);
+  if ((rc = check_launch("ln_bwd_finalize"))) return rc;
+  if ((rc = reduce_parts(slices, LN_FIN_SLICES, 2LL * d, d, dgamma, accumulate, st))) return rc;
+  return reduce_parts(slices + d, LN_FIN_SLICES, 2LL * d, d, dbeta, accumulate, st);
 }
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-// Batched tcgen05 GEMM on the persistent engine: C_z[M,N] = alpha * sum_k A_z(m,k) B_z(k,n) for z = (batch, head).
+// Batched tensor-core GEMM on the persistent engine: C_z[M,N] = alpha * sum_k A_z(m,k) B_z(k,n) for z = (batch, head).
 //
 // This is the contraction engine of the "materialised" attention path (attention_mat.cu): Q K^T, P V and the four
 // backward products are small per-head GEMMs (T x T x d), and at 3xTF32 the tensor cores run them ~10x faster than the
@@ -53,12 +53,6 @@ struct BGemmPolicy {
 #pragma unroll
       for (int c = 0; c < BN / 32; c++) tma_load_4d(sb + c * 4096, mapB, bar, t.n0 + 32 * c, t.bh, k0, t.bb);
   }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) {
-    return A_MN ? make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B) : make_smem_desc(s + ks * 32, 16, 1024);
-  }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) {
-    return B_MN ? make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B) : make_smem_desc(s + ks * 32, 16, 1024);
-  }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const int row = t.m0 + r;
     if (row >= p.M) return;
@@ -79,7 +73,7 @@ static int make_operand_map(CUtensorMap* map, const BOperand& x, bool kmaj, int 
   uint64_t dims[4] = {(uint64_t)x.cols, (uint64_t)(x.heads ? H : 1), (uint64_t)x.rows, (uint64_t)(x.heads ? Bsz : Bsz * H)};
   uint64_t strides[3] = {(uint64_t)(x.heads ? x.hs : x.rs), (uint64_t)x.rs, (uint64_t)x.bs};
   uint32_t box[4] = {32u, 1u, kmaj ? (uint32_t)mn_box : 32u, 1u};
-  return make_tensor_map_f32(map, x.p, 4, dims, strides, box, !kmaj, tf32_dtype);
+  return make_tensor_map_f32(map, x.p, 4, dims, strides, box, tf32_dtype);
 }
 
 template <bool A_MN, bool B_MN, int BN, int NSPLIT>

@@ -1,7 +1,7 @@
-// sm_100a building blocks shared by the tcgen05 kernels: mbarrier, TMA (cp.async.bulk.tensor), TMEM allocation,
-// tcgen05.mma / commit / ld wrappers, UMMA shared-memory + instruction descriptors, host-side tensor-map encoding.
-// Bit layouts follow the PTX ISA "tcgen05 matrix descriptors" tables (same fields CUTLASS names in
-// cute/arch/mma_sm100_desc.hpp); everything here is written from those tables, not copied.
+// sm_90a building blocks shared by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with
+// the A operand in registers and B described in shared memory), Hopper shared-memory matrix descriptors, operand splits,
+// host-side tensor-map encoding.  Bit layouts follow the PTX ISA "asynchronous warpgroup level matrix shared memory layout"
+// tables; everything here is written from those tables.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -18,6 +18,7 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// generic-proxy writes to shared memory (threads) made visible to the async proxy (wgmma operand reads, TMA writes)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -50,6 +51,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// named barrier over `count` threads (a multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
@@ -73,230 +78,100 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 
-// one 16-byte reduction instead of four scalar ones (sm_90+): split-K partial tiles are added with a quarter of the L2 atomic operations
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-// TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {    // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// one lane of a CONVERGED warp (elect.sync); the issuing warps stay convergent and predicate only the tcgen05 / TMA
-// instructions on it, so their operands live in uniform registers (inside an `if (lane == 0)` region the compiler wraps
-// every UTCHMMA / UTMALDG in an ELECT + BRA.U.ANY loop, ~10 extra dependent instructions per MMA on the critical thread)
+// one lane of a CONVERGED warp (elect.sync): the issuing warp stays convergent and predicates only the TMA instructions on it
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], fp32 operands consumed as TF32, fp32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp receives TMEM lane (base_lane + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]),
-        "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-// 32 lanes x 32 columns store (registers -> TMEM), used to stage the A operand of P*V in TMEM
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-      "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-      "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-      "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-      "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// 3xTF32 operand split, in place: hi <- x rounded to TF32 (nearest, ties away -- the same value cvt.rna.tf32.f32 gives,
-// but computed with two integer ops on the ALU pipe: the cvt instruction issues at a fraction of the rate and made the
-// split warps the bottleneck of the mainloop, see profiles/), lo <- x - hi (exact in fp32, |lo| <= 2^-12 |x|; the tensor
-// core truncates it to TF32, an error of <= 2^-22 |x|).  Elementwise, hence independent of the (swizzled) tile layout.
+// ---------------------------------------------------------------------------------------------- operand splits
+// 3xTF32 operand split: hi <- x rounded to TF32 (nearest, ties away -- the same value cvt.rna.tf32.f32 gives, computed with
+// two integer ops on the ALU pipe), lo <- x - hi (exact in fp32, |lo| <= 2^-12 |x|; the tensor core truncates it to TF32,
+// an error of <= 2^-22 |x|).
 __device__ __forceinline__ float tf32_rn(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
-__device__ __forceinline__ void split_tf32_inplace(float4* __restrict__ hi, float4* __restrict__ lo, int n_f4, int t, int nthreads) {
-#pragma unroll 4
-  for (int idx = t; idx < n_f4; idx += nthreads) {
-    const float4 x = hi[idx];
-    float4 h, l;
-    h.x = tf32_rn(x.x); l.x = x.x - h.x;
-    h.y = tf32_rn(x.y); l.y = x.y - h.y;
-    h.z = tf32_rn(x.z); l.z = x.z - h.z;
-    h.w = tf32_rn(x.w); l.w = x.w - h.w;
-    hi[idx] = h;
-    lo[idx] = l;
-  }
-}
 
-// 32 lanes x 16 columns store (registers -> TMEM)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem] (A: lane = row, one 32-bit column per k element)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------- bf16 operands (kind::f16)
 // 2-term bf16 split ("bf16x3"): x ~ hi + lo with hi = bf16(x), lo = bf16(x - hi) -- 16 significant bits, |x - hi - lo| <=
-// 2^-18 |x| -- and hi*hi + hi*lo + lo*hi per product: three kind::f16 MMAs at TWICE the tf32 rate with half the operand
-// bytes in shared memory.  Error per product ~2^-17 (dropped lo*lo and the representation error), i.e. ~100x below
-// single-pass TF32 and ~30x above 3xTF32.  Rounding is done with integer adds on the ALU pipe (round to nearest, ties away),
-// like the tf32 split: bf16(x) = top 16 bits of (bits(x) + 0x8000).
+// 2^-18 |x| -- and hi*hi + hi*lo + lo*hi per product: three bf16 MMAs at TWICE the tf32 rate.  Error per product ~2^-17
+// (dropped lo*lo and the representation error), i.e. ~100x below single-pass TF32 and ~30x above 3xTF32.
 // pack2(a, b): 32-bit word with bf16(a) in the low half (element k) and bf16(b) in the high half (element k + 1) -- the
-// order in which a TMEM column holds two consecutive-k elements of a 16-bit A operand.
-#ifndef B200ASR_SPLIT_F2FP
-#define B200ASR_SPLIT_F2FP 1
-#endif
+// order in which an MMA register fragment holds two consecutive-k elements of a 16-bit operand.
 __device__ __forceinline__ uint32_t cvt_bf16x2(float lo_elem, float hi_elem) {     // one F2FP: {hi_elem, lo_elem} -> packed bf16x2 (RN)
   uint32_t d;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi_elem), "f"(lo_elem));
   return d;
 }
 __device__ __forceinline__ void split_bf16_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-#if B200ASR_SPLIT_F2FP
   hi = cvt_bf16x2(x0, x1);
   lo = cvt_bf16x2(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
-  return;
-#endif
-  const uint32_t r0 = __float_as_uint(x0) + 0x8000u, r1 = __float_as_uint(x1) + 0x8000u;
-  hi = __byte_perm(r0, r1, 0x7632);
-  const float l0 = x0 - __uint_as_float(r0 & 0xFFFF0000u), l1 = x1 - __uint_as_float(r1 & 0xFFFF0000u);
-  lo = __byte_perm(__float_as_uint(l0) + 0x8000u, __float_as_uint(l1) + 0x8000u, 0x7632);
 }
 __device__ __forceinline__ uint32_t pack_bf16_pair(float x0, float x1) {
   return __byte_perm(__float_as_uint(x0) + 0x8000u, __float_as_uint(x1) + 0x8000u, 0x7632);
 }
-// 32 lanes x 16 columns store of raw 32-bit words (registers -> TMEM)
-__device__ __forceinline__ void tmem_st16u(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-      "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem], bf16 operands (A: lane = row, one 32-bit column per TWO k elements), fp32 accumulate
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 operands
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 
-// ---------------------------------------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor, SWIZZLE_128B.  Fields (bits): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-// version=1 [46,48), base_offset [49,52) = 0 (tiles are 1024-byte aligned), layout [61,64) = 2 (128B swizzle).
-//   K-major  tile (rows x 32 fp32, row = 128 B):  8-row groups 1024 B apart  -> SBO = 1024, LBO unused (=16)
-//   MN-major fp32/tf32 tile: the only legal layout is "128B swizzle, 32-byte atoms" (layout type 1; TMA mode
-//   CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): 128 B (32 fp32) contiguous along MN per k-line, swizzle period 4 k-lines
-//   (512 B).  Chunks of 32 MN-elements are LBO apart, groups of 4 k-lines SBO = 512 B apart.
-//   K-major bf16 tile with 64-byte rows (32 bf16; the 32-deep k-block of the bf16 modes): SWIZZLE_64B (layout type 4), 8-row
-//   groups 512 B apart -> SBO = 512; a k-step (16 bf16 = 32 B) advances the start address by 32 B, as in the tf32 tiles.
-constexpr uint32_t kLayoutSW128 = 2, kLayoutSW128Base32B = 1, kLayoutSW64 = 4;
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type = 2, uint32_t base_offset = 0) {
+// ---------------------------------------------------------------------------------------------- wgmma
+// Every B operand the kernels hand to wgmma is K-major (contraction contiguous) in one of two canonical swizzled layouts:
+//   * 128-byte rows (32 fp32 / tf32 k-values), SWIZZLE_128B: 16-byte chunk c of row r stored at chunk c ^ (r & 7), 8-row
+//     groups 1024 B apart (SBO = 1024); a k-step of 8 tf32 advances the start address by 32 B;
+//   * 64-byte rows (32 bf16 k-values), SWIZZLE_64B: chunk c of row r stored at c ^ ((r >> 1) & 3), 8-row groups 512 B apart
+//     (SBO = 512); a k-step of 16 bf16 advances the start address by 32 B.
+// Tiles start on 1024-byte boundaries, so the descriptor's base offset is 0; LBO is unused by swizzled K-major layouts.
+// The A operand always comes from registers: the kernels read the fp32 tile from shared memory, round or split it, and build
+// the fragment (for tf32 k8: a0 = (row g, k q), a1 = (row g + 8, k q), a2 = (g, q + 4), a3 = (g + 8, q + 4) with g = lane / 4,
+// q = lane % 4, rows relative to 16 * (warp % 4); for bf16 k16 the pairs (k 2q, 2q + 1) and (k 8 + 2q, 9 + 2q)).
+// Accumulator fragment (m64nN, f32): d[4j + {0,1}] = (row g, col 8j + 2q + {0,1}), d[4j + {2,3}] = (row g + 8, same cols).
+constexpr uint32_t kLayoutSW128 = 1, kLayoutSW64 = 2;
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
   uint64_t d = 0;
-  d |= (uint64_t)(base_offset & 7u) << 49;   // swizzle phase of the first row when the start is not 1024-byte aligned
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
+  d |= (uint64_t)1 << 16;                                    // LBO (unused for swizzled K-major layouts)
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)layout_type << 62;
   return d;
 }
-// Instruction descriptor for kind::tf32 with fp32 accumulation.
-//   c_format=F32 (1) [4,6); a_format=TF32 (2) [7,10); b_format=TF32 (2) [10,13); a_major [15]; b_major [16] (1 = MN-major);
-//   N>>3 [17,23); M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ uint64_t kmajor_desc_tf32(uint32_t saddr) { return make_smem_desc(saddr, 1024, kLayoutSW128); }
+__device__ __forceinline__ uint64_t kmajor_desc_bf16(uint32_t saddr) { return make_smem_desc(saddr, 512, kLayoutSW64); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// accumulator registers must not be touched by other code between a wgmma and the wait that retires it
+template <int N> __device__ __forceinline__ void acc_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Instruction descriptor for kind::f16 with BF16 operands (a_format = b_format = 1) and fp32 accumulation; K = 16 per MMA.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// D[64 x N] += A[64 x k] (registers) * B[k x N] (shared memory, K-major), fp32 accumulate; k = 8 (tf32) or 16 (bf16).
+// The operand lists: N / 2 accumulator registers, the four A registers, the B descriptor, scale-d = scale-a = scale-b = 1
+// (and, for bf16, B not transposed).
+#define WG_R32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1"
+#define WG_R64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1"
+#define WG_R128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, 1, 1, 1"
+#define WG_O4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define WG_O16(i) WG_O4(i), WG_O4(i + 4), WG_O4(i + 8), WG_O4(i + 12)
+#define WG_IN "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
+#define WG_MMA(N, ...)                                                                                                            \
+  if constexpr (BF16) asm volatile("wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 " WG_R##N ", 0;" : __VA_ARGS__ : WG_IN); \
+  else asm volatile("wgmma.mma_async.sync.aligned.m64n" #N "k8.f32.tf32.tf32 " WG_R##N ";" : __VA_ARGS__ : WG_IN)
+template <int N, bool BF16> __device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc) {
+  static_assert(N == 32 || N == 64 || N == 128, "wgmma N");
+  if constexpr (N == 32) { WG_MMA(32, WG_O16(0)); }
+  else if constexpr (N == 64) { WG_MMA(64, WG_O16(0), WG_O16(16)); }
+  else { WG_MMA(128, WG_O16(0), WG_O16(16), WG_O16(32), WG_O16(48)); }
 }
+template <int N> __device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b) { wgmma_rs<N, false>(d, a, b); }
+template <int N> __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b) { wgmma_rs<N, true>(d, a, b); }
 
 // ---------------------------------------------------------------------------------------------- host: tensor maps
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn get_encode_tiled();
-// fp32 tensor, `rank` dims (innermost first), strides in ELEMENTS for dims 1..rank-1 (dim 0 is contiguous), 128B swizzle,
-// out-of-bounds elements read as zero.  tf32_dtype selects CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 (the copy engine converts
-// fp32 -> tf32 in flight) instead of FLOAT32.  Returns 0 on success.
+// fp32 tensor, `rank` dims (innermost first), strides in ELEMENTS for dims 1..rank-1 (dim 0 is contiguous), box[0] = 32
+// (128-byte rows, SWIZZLE_128B), out-of-bounds elements read as zero.  tf32_dtype selects CU_TENSOR_MAP_DATA_TYPE_TFLOAT32
+// (the copy engine rounds fp32 -> tf32 to nearest in flight) instead of FLOAT32.  Returns 0 on success.
 int make_tensor_map_f32(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                        const uint32_t* box, bool atom32b = false, bool tf32_dtype = false);
+                        const uint32_t* box, bool tf32_dtype = false);
 
 // bf16 tensor (2 bytes / element), `rank` dims, strides in ELEMENTS; box[0] * 2 bytes = 64 -> SWIZZLE_64B, = 128 -> SWIZZLE_128B.
 int make_tensor_map_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,

@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM 3x3 convolution on channels-last [B,T,F,C] activations: forward / data gradient and weight
+// Tensor-core implicit-GEMM 3x3 convolution on channels-last [B,T,F,C] activations: forward / data gradient and weight
 // gradient, as policies of the persistent tile engine (tc_engine.cuh).
 //
 //   out[p][n] = act( sum_{tap} sum_c in[p + off(tap)][c] * wk[tap][n][c] + bias[n] ) (.* mask > 0)
@@ -6,7 +6,7 @@
 // One tile = an 8 (time) x 16 (freq) patch = 128 output pixels x BN output channels.  The A operand of k-block
 // (tap, 32-channel slice) is ONE 4-D TMA box {32 ch, 16 freq, 8 time, 1 utt} fetched at the tap-shifted coordinate:
 // the zero padding of the convolution is TMA's out-of-bounds fill, so there is no im2col buffer and no halo logic.
-// The box lands in shared memory as 128 rows x 128 B (K-major, 128B swizzle) -- exactly the UMMA canonical tile.
+// The box lands in shared memory as 128 rows x 128 B (K-major, 128B swizzle).
 // The B operand is the repacked weight wk[tap][n][c] (K-major, one 2-D box), pre-split into hi | lo for 3xTF32.
 //
 // Weight gradient:  dwr[tap][ci][co] += sum_p x[p + off(tap)][ci] * dy[p][co]
@@ -15,13 +15,9 @@
 // of 32 pixels; the A tile is four 32-channel chunks {32 ch, 16, 2, 1} fetched at the tap-shifted coordinate (zero fill
 // = padding), the B tile Co/32 chunks of dy at the unshifted coordinate.  M = 128 rows: one tap when Cin = 128, a PAIR of
 // taps when Cin = 64 (rows 0-63 tap a, 64-127 tap b; they share the dy tile).  Each tile reduces a contiguous range of
-// pixel blocks and adds its 128 x Co partial into dwr with fp32 atomics (dwr is zeroed by the caller).  The bias gradient
-// (column sums of dy over all pixels) is accumulated by the split warps of the tap-group-0 tiles while the dy tile is in
-// shared memory (3xTF32 only), instead of a separate pass that re-reads dy from HBM.
-//
-// (An earlier non-persistent kernel pair and a "halo" variant -- one 18 x 16 patch fetch shared by the nine taps through
-// shifted UMMA descriptor views, base_offset 0 -- were measured and removed: the engine policies below supersede the
-// former, and the latter gained only ~8% because the 3xTF32 mainloop is bound by shared-memory bandwidth on the B side.)
+// pixel blocks (its split) and writes its 128 x Co partial to the split's slot; reduce_parts sums the splits in order.  The
+// bias gradient (column sums of dy over all pixels) is taken by the tap-group-0 tiles while the dy tile is in shared memory,
+// instead of a separate pass that re-reads dy from HBM, and summed over the splits the same way.
 #include <stdlib.h>
 
 #include "../../include/b200asr.h"
@@ -45,8 +41,8 @@ struct ConvEpi {
 };
 
 struct WgP {
-  float* dwr;
-  float* dbias;        // [Co] accumulated (caller zeroes), or nullptr
+  float* part;         // [splits][9][Ci][Co] partial weight gradients
+  float* bpart;        // [splits][Co] partial bias gradients, or nullptr
   int B, T, F, Ci, Co, nft, ntt, blocks_per_cta, total_blocks;
 };
 
@@ -82,8 +78,6 @@ struct ConvPolicy {
       if (++t.dt == 2) { t.dt = -1; t.df++; }
     }
   }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const ConvEpi& e = p.e;
     const int tt = t.t0 + r / CT_F, ff = t.f0 + r % CT_F;
@@ -119,12 +113,6 @@ struct WgradPolicy {
   static constexpr int BN = BN_, kABytes = 4 * 4096, kBBytes = (BN_ / 32) * 4096;
   static constexpr bool kSplitA = true, kSplitB = true, kAMN = true, kBMN = true;
   static constexpr bool kSumA = false, kSumB = true;       // bias gradient = column sums of the dy tiles
-#ifndef WGRAD_CAT
-#define WGRAD_CAT 0
-#endif
-  // Co = 64: [hi*hi | hi*lo] as one N = 128 MMA (tc_engine.cuh).  Measured at cfg2's conv1_2: 1.91 ms with, 1.76 ms without --
-  // the wider accumulator leaves 4 instead of 6 stages of A in tensor memory, which costs more than the N = 64 MMAs do.
-  static constexpr bool kCat = WGRAD_CAT != 0;
   static constexpr int kGroups = CI == 64 ? 5 : 9;
   struct Params { WgP e; int splits; };
   static __device__ __forceinline__ int num_tiles(const Params& p) { return kGroups * p.splits; }
@@ -136,10 +124,11 @@ struct WgradPolicy {
     tap_a = (tile % kGroups) * (128 / CI);
     tap_b = (CI == 64 && tap_a + 1 < 9) ? tap_a + 1 : tap_a;
   }
-  struct Tile { int tap_a, tap_b, ft, tt, b, nkb; };     // tap pair + pixel-block cursor (ft fastest, then tt, then b)
+  struct Tile { int tap_a, tap_b, z, ft, tt, b, nkb; };  // tap pair, split + pixel-block cursor (ft fastest, then tt, then b)
   static __device__ __forceinline__ Tile tile(const Params& p, int tile) {
     Tile t;
     taps(tile, t.tap_a, t.tap_b);
+    t.z = tile / kGroups;
     const int blk = (tile / kGroups) * p.e.blocks_per_cta;
     t.ft = blk % p.e.nft; t.tt = (blk / p.e.nft) % p.e.ntt; t.b = blk / (p.e.nft * p.e.ntt);
     t.nkb = num_kb(p, tile);
@@ -163,22 +152,14 @@ struct WgradPolicy {
     }
   }
   // every pixel block is visited once by the tap-group-0 tiles (over all splits)
-  static __device__ __forceinline__ bool want_sums(const Params& p, const Tile& t) { return p.e.dbias != nullptr && t.tap_a == 0 && t.nkb > 0; }
-  static __device__ __forceinline__ void sum_b_store(const Params& p, const Tile&, int col, const float4& v) {
-    atomicAdd(p.e.dbias + col, v.x); atomicAdd(p.e.dbias + col + 1, v.y);
-    atomicAdd(p.e.dbias + col + 2, v.z); atomicAdd(p.e.dbias + col + 3, v.w);
-  }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B); }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B); }
-  // bf16 modes: the dy tile converted by the split warps into bf16 MN-major 64-column chunks (tc_engine.cuh)
-  static __device__ __forceinline__ uint64_t b_desc16(uint32_t s, int ks) { return make_smem_desc(s + ks * 2048, 4096, 1024, kLayoutSW128); }
+  static __device__ __forceinline__ bool want_sums(const Params& p, const Tile& t) { return p.e.bpart != nullptr && t.tap_a == 0; }
+  static __device__ __forceinline__ void sum_b_store1(const Params& p, const Tile& t, int col, float v) { p.e.bpart[(size_t)t.z * p.e.Co + col] = v; }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const int slot = r / CI, ci = r % CI;
     if (slot == 1 && t.tap_b == t.tap_a) return;
-    if (t.nkb == 0) return;
-    float* orow = p.e.dwr + ((size_t)(slot == 0 ? t.tap_a : t.tap_b) * p.e.Ci + ci) * p.e.Co + c0;
+    float* orow = p.e.part + (((size_t)t.z * 9 + (slot == 0 ? t.tap_a : t.tap_b)) * p.e.Ci + ci) * p.e.Co + c0;
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) red_add_v4(orow + j, v[j], v[j + 1], v[j + 2], v[j + 3]);     // dwr: 16-byte aligned rows of Co floats
+    for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(orow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
   }
 };
 
@@ -212,7 +193,6 @@ struct WgradPairPolicy : WgradPolicy<CI, BN_> {
       if (++t.tt == p.e.ntt) { t.tt = 0; t.b++; }
     }
   }
-  static __device__ __forceinline__ void sum_b_store1(const Params& p, const Tile&, int col, float v) { atomicAdd(p.e.dbias + col, v); }
 };
 
 template <int BN, int NSPLIT>
@@ -223,26 +203,18 @@ static int launch_conv_persistent(const CUtensorMap& ma, const CUtensorMap& mb, 
   return launch_engine<ConvPolicy<BN, NSPLIT>, NSPLIT>(ma, mb, p, (int)tiles, st, "tc_conv3x3");
 }
 
-template <int CI, int BN, int NSPLIT>
-static int launch_wgrad_persistent(const CUtensorMap& mx, const CUtensorMap& mdy, WgP e, cudaStream_t st) {
-  using Pol = WgradPolicy<CI, BN>;
-  const int sms = device_sm_count();
-  int splits = max(1, (2 * sms) / Pol::kGroups);
-  e.blocks_per_cta = max(64, ceil_div(e.total_blocks, splits));
-  splits = ceil_div(e.total_blocks, e.blocks_per_cta);
-  typename Pol::Params p{e, splits};
-  return launch_engine<Pol, NSPLIT>(mx, mdy, p, Pol::kGroups * splits, st, "tc_conv3x3_wgrad");
+// pixel blocks per split and number of splits: about two tiles per SM over the tap groups, at least 64 blocks per tile
+static int wgrad_splits(int Ci, int total_blocks, int& blocks_per_cta) {
+  const int groups = Ci == 64 ? 5 : 9;
+  const int splits = max(1, (2 * device_sm_count()) / groups);
+  blocks_per_cta = max(64, ceil_div(total_blocks, splits));
+  return ceil_div(total_blocks, blocks_per_cta);
 }
 
-template <int CI, int BN, int NSPLIT>
-static int launch_wgrad_pairs(const CUtensorMap& mx, const CUtensorMap& mdy, WgP e, cudaStream_t st) {
-  using Pol = WgradPairPolicy<CI, BN>;
-  const int sms = device_sm_count();
-  int splits = max(1, (2 * sms) / Pol::kGroups);
-  e.blocks_per_cta = max(64, ceil_div(e.total_blocks, splits));
-  splits = ceil_div(e.total_blocks, e.blocks_per_cta);
+template <int CI, int BN, int NSPLIT, class Pol = WgradPolicy<CI, BN>>
+static int launch_wgrad(const CUtensorMap& mx, const CUtensorMap& mdy, const WgP& e, int splits, cudaStream_t st) {
   typename Pol::Params p{e, splits};
-  return launch_engine<Pol, NSPLIT>(mx, mdy, p, Pol::kGroups * splits, st, "tc_conv3x3_wgrad_pairs");
+  return launch_engine<Pol, NSPLIT>(mx, mdy, p, Pol::kGroups * splits, st, "tc_conv3x3_wgrad");
 }
 
 }  // namespace tc
@@ -266,14 +238,14 @@ int conv3x3_tc(const float* in, const float* wk, const float* bias, const float*
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Cin, (uint64_t)F * Cin, (uint64_t)T * F * Cin};
     uint32_t box[4] = {32, CT_F, CT_T, 1};
-    int rc = make_tensor_map_f32(&ma, in, 4, dims, strides, box, false, precision == 1);
+    int rc = make_tensor_map_f32(&ma, in, 4, dims, strides, box, precision == 1);
     if (rc) return rc;
   }
   {
     uint64_t dims[2] = {(uint64_t)Cin, (uint64_t)(precision == 3 ? 18 : 9) * Cout};     // [hi | lo] halves for 3xTF32
     uint64_t strides[1] = {(uint64_t)Cin};
     uint32_t box[2] = {32, (uint32_t)Cout};
-    int rc = make_tensor_map_f32(&mb, wk, 2, dims, strides, box, false, precision == 1);
+    int rc = make_tensor_map_f32(&mb, wk, 2, dims, strides, box, precision == 1);
     if (rc) return rc;
   }
   ConvEpi e{out, bias, mask, relu, B, T, F, Cin, Cout};
@@ -287,79 +259,59 @@ int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, 
                      cudaStream_t st, float* dbias, int* dbias_done, const void* dy16) {
   using namespace tc;
   if (dbias_done) *dbias_done = 0;
-  if (dy16 && (precision == 6 || precision == 2)) {
-    // dy as bf16 pairs [2][B,T,F,Co] written by its producer: B tiles by TMA, no conversion in the kernel
-    B200_REQUIRE((Ci == 64 || Ci == 128) && (Co == 64 || Co == 128), B200ASR_BAD_SHAPE, "conv3x3_wgrad_tc: needs Ci, Co in {64,128} (Ci=%d Co=%d)", Ci, Co);
-    B200_REQUIRE(aligned16(x) && aligned16(dy16) && aligned16(dwr), B200ASR_BAD_ALIGN, "conv3x3_wgrad_tc: alignment");
-    CUtensorMap mx, mdy;
-    {
-      uint64_t dims[4] = {(uint64_t)Ci, (uint64_t)F, (uint64_t)T, (uint64_t)B};
-      uint64_t strides[3] = {(uint64_t)Ci, (uint64_t)F * Ci, (uint64_t)T * F * Ci};
-      uint32_t box[4] = {32, WG_PF, WG_PT, 1};
-      if (int rc = make_tensor_map_f32(&mx, x, 4, dims, strides, box, true, false)) return rc;
-    }
-    {
-      uint64_t dims[4] = {(uint64_t)Co, (uint64_t)F, (uint64_t)T, (uint64_t)2 * B};
-      uint64_t strides[3] = {(uint64_t)Co, (uint64_t)F * Co, (uint64_t)T * F * Co};
-      uint32_t box[4] = {64, WG_PF, WG_PT, 1};
-      if (int rc = make_tensor_map_bf16(&mdy, dy16, 4, dims, strides, box)) return rc;
-    }
-    if (dbias) {
-      cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)Co, st);
-      if (dbias_done) *dbias_done = 1;
-    }
-    WgP e{dwr, dbias, B, T, F, Ci, Co, ceil_div(F, WG_PF), ceil_div(T, WG_PT), 0, 0};
-    const long long total = (long long)B * e.nft * e.ntt;
-    B200_REQUIRE(total < (1LL << 31), B200ASR_BAD_SHAPE, "conv3x3_wgrad_tc: too many pixel blocks");
-    e.total_blocks = (int)total;
-#define WGPP(CIv, BNv) return precision == 6 ? launch_wgrad_pairs<CIv, BNv, 6>(mx, mdy, e, st) : launch_wgrad_pairs<CIv, BNv, 2>(mx, mdy, e, st)
-    if (Ci == 64 && Co == 64) WGPP(64, 64);
-    if (Ci == 64 && Co == 128) WGPP(64, 128);
-    if (Ci == 128 && Co == 64) WGPP(128, 64);
-    WGPP(128, 128);
-#undef WGPP
-  }
+  // dy as bf16 pairs [2][B,T,F,Co] written by its producer (bf16 modes): B tiles by TMA, no conversion in the kernel
+  const bool pairs = dy16 && (precision == 6 || precision == 2);
   B200_REQUIRE(precision == 1 || precision == 3 || precision == 2 || precision == 6, B200ASR_BAD_ARG, "conv3x3_wgrad_tc: precision must be 1, 3 (tf32) or 2, 6 (bf16)");
   B200_REQUIRE((Ci == 64 || Ci == 128) && (Co == 64 || Co == 128), B200ASR_BAD_SHAPE,
                "conv3x3_wgrad_tc: needs Ci, Co in {64,128} (Ci=%d Co=%d)", Ci, Co);
-  B200_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dwr), B200ASR_BAD_ALIGN, "conv3x3_wgrad_tc: alignment");
+  B200_REQUIRE(aligned16(x) && aligned16(pairs ? dy16 : (const void*)dy) && aligned16(dwr), B200ASR_BAD_ALIGN, "conv3x3_wgrad_tc: alignment");
   CUtensorMap mx, mdy;
   const bool tf32 = precision == 1;
   {
     uint64_t dims[4] = {(uint64_t)Ci, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Ci, (uint64_t)F * Ci, (uint64_t)T * F * Ci};
     uint32_t box[4] = {32, WG_PF, WG_PT, 1};
-    int rc = make_tensor_map_f32(&mx, x, 4, dims, strides, box, true, tf32);
-    if (rc) return rc;
+    if (int rc = make_tensor_map_f32(&mx, x, 4, dims, strides, box, tf32 && !pairs)) return rc;
   }
-  {
+  if (pairs) {
+    uint64_t dims[4] = {(uint64_t)Co, (uint64_t)F, (uint64_t)T, (uint64_t)2 * B};
+    uint64_t strides[3] = {(uint64_t)Co, (uint64_t)F * Co, (uint64_t)T * F * Co};
+    uint32_t box[4] = {64, WG_PF, WG_PT, 1};
+    if (int rc = make_tensor_map_bf16(&mdy, dy16, 4, dims, strides, box)) return rc;
+  } else {
     uint64_t dims[4] = {(uint64_t)Co, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Co, (uint64_t)F * Co, (uint64_t)T * F * Co};
     uint32_t box[4] = {32, WG_PF, WG_PT, 1};
-    int rc = make_tensor_map_f32(&mdy, dy, 4, dims, strides, box, true, tf32);
-    if (rc) return rc;
+    if (int rc = make_tensor_map_f32(&mdy, dy, 4, dims, strides, box, tf32)) return rc;
   }
-  const bool fuse_bias = dbias != nullptr && precision != 1;
-  if (fuse_bias) {
-    cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)Co, st);
-    if (dbias_done) *dbias_done = 1;
-  }
-  WgP e{dwr, fuse_bias ? dbias : nullptr, B, T, F, Ci, Co, ceil_div(F, WG_PF), ceil_div(T, WG_PT), 0, 0};
+  const bool fuse_bias = dbias != nullptr && (pairs || precision != 1);
+  WgP e{nullptr, nullptr, B, T, F, Ci, Co, ceil_div(F, WG_PF), ceil_div(T, WG_PT), 0, 0};
   const long long total = (long long)B * e.nft * e.ntt;
   B200_REQUIRE(total < (1LL << 31), B200ASR_BAD_SHAPE, "conv3x3_wgrad_tc: too many pixel blocks");
   e.total_blocks = (int)total;
-#define WGP(CIv, BNv)                                                                     \
-  switch (precision) {                                                                    \
-    case 1: return launch_wgrad_persistent<CIv, BNv, 1>(mx, mdy, e, st);                  \
-    case 3: return launch_wgrad_persistent<CIv, BNv, 3>(mx, mdy, e, st);                  \
-    case 6: return launch_wgrad_persistent<CIv, BNv, 6>(mx, mdy, e, st);                  \
-    default: return launch_wgrad_persistent<CIv, BNv, 2>(mx, mdy, e, st);                 \
-  }
-  if (Ci == 64 && Co == 64) WGP(64, 64);
-  if (Ci == 64 && Co == 128) WGP(64, 128);
-  if (Ci == 128 && Co == 64) WGP(128, 64);
-  WGP(128, 128);
+  const int splits = wgrad_splits(Ci, e.total_blocks, e.blocks_per_cta);
+  const long long wn = 9LL * Ci * Co;
+  e.part = (float*)stream_scratch(sizeof(float) * (size_t)splits * (wn + (fuse_bias ? Co : 0)), st);
+  if (!e.part) return B200ASR_CUDA_ERROR;
+  e.bpart = fuse_bias ? e.part + (size_t)splits * wn : nullptr;
+  int rc;
+#define WGP(CIv, BNv)                                                                                                  \
+  if (pairs) rc = precision == 6 ? launch_wgrad<CIv, BNv, 6, WgradPairPolicy<CIv, BNv>>(mx, mdy, e, splits, st)        \
+                                 : launch_wgrad<CIv, BNv, 2, WgradPairPolicy<CIv, BNv>>(mx, mdy, e, splits, st);       \
+  else if (precision == 1) rc = launch_wgrad<CIv, BNv, 1>(mx, mdy, e, splits, st);                                     \
+  else if (precision == 3) rc = launch_wgrad<CIv, BNv, 3>(mx, mdy, e, splits, st);                                     \
+  else if (precision == 6) rc = launch_wgrad<CIv, BNv, 6>(mx, mdy, e, splits, st);                                     \
+  else rc = launch_wgrad<CIv, BNv, 2>(mx, mdy, e, splits, st);
+  if (Ci == 64 && Co == 64) { WGP(64, 64) }
+  else if (Ci == 64 && Co == 128) { WGP(64, 128) }
+  else if (Ci == 128 && Co == 64) { WGP(128, 64) }
+  else { WGP(128, 128) }
 #undef WGP
+  if (rc) return rc;
+  if ((rc = reduce_parts(e.part, splits, wn, wn, dwr, 0, st))) return rc;
+  if (!fuse_bias) return B200ASR_OK;
+  if (dbias_done) *dbias_done = 1;
+  return reduce_parts(e.bpart, splits, Co, Co, dbias, 0, st);
 }
 
 }  // namespace b200asr

@@ -1,26 +1,23 @@
-// 3x3 convolution (forward / data gradient), 3xTF32, "halo" variant of the persistent tcgen05 kernel.
+// 3x3 convolution (forward / data gradient), "halo" variant of the persistent wgmma kernel: 3xTF32, bf16x3 or bf16.
 //
-// Why: ncu on the tap-shifted implicit GEMM (tc_conv.cu) shows l1tex__m_xbar2l1tex_read_bytes (TMA) at 12.3 TB/s = the
-// chip-wide L2 throughput cap (~6300 B/clk, B300_MICROARCH.md): that kernel fetches the activation tile nine times per
-// 32-channel slice (once per tap, 16 KB each).  (Measured effect of removing that traffic alone: small -- the kernel is
-// not bound by one resource; what moved it was requesting the first-touch patch a slice ahead and the N = 128 MMA for
-// Cout = 64, see DESIGN.md section 4.1.)  Here the 16 x 8 output tile's input
-// patch INCLUDING its one-pixel halo -- 18 x 10 pixels x 32 channels = 22.5 KB -- is fetched ONCE per slice, and the nine
-// taps are nine shifted row mappings of that patch: 6.4x less activation traffic (weights are unchanged).
+// Why: the tap-shifted implicit GEMM (tc_conv.cu) fetches the activation tile nine times per 32-channel slice (once per tap,
+// 16 KB each).  Here the 16 x 8 output tile's input patch INCLUDING its one-pixel halo -- 18 x 10 pixels x 32 channels =
+// 22.5 KB -- is fetched ONCE per slice, and the nine taps are nine shifted row mappings of that patch: 6.4x less activation
+// traffic (weights are unchanged).
 //
-// This is possible because with 3xTF32 the A operand never reaches the tensor core from shared memory: the split warps
-// read the fp32 patch, form hi = rn_tf32(x) and lo = x - hi in registers and store them to TENSOR MEMORY (tcgen05.st);
-// the MMAs are TS-form (A from TMEM, B = pre-split weights from smem).  So the patch needs no UMMA-legal layout -- a
-// thread simply reads patch row (tt + dt) * 10 + (ff + df) for its output pixel (tt, ff) and tap (dt, df).
+// This is possible because the A operand never reaches the tensor core from shared memory: the consumer threads read the
+// fp32 patch, round / split it in registers and issue register-A wgmma (tc_engine.cuh, mma_kblock).  So the patch needs no
+// MMA-legal layout -- a thread simply reads patch row (tt + dt) * 10 + (ff + df) for its output pixel (tt, ff) and tap (dt, df).
 //
-// Roles (448 threads, 1 CTA / SM, persistent over tiles): warp 0 TMA (patch ring of 3, one slice ahead; weight ring of S),
-// warp 1 MMA issue + TMEM owner, warps 2-5 epilogue (double-buffered accumulators), warps 6-13 split (two groups on alternating taps).
+// Roles (384 threads, 1 CTA / SM, persistent over tiles): warp 0 TMA (patch ring of 3, one slice ahead; weight ring of S),
+// warpgroups 1 and 2 consumers (output pixels 0-63 / 64-127 of the tile: MMAs, then the epilogue).
 #include <stdlib.h>
 
 #include "../../include/b200asr.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "tc_common.cuh"
+#include "tc_engine.cuh"
 
 namespace b200asr {
 namespace tc {
@@ -30,10 +27,6 @@ constexpr int HPT = HT + 2, HPF = HF + 2;              // input patch incl. halo
 constexpr int HPATCH_BYTES = HPT * HPF * 128;          // 23,040 B per 32-channel slice
 constexpr int HPATCH_STAGE = (HPATCH_BYTES + 1023) / 1024 * 1024;
 constexpr int HPATCH_SLOTS = 3;                        // the patch of slice i+1 is requested before the weights of slice i
-#ifndef HALO_GROUPS_N
-#define HALO_GROUPS_N 2
-#endif
-constexpr int HALO_GROUPS = HALO_GROUPS_N, HALO_SPLIT = 128 * HALO_GROUPS, HALO_THREADS = 192 + HALO_SPLIT;
 
 struct HaloP {
   uint16_t* out16;       // optional bf16 hi | lo pairs of the output, [2][pixels][Cout] (lo at + npix * Cout), or nullptr
@@ -45,74 +38,47 @@ struct HaloP {
 };
 
 // MODE: 3 = 3xTF32 (fp32 weight tiles hi | lo, 128-byte rows), 6 = bf16x3 (bf16 weight tiles hi | lo, 64-byte rows, three
-// kind::f16 MMAs per product at twice the tf32 rate), 2 = bf16 (one bf16 weight tile, one MMA).  In the bf16 modes the split
-// warps convert the fp32 patch to bf16 and pack two channels per TMEM column.
+// bf16 MMAs per product at twice the tf32 rate), 2 = bf16 (one bf16 weight tile, one MMA).
 template <int BN, int MODE> struct HaloCfg {
   static constexpr bool kBf16 = MODE != 3;
-#ifndef HALO_CONVERT_ONCE
-#define HALO_CONVERT_ONCE 1
-#endif
-  static constexpr bool kOnce = kBf16 && HALO_CONVERT_ONCE;      // convert each patch once per slice, in place (see the split warps)
   static constexpr int kHalves = MODE == 2 ? 1 : 2;
   static constexpr int kBBytes = BN * (kBf16 ? 64 : 128);
-  static constexpr int kACols = MODE == 3 ? 64 : (MODE == 6 ? 32 : 16);        // TMEM columns of A (hi | lo) per stage
   static constexpr int kStageBytes = kHalves * kBBytes;                         // weights hi | lo of one (tap, slice)
-  // BN = 64 runs "concatenated": the tensor core is markedly less efficient at N = 64 than at N = 128 (measured: ~57% vs
-  // ~87% of the tf32 rate, whatever the rest of the kernel does), so hi*hi and hi*lo are ONE N = 128 MMA against the
-  // weight tile [B_hi ; B_lo] (adjacent in the stage, 128 K-major rows) into a 128-column accumulator, lo*hi is an N = 64
-  // MMA into its first half, and the epilogue adds the two halves.
-#ifndef HALO_CAT
-#define HALO_CAT 1
-#endif
-  static constexpr bool kCat = BN == 64 && HALO_CAT && MODE != 2;
-  static constexpr int kAccW = kCat ? 128 : BN;                                  // accumulator columns per buffer
-  static constexpr int kMaxByTmem0 = (512 - 2 * kAccW) / kACols;
-  static constexpr int kMaxByTmem = kMaxByTmem0 > 8 ? 8 : kMaxByTmem0;
-  static constexpr int kBySmem = (200 * 1024 - HPATCH_SLOTS * HPATCH_STAGE) / kStageBytes;
-  static constexpr int kRaw = kBySmem < kMaxByTmem ? kBySmem : kMaxByTmem;
-  static constexpr int kStages = kRaw - kRaw % HALO_GROUPS;                       // a stage always belongs to one split group
   static constexpr int kRingOff = HPATCH_SLOTS * HPATCH_STAGE;
-  static constexpr int kBarOff = kRingOff + kStages * kStageBytes;
-  static constexpr int kSmemBytes = kBarOff + 512 + 1024;
-  static constexpr int kAccCols = 2 * kAccW;
+  static constexpr int kBySmem = (ENG_SMEM_CAP - 1024 - kRingOff - epilogue_bytes(BN) - 256) / kStageBytes;
+  static constexpr int kStages = kBySmem > 8 ? 8 : kBySmem;
+  static constexpr int kOffEpi = kRingOff + kStages * kStageBytes;
+  static constexpr int kBarOff = kOffEpi + epilogue_bytes(BN);
+  static constexpr int kSmemBytes = kBarOff + 256 + 1024;
   static_assert(kStages >= 2, "stage too large");
+  static_assert(kSmemBytes <= ENG_SMEM_CAP, "shared memory");
 };
 
 template <int BN, int MODE>
-__global__ void __launch_bounds__(HALO_THREADS, 1)
+__global__ void __launch_bounds__(ENG_THREADS, 1)
 tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const HaloP p) {
   using Cfg = HaloCfg<BN, MODE>;
-  constexpr int S = Cfg::kStages, G = HALO_GROUPS;
+  constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen_base = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + Cfg::kBarOff;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };              // weights of stage s landed
-  auto xfm_bar = [&](int s) { return bar_base + 8u * (S + s); };         // A hi/lo of stage s are in TMEM
-  auto empty_bar = [&](int s) { return bar_base + 8u * (2 * S + s); };   // the MMAs of stage s completed
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (3 * S + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (3 * S + 2 + b); };
-  auto pfull_bar = [&](int b) { return bar_base + 8u * (3 * S + 4 + b); };
-  auto pempty_bar = [&](int b) { return bar_base + 8u * (3 * S + 4 + HPATCH_SLOTS + b); };
-  const uint32_t tmem_slot = bar_base + 8u * (3 * S + 4 + 2 * HPATCH_SLOTS);
+  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };       // the MMAs of stage s completed
+  auto pfull_bar = [&](int b) { return bar_base + 8u * (2 * S + b); };
+  auto pempty_bar = [&](int b) { return bar_base + 8u * (2 * S + HPATCH_SLOTS + b); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = p.nft * p.ntt * p.B;
-  const int nkb = 9 * p.cch;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; s++) { mbar_init(full_bar(s), 1); mbar_init(xfm_bar(s), HALO_SPLIT / G); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; b++) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), 128); }
-    for (int b = 0; b < HPATCH_SLOTS; b++) { mbar_init(pfull_bar(b), 1); mbar_init(pempty_bar(b), HALO_SPLIT); }
+    for (int s = 0; s < S; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), ENG_CONSUMERS / 32); }
+    for (int b = 0; b < HPATCH_SLOTS; b++) { mbar_init(pfull_bar(b), 1); mbar_init(pempty_bar(b), ENG_CONSUMERS / 32); }
     fence_barrier_init();
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(gen_base + (tmem_slot - smem_base));
   griddep_launch();      // programmatic dependent launch, see common.cuh
   griddep_wait();
 
@@ -125,8 +91,8 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
-    // Patches run ONE SLICE AHEAD of the weights: a patch is first-touch data from HBM (~1-2 us under load) while the split
-    // warps want it as soon as its slice starts, so it is requested a whole slice (9 k-blocks) early into a ring of three.
+    // Patches run ONE SLICE AHEAD of the weights: a patch is first-touch data from HBM while the consumers want it as soon
+    // as its slice starts, so it is requested a whole slice (9 k-blocks) early into a ring of three.
     const bool leader = elect_one();
     uint32_t s = 0, ph = 0;
     uint32_t pslot = 0, pph = 0;                     // ring position / phase of the NEXT patch to request
@@ -159,269 +125,99 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
       }
       tile = ntile; sl = nsl;
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (see tc_engine.cuh for the idioms)
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_ts = Cfg::kBf16 ? make_idesc_bf16(128, BN, false, false) : make_idesc_tf32(128, BN, false, false);
-    constexpr uint32_t idesc_cat = Cfg::kBf16 ? make_idesc_bf16(128, 128, false, false) : make_idesc_tf32(128, 128, false, false);
-    constexpr uint32_t kStageStep = Cfg::kStageBytes >> 4, kLoStep = Cfg::kBBytes >> 4;
-    const uint64_t bd0 = Cfg::kBf16 ? make_smem_desc(smem_base + Cfg::kRingOff, 16, 512, kLayoutSW64)
-                                    : make_smem_desc(smem_base + Cfg::kRingOff, 16, 1024);
-    const uint32_t bd_hi = (uint32_t)(bd0 >> 32);
-    auto mk = [](uint32_t hi, uint32_t lo) { return ((uint64_t)hi << 32) | lo; };
-    uint32_t s = 0, ph = 0, tcount = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, tcount++) {
-      const uint32_t buf = tcount & 1;
-      mbar_wait(tempty_bar(buf), ((tcount >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * Cfg::kAccW;
-      for (int kb = 0; kb < nkb; kb++) {
+    return;
+  }
+  if (warp < 4) return;
+
+  // -------------------------------------------------------------------- consumers
+  const int ctid = threadIdx.x - 128;
+  const int wg = ctid >> 7, cw = (ctid >> 5) & 3;
+  const int g = lane >> 2, q = lane & 3;
+  const int r0 = wg * 64 + cw * 16 + g, r1 = r0 + 8;             // output pixels (row / 8, row % 8) of the tile
+  const int prow0 = (r0 >> 3) * HPF + (r0 & 7), prow1 = (r1 >> 3) * HPF + (r1 & 7);   // their patch rows for tap (0, 0)
+  float* epi = reinterpret_cast<float*>(gen_base + Cfg::kOffEpi);
+  float dummy0 = 0.f, dummy1 = 0.f;
+  uint32_t s = 0, ph = 0, ps = 0, pph = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    for (int sl = 0; sl < p.cch; sl++) {
+      const uint8_t* patch = gen_base + ps * HPATCH_STAGE;
+      mbar_wait(pfull_bar(ps), pph);
+      for (int tap = 0; tap < 9; tap++) {
         mbar_wait(full_bar(s), ph);
-        mbar_wait(xfm_bar(s), ph);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t b_lo32 = (uint32_t)bd0 + s * kStageStep;
-          const uint32_t a_t = tmem_base + Cfg::kAccCols + s * Cfg::kACols;
-          if constexpr (Cfg::kBf16) {
-            // 32 channels = two 16-deep kind::f16 steps; a TMEM column holds two channels
-#pragma unroll
-            for (int ks = 0; ks < 2; ks++) {
-              const uint64_t b_hi = mk(bd_hi, b_lo32 + ks * 2), b_lo = mk(bd_hi, b_lo32 + kLoStep + ks * 2);
-              const uint32_t a_hi = a_t + ks * 8, a_lo = a_hi + 16;
-              const uint32_t acc0 = (kb | ks) != 0 ? 1u : 0u;
-              if constexpr (MODE == 2) {
-                umma_bf16_ts(d_tmem, a_hi, b_hi, idesc_ts, acc0);
-              } else if constexpr (Cfg::kCat) {
-                umma_bf16_ts(d_tmem, a_hi, b_hi, idesc_cat, acc0);                         // [hi*hi | hi*lo], 128 columns
-                umma_bf16_ts(d_tmem, a_lo, b_hi, idesc_ts, 1u);                            // + lo*hi into the first 64
-              } else {
-                umma_bf16_ts(d_tmem, a_lo, b_hi, idesc_ts, acc0);
-                umma_bf16_ts(d_tmem, a_hi, b_lo, idesc_ts, 1u);
-                umma_bf16_ts(d_tmem, a_hi, b_hi, idesc_ts, 1u);
-              }
-            }
-          } else
-#pragma unroll
-          for (int ks = 0; ks < 4; ks++) {
-            const uint64_t b_hi = mk(bd_hi, b_lo32 + ks * 2), b_lo = mk(bd_hi, b_lo32 + kLoStep + ks * 2);
-            const uint32_t a_hi = a_t + ks * 8, a_lo = a_hi + 32;
-            if (Cfg::kCat) {
-              umma_tf32_ts(d_tmem, a_hi, b_hi, idesc_cat, (kb | ks) != 0 ? 1u : 0u);   // [hi*hi | hi*lo], 128 columns
-              umma_tf32_ts(d_tmem, a_lo, b_hi, idesc_ts, 1u);                          // + lo*hi into the first 64
-            } else {
-              umma_tf32_ts(d_tmem, a_lo, b_hi, idesc_ts, (kb | ks) != 0 ? 1u : 0u);
-              umma_tf32_ts(d_tmem, a_hi, b_lo, idesc_ts, 1u);
-              umma_tf32_ts(d_tmem, a_hi, b_hi, idesc_ts, 1u);
-            }
-          }
-          umma_commit(empty_bar(s));
-        }
+        const int shift = (tap % 3) * HPF + tap / 3;                // tap = 3 * (df + 1) + (dt + 1)
+        const int pr0 = prow0 + shift, pr1 = prow1 + shift;
+        const uint32_t sb = smem_base + Cfg::kRingOff + s * Cfg::kStageBytes;
+        // A element (pixel row r, channel k): patch row pr, 128B swizzle of the TMA box
+        mma_kblock<MODE, BN, true, false>(
+            acc,
+            [&](int r, int k) {
+              const int pr = r == r0 ? pr0 : pr1;
+              return reinterpret_cast<const float*>(patch + pr * 128 + (((k >> 2) ^ (pr & 7)) << 4) + (k & 3) * 4);
+            },
+            r0, r1, q, sb, sb + Cfg::kBBytes, dummy0, dummy1);
         __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar(s));
         if (++s == S) { s = 0; ph ^= 1; }
       }
-      if (leader) umma_commit(tfull_bar(buf));
       __syncwarp();
+      if (lane == 0) mbar_arrive(pempty_bar(ps));      // this warp has read the patch for the last time
+      if (++ps == HPATCH_SLOTS) { ps = 0; pph ^= 1; }
     }
-  } else if (warp < 6) {
-    // ------------------------------------------------------------------ epilogue (warps 2-5: TMEM lane quarters 2,3,0,1)
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, tcount++) {
-      const uint32_t buf = tcount & 1;
-      int f0, t0, b;
-      decode(tile, f0, t0, b);
+
+    // ---- epilogue: bias, ReLU, mask, optional bf16 pairs and fused 2 x 2 max-pool; a warp covers 4 time rows x 8 freq bins
+    int f0, t0, b;
+    decode(tile, f0, t0, b);
+    epilogue_rows<BN>(acc, epi, ctid, r0, r1, q, [&](int r, int c0, const float (&v)[32]) {
       const int tt = t0 + (r >> 3), ff = f0 + (r & 7);
       const bool valid = tt < p.T && ff < p.F;
+      if (!valid && !p.pool) return;                  // (with pooling every lane takes part in the shuffles below)
       const size_t pix = ((size_t)b * p.T + tt) * p.F + ff;
       float* orow = p.out + pix * p.Cout;
       uint16_t* orow16 = p.out16 ? p.out16 + pix * p.Cout : nullptr;
       const size_t lo_off = (size_t)p.B * p.T * p.F * p.Cout;
       const float* mrow = p.mask ? p.mask + pix * p.Cout : nullptr;
-      mbar_wait(tfull_bar(buf), (tcount >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; c++) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * Cfg::kAccW + (uint32_t)(c * 32), v);
-        if (Cfg::kCat) {
-          float w[32];
-          tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * Cfg::kAccW + (uint32_t)(64 + c * 32), w);
 #pragma unroll
-          for (int j = 0; j < 32; j++) v[j] += w[j];
+      for (int half = 0; half < 2; half++) {     // all loads of a 16-channel half before its first store
+        float4 bb[4], mm[4];
+#pragma unroll
+        for (int qq = 0; qq < 4; qq++) {
+          const int col = c0 + half * 16 + qq * 4;
+          bb[qq] = (p.bias && valid) ? __ldg(reinterpret_cast<const float4*>(p.bias + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          mm[qq] = (mrow && valid) ? __ldg(reinterpret_cast<const float4*>(mrow + col)) : make_float4(1.f, 1.f, 1.f, 1.f);
         }
-        if (c == BN / 32 - 1) {            // all TMEM reads of this buffer are done: hand it back before the global stores
-          tc_fence_before();
-          mbar_arrive(tempty_bar(buf));
-        }
-        if (!valid && !p.pool) continue;                // (with pooling every lane takes part in the shuffles below)
 #pragma unroll
-        for (int half = 0; half < 2; half++) {     // all loads of a 16-channel half before its first store
-          float4 bb[4], mm[4];
-#pragma unroll
-          for (int q = 0; q < 4; q++) {
-            const int col = c * 32 + half * 16 + q * 4;
-            bb[q] = (p.bias && valid) ? __ldg(reinterpret_cast<const float4*>(p.bias + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            mm[q] = (mrow && valid) ? __ldg(reinterpret_cast<const float4*>(mrow + col)) : make_float4(1.f, 1.f, 1.f, 1.f);
+        for (int qq = 0; qq < 4; qq++) {
+          const int col = c0 + half * 16 + qq * 4, j = half * 16 + qq * 4;
+          float o[4] = {v[j] + bb[qq].x, v[j + 1] + bb[qq].y, v[j + 2] + bb[qq].z, v[j + 3] + bb[qq].w};
+          if (p.relu) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); o[2] = fmaxf(o[2], 0.f); o[3] = fmaxf(o[3], 0.f); }
+          o[0] = mm[qq].x > 0.f ? o[0] : 0.f; o[1] = mm[qq].y > 0.f ? o[1] : 0.f;
+          o[2] = mm[qq].z > 0.f ? o[2] : 0.f; o[3] = mm[qq].w > 0.f ? o[3] : 0.f;
+          if (valid) *reinterpret_cast<float4*>(orow + col) = make_float4(o[0], o[1], o[2], o[3]);
+          if (orow16 && valid) {       // the same values as bf16 pairs: the weight-gradient kernel's B operand (WgradPairPolicy)
+            uint2 h, l;
+            split_bf16_pair(o[0], o[1], h.x, l.x);
+            split_bf16_pair(o[2], o[3], h.y, l.y);
+            *reinterpret_cast<uint2*>(orow16 + col) = h;
+            *reinterpret_cast<uint2*>(orow16 + lo_off + col) = l;
           }
+          if (p.pool) {
+            // fused MaxPool2d(2, 2): a warp holds 4 time rows x 8 freq bins of the tile (lane = 8 * row + bin, tile origin
+            // even in both), so the 2 x 2 window of lane l is {l, l ^ 1, l ^ 8, l ^ 9}; the even / even lane stores it
 #pragma unroll
-          for (int q = 0; q < 4; q++) {
-            const int col = c * 32 + half * 16 + q * 4, j = half * 16 + q * 4;
-            float o[4] = {v[j] + bb[q].x, v[j + 1] + bb[q].y, v[j + 2] + bb[q].z, v[j + 3] + bb[q].w};
-            if (p.relu) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); o[2] = fmaxf(o[2], 0.f); o[3] = fmaxf(o[3], 0.f); }
-            o[0] = mm[q].x > 0.f ? o[0] : 0.f; o[1] = mm[q].y > 0.f ? o[1] : 0.f;
-            o[2] = mm[q].z > 0.f ? o[2] : 0.f; o[3] = mm[q].w > 0.f ? o[3] : 0.f;
-            if (valid) *reinterpret_cast<float4*>(orow + col) = make_float4(o[0], o[1], o[2], o[3]);
-            if (orow16 && valid) {       // the same values as bf16 pairs: the weight-gradient kernel's B operand (WgradPairPolicy)
-              uint2 ph, pl;
-              split_bf16_pair(o[0], o[1], ph.x, pl.x);
-              split_bf16_pair(o[2], o[3], ph.y, pl.y);
-              *reinterpret_cast<uint2*>(orow16 + col) = ph;
-              *reinterpret_cast<uint2*>(orow16 + lo_off + col) = pl;
+            for (int e = 0; e < 4; e++) {
+              o[e] = fmaxf(o[e], __shfl_xor_sync(0xffffffffu, o[e], 1));
+              o[e] = fmaxf(o[e], __shfl_xor_sync(0xffffffffu, o[e], 8));
             }
-            if (p.pool) {
-              // fused MaxPool2d(2, 2): a warp holds 4 time rows x 8 freq bins of the tile (lane = 8 * row + bin, tile origin
-              // even in both), so the 2 x 2 window of lane l is {l, l ^ 1, l ^ 8, l ^ 9}; the even / even lane stores it
-#pragma unroll
-              for (int e = 0; e < 4; e++) {
-                o[e] = fmaxf(o[e], __shfl_xor_sync(0xffffffffu, o[e], 1));
-                o[e] = fmaxf(o[e], __shfl_xor_sync(0xffffffffu, o[e], 8));
-              }
-              if ((lane & 9) == 0 && tt + 1 < p.T && ff + 1 < p.F)
-                *reinterpret_cast<float4*>(p.pool + ((((size_t)b * (p.T >> 1) + (tt >> 1)) * (p.F >> 1) + (ff >> 1)) * p.Cout + col)) =
-                    make_float4(o[0], o[1], o[2], o[3]);
-            }
+            if ((lane & 9) == 0 && tt + 1 < p.T && ff + 1 < p.F)
+              *reinterpret_cast<float4*>(p.pool + ((((size_t)b * (p.T >> 1) + (tt >> 1)) * (p.F >> 1) + (ff >> 1)) * p.Cout + col)) =
+                  make_float4(o[0], o[1], o[2], o[3]);
           }
         }
       }
-    }
-  } else {
-    // ------------------------------------------------------------------ split warps: patch (smem) -> hi / lo (TMEM)
-    const int group = (warp - 6) >> 2;               // two groups of four warps take alternating taps
-    const int quarter = warp & 3;                    // TMEM lanes this warp may touch
-    const int row = quarter * 32 + lane;             // output pixel (row / 8, row % 8) of the tile
-    const int prow0 = (row >> 3) * HPF + (row & 7);  // its patch row for tap (0, 0)
-    // Software-pipelined by one tap: the smem loads of this group's NEXT tap are issued right after the TMEM stores of the
-    // current one, so their latency (and the bank conflicts of the row-strided reads) overlaps tcgen05.wait::st and the
-    // barrier round trip instead of adding to the per-tap chain.
-    auto load_tap = [&](const uint8_t* patch, int tap, float4 (&x)[8]) {
-      const int pr = prow0 + (tap % 3) * HPF + tap / 3;     // tap = 3 * (df + 1) + (dt + 1)
-      const uint8_t* prow = patch + pr * 128;
-#pragma unroll
-      for (int j = 0; j < (Cfg::kOnce ? 4 * Cfg::kHalves : 8); j++)                                          // 128B swizzle of the TMA box
-        x[j] = *reinterpret_cast<const float4*>(prow + ((j ^ (pr & 7)) << 4));
-    };
-    // kind::f16 modes: every patch pixel is converted ONCE per slice, in place -- its 128-byte row (32 fp32 channels) becomes
-    // 16 words of packed bf16 hi (chunks 0-3) and 16 words of packed bf16 lo (chunks 4-7), same chunk swizzle -- instead of
-    // once per tap by whichever thread maps to it: 180 conversions per slice instead of 9 x 128, and a tap is then eight
-    // LDS.128 and two tcgen05.st.  (ncu on the per-tap version: the split warps were issue-bound on the conversion ALU work,
-    // tensor pipe 39 % at Cout = 64.)
-    const int ctid = threadIdx.x - 192;              // 0 .. HALO_SPLIT-1 over all split warps
-    auto convert_patch = [&](uint8_t* patch) {
-      for (int pr = ctid; pr < HPT * HPF; pr += HALO_SPLIT) {
-        uint8_t* prow = patch + pr * 128;
-        float4 v[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) v[j] = *reinterpret_cast<const float4*>(prow + ((j ^ (pr & 7)) << 4));
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          if constexpr (MODE == 6) {
-            split_bf16_pair(v[j].x, v[j].y, hi[2 * j], lo[2 * j]);
-            split_bf16_pair(v[j].z, v[j].w, hi[2 * j + 1], lo[2 * j + 1]);
-          } else {
-            hi[2 * j] = pack_bf16_pair(v[j].x, v[j].y);
-            hi[2 * j + 1] = pack_bf16_pair(v[j].z, v[j].w);
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          *reinterpret_cast<uint4*>(prow + ((j ^ (pr & 7)) << 4)) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-          if constexpr (MODE == 6)
-            *reinterpret_cast<uint4*>(prow + (((4 + j) ^ (pr & 7)) << 4)) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
-        }
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(HALO_SPLIT) : "memory");      // all split warps: the converted patch is complete
-    };
-    uint32_t kbg = 0, ps = 0, pph = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      for (int sl = 0; sl < p.cch; sl++) {
-        uint8_t* patch = gen_base + ps * HPATCH_STAGE;
-        const int first = (group + G - (int)(kbg % G)) % G;     // this group's first tap of the slice: (kbg + first) % G == group
-        mbar_wait(pfull_bar(ps), pph);                       // every group waits for every patch
-        if constexpr (Cfg::kOnce) convert_patch(patch);
-        float4 x[8];
-        load_tap(patch, first, x);
-        for (int tap = first; tap < 9; tap += G) {
-          const uint32_t k = kbg + tap;
-          const int s = k % S;
-          mbar_wait(empty_bar(s), ((k / S) & 1) ^ 1);       // the MMAs that read this TMEM slot last have completed
-          tc_fence_after();
-          const uint32_t acol = tmem_base + ((uint32_t)(quarter * 32) << 16) + Cfg::kAccCols + s * Cfg::kACols;
-          if constexpr (Cfg::kOnce) {
-            uint32_t w[16];
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-              w[4 * j] = __float_as_uint(x[j].x); w[4 * j + 1] = __float_as_uint(x[j].y);
-              w[4 * j + 2] = __float_as_uint(x[j].z); w[4 * j + 3] = __float_as_uint(x[j].w);
-            }
-            tmem_st16u(acol, w);
-            if constexpr (MODE == 6) {
-#pragma unroll
-              for (int j = 0; j < 4; j++) {
-                w[4 * j] = __float_as_uint(x[4 + j].x); w[4 * j + 1] = __float_as_uint(x[4 + j].y);
-                w[4 * j + 2] = __float_as_uint(x[4 + j].z); w[4 * j + 3] = __float_as_uint(x[4 + j].w);
-              }
-              tmem_st16u(acol + 16, w);
-            }
-          } else if constexpr (Cfg::kBf16) {
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-              const float4 v = x[j];
-              if constexpr (MODE == 6) {
-                split_bf16_pair(v.x, v.y, hi[2 * j], lo[2 * j]);
-                split_bf16_pair(v.z, v.w, hi[2 * j + 1], lo[2 * j + 1]);
-              } else {
-                hi[2 * j] = pack_bf16_pair(v.x, v.y);
-                hi[2 * j + 1] = pack_bf16_pair(v.z, v.w);
-              }
-            }
-            tmem_st16u(acol, hi);
-            if constexpr (MODE == 6) tmem_st16u(acol + 16, lo);
-          } else
-#pragma unroll
-          for (int half = 0; half < 2; half++) {            // 16 columns at a time keeps the live registers low
-            float hi[16], lo[16];
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-              const float4 v = x[half * 4 + j];
-              hi[j * 4 + 0] = tf32_rn(v.x); lo[j * 4 + 0] = v.x - hi[j * 4 + 0];
-              hi[j * 4 + 1] = tf32_rn(v.y); lo[j * 4 + 1] = v.y - hi[j * 4 + 1];
-              hi[j * 4 + 2] = tf32_rn(v.z); lo[j * 4 + 2] = v.z - hi[j * 4 + 2];
-              hi[j * 4 + 3] = tf32_rn(v.w); lo[j * 4 + 3] = v.w - hi[j * 4 + 3];
-            }
-            tmem_st16(acol + half * 16, hi);
-            tmem_st16(acol + 32 + half * 16, lo);
-          }
-          if (tap + G < 9) load_tap(patch, tap + G, x);
-          tmem_wait_st();
-          tc_fence_before();
-          mbar_arrive(xfm_bar(s));
-        }
-        kbg += 9;
-        if constexpr (Cfg::kOnce) fence_proxy_async_smem();   // our generic-proxy writes to the slot precede TMA's next write to it
-        mbar_arrive(pempty_bar(ps));                 // this thread has read the patch for the last time
-        if (++ps == HPATCH_SLOTS) { ps = 0; pph ^= 1; }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    });
   }
 }
 
@@ -435,7 +231,7 @@ static int launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const HaloP
   if (tiles <= 0) return B200ASR_OK;
   if (tiles >= (1LL << 31)) { set_error("tc_conv3x3_halo: too many tiles"); return B200ASR_BAD_SHAPE; }
   const int grid = (int)min(tiles, (long long)device_sm_count());
-  launch_pdl(kern, dim3(grid), dim3(HALO_THREADS), Cfg::kSmemBytes, st, ma, mb, p);
+  launch_pdl(kern, dim3(grid), dim3(ENG_THREADS), Cfg::kSmemBytes, st, ma, mb, p);
   return check_launch("tc_conv3x3_halo");
 }
 
@@ -456,14 +252,14 @@ int conv3x3_tc_halo(const float* in, const void* wk, const float* bias, const fl
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Cin, (uint64_t)F * Cin, (uint64_t)T * F * Cin};
     uint32_t box[4] = {32, HPF, HPT, 1};
-    int rc = make_tensor_map_f32(&ma, in, 4, dims, strides, box, false, false);
+    int rc = make_tensor_map_f32(&ma, in, 4, dims, strides, box, false);
     if (rc) return rc;
   }
   {
     uint64_t dims[2] = {(uint64_t)Cin, (uint64_t)(mode == 2 ? 9 : 18) * Cout};
     uint64_t strides[1] = {(uint64_t)Cin};
     uint32_t box[2] = {32, (uint32_t)Cout};
-    int rc = mode == 3 ? make_tensor_map_f32(&mb, wk, 2, dims, strides, box, false, false) : make_tensor_map_bf16(&mb, wk, 2, dims, strides, box);
+    int rc = mode == 3 ? make_tensor_map_f32(&mb, wk, 2, dims, strides, box, false) : make_tensor_map_bf16(&mb, wk, 2, dims, strides, box);
     if (rc) return rc;
   }
   HaloP p{(uint16_t*)out16, pool, out, bias, mask, relu, B, T, F, Cin, Cout, ceil_div(F, HF), ceil_div(T, HT), Cin / 32};

@@ -1,5 +1,5 @@
 // emb_cnn front end, second convolution (models/asr/transformer.py:37: Conv2d(32, 32, kernel (21, 11), stride (2, 1)) on the
-// NCHW activation) as IMPLICIT GEMMs on the persistent tcgen05 engine -- no im2col matrix, no col2im scatter.
+// NCHW activation) as IMPLICIT GEMMs on the persistent wgmma engine -- no im2col matrix, no col2im scatter.
 //
 // Geometry: x [B, 32, H, W], w [32, 32, KH, KW], y [B, 32, OH, OW] with OH = (H - KH) / SH + 1, OW = W - KW + 1 (stride 1
 // along W, no padding).  Because the stride along W is 1, the GEMM row index can be the output column:
@@ -7,15 +7,15 @@
 //   forward        y[b, :, oh, ow0 + m]  = sum_{kh, kw} sum_ci  x[b, ci, SH*oh + kh, ow0 + m + kw] * w[:, ci, kh, kw]
 //     one k-block = one (kh, kw): the A tile (128 m x 32 ci, MN-major) is ONE strided window of the activation -- 4 TMA
 //     boxes {32 w, 32 c} of the (w, c, h, b) view at (ow0 + kw, 0, SH*oh + kh) -- and the B tile the 32 x 32 weight slice of that tap (K-major,
-//     pre-converted: bf16 hi | lo for the kind::f16 modes, tf32 hi | lo for 3xTF32).
+//     pre-converted: bf16 hi | lo for the bf16 modes, tf32 hi | lo for 3xTF32).
 //   data gradient  dx[b, :, h, w0 + m]   = sum_{kh == h (mod SH), kw} sum_co  dy[b, co, (h - kh) / SH, w0 + m - kw] * w[co, :, kh, kw]
 //     the same kernel: a gather over the taps whose row parity matches h; boxes that reach outside dy are zero-filled by TMA.
 //   weight gradient dw[:, ci, kh, kw]    = sum_{b, oh, ow} dy[b, :, oh, ow] * x[b, ci, SH*oh + kh, ow + kw]
 //     GEMM rows = (kw, ci) -- four taps x 32 channels per 128-row tile --, columns = co, contraction = output pixels along ow:
-//     both operands K-major fp32 windows (3xTF32, B split in the kernel), partial sums added to dw with fp32 atomics.
+//     both operands K-major fp32 windows (3xTF32, B split in the kernel), one partial per row split, summed in split order.
 //
-// MMA N = 32 (the layer has 32 output channels); the engine's conversion warps turn the fp32 A tile into the tensor-memory
-// operand exactly as for the other policies.  TMA needs 16-byte row pitches, so the NCHW tensors these kernels touch are
+// MMA N = 32 (the layer has 32 output channels); the engine's consumers turn the fp32 A tile into register operands exactly
+// as for the other policies.  TMA needs 16-byte row pitches, so the NCHW tensors these kernels touch are
 // PITCHED: rows of `pitch` floats (a multiple of 4) of which the first W are valid (W = 205 / 195 at cfg3).
 //
 // TMA also needs the INNERMOST start coordinate of a box to be 16-byte aligned (UTMALDG raises an illegal-instruction
@@ -99,7 +99,7 @@ struct EmbConvPolicy {
     }
     advance(p, t);
   }
-  // kind::f16 modes: bf16 hi (| lo) weight slices (64-byte rows)
+  // bf16 modes: bf16 hi (| lo) weight slices (64-byte rows)
   static __device__ __forceinline__ void load16(const Params& p, Tile& t, const CUtensorMap* mapA, const CUtensorMap* mapB,
                                                 uint32_t sa, uint32_t sb, uint32_t sb_lo, uint32_t bar, bool leader, int halves) {
     if (leader) {
@@ -110,9 +110,6 @@ struct EmbConvPolicy {
     }
     advance(p, t);
   }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B); }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
-  static __device__ __forceinline__ uint64_t b_desc16(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 512, kLayoutSW64); }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const int w = t.w0 + r;
     if (w >= p.e.width) return;
@@ -125,7 +122,7 @@ struct EmbConvPolicy {
 };
 
 struct EmbWgP {
-  float* dw;             // [32 co, 32 ci, KH, KW], zeroed by the caller
+  float* part;           // [splits][32 co, 32 ci, KH, KW] partial weight gradients
   EmbG g;
   int m_tiles, splits, rows_per_split, owb;      // ceil(KW / 4); splits of the B*OH output rows; 32-wide ow blocks per row
 };
@@ -135,13 +132,14 @@ struct EmbWgradPolicy {
   static constexpr bool kSplitA = true, kSplitB = true, kAMN = false, kBMN = false, kSumA = false, kSumB = false;
   struct Params { EmbWgP e; };
   static __device__ __forceinline__ int num_tiles(const Params& p) { return p.e.g.KH * p.e.m_tiles * p.e.splits; }
-  struct Tile { int kh, mt, row, row_end, ob; };          // tap row, kw group, (b, oh) row cursor, ow-block cursor
+  struct Tile { int kh, mt, z, row, row_end, ob; };       // tap row, kw group, split, (b, oh) row cursor, ow-block cursor
   static __device__ __forceinline__ Tile tile(const Params& p, int tile) {
     Tile t;
     t.kh = tile % p.e.g.KH;
     const int q = tile / p.e.g.KH;
     t.mt = q % p.e.m_tiles;
     const int z = q / p.e.m_tiles;
+    t.z = z;
     t.row = z * p.e.rows_per_split;
     t.row_end = min(p.e.g.B * p.e.g.OH, t.row + p.e.rows_per_split);
     t.ob = 0;
@@ -167,15 +165,13 @@ struct EmbWgradPolicy {
     }
     if (++t.ob == p.e.owb) { t.ob = 0; t.row++; }
   }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const int kw = t.mt * 4 + r / EC, ci = r % EC;
     if (kw >= p.e.g.KW) return;
-    float* o = p.e.dw + ((size_t)ci * p.e.g.KH + t.kh) * p.e.g.KW + kw;        // + co * (32 * KH * KW)
     const size_t cs = (size_t)EC * p.e.g.KH * p.e.g.KW;
+    float* o = p.e.part + (size_t)t.z * EC * cs + ((size_t)ci * p.e.g.KH + t.kh) * p.e.g.KW + kw;        // + co * (32 * KH * KW)
 #pragma unroll
-    for (int j = 0; j < 32; j++) atomicAdd(o + (size_t)(c0 + j) * cs, v[j]);
+    for (int j = 0; j < 32; j++) o[(size_t)(c0 + j) * cs] = v[j];
   }
 };
 
@@ -243,9 +239,6 @@ struct Emb1ConvPolicy {
     }
     t.t++;
   }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B); }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
-  static __device__ __forceinline__ uint64_t b_desc16(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 512, kLayoutSW64); }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const int w = t.w0 + r;
     if (w >= p.e.g.OW) return;
@@ -259,7 +252,7 @@ struct Emb1ConvPolicy {
 // weight gradient of the first convolution: rows = (kw (4 per tile), kh in its 32-block), columns = co, contraction = output
 // pixels along ow (32 per k-block); x windows from the de-interleaved copies, dy [B, 32, OH, OW] (row pitch a multiple of 4)
 struct Emb1WgP {
-  float* dw;             // [32 co, 1, KH, KW], zeroed by the caller
+  float* part;           // [splits][32 co, 1, KH, KW] partial weight gradients
   Emb1G g;
   int m_tiles, nkblk, splits, rows_per_split, owb;
 };
@@ -269,13 +262,14 @@ struct Emb1WgradPolicy {
   static constexpr bool kSplitA = true, kSplitB = true, kAMN = false, kBMN = false, kSumA = false, kSumB = false;
   struct Params { Emb1WgP e; };
   static __device__ __forceinline__ int num_tiles(const Params& p) { return p.e.nkblk * p.e.m_tiles * p.e.splits; }
-  struct Tile { int kblk, mt, row, row_end, ob; };
+  struct Tile { int kblk, mt, z, row, row_end, ob; };
   static __device__ __forceinline__ Tile tile(const Params& p, int tile) {
     Tile t;
     t.kblk = tile % p.e.nkblk;
     const int q = tile / p.e.nkblk;
     t.mt = q % p.e.m_tiles;
     const int z = q / p.e.m_tiles;
+    t.z = z;
     t.row = z * p.e.rows_per_split;
     t.row_end = min(p.e.g.B * p.e.g.OH, t.row + p.e.rows_per_split);
     t.ob = 0;
@@ -302,15 +296,13 @@ struct Emb1WgradPolicy {
     }
     if (++t.ob == p.e.owb) { t.ob = 0; t.row++; }
   }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) { return make_smem_desc(s + ks * 32, 16, 1024); }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const int kw = t.mt * 4 + r / 32, kh = t.kblk * 32 + r % 32;
     if (kw >= p.e.g.KW || kh >= p.e.g.KH) return;
-    float* o = p.e.dw + (size_t)kh * p.e.g.KW + kw;        // + co * (KH * KW)
     const size_t cs = (size_t)p.e.g.KH * p.e.g.KW;
+    float* o = p.e.part + (size_t)t.z * EC * cs + (size_t)kh * p.e.g.KW + kw;        // + co * (KH * KW)
 #pragma unroll
-    for (int j = 0; j < 32; j++) atomicAdd(o + (size_t)(c0 + j) * cs, v[j]);
+    for (int j = 0; j < 32; j++) o[(size_t)(c0 + j) * cs] = v[j];
   }
 };
 
@@ -385,9 +377,10 @@ __global__ void emb_repack_kernel(const float* __restrict__ w, void* __restrict_
   }
 }
 
-// db[c] = sum over (b, h, w) of dy: grid (splits, 32 channels), a warp walks a row, partial sums joined by one atomic per block
-// (db zeroed by the caller; the weight gradient next to it accumulates with atomics as well)
-__global__ void emb_bias_grad_kernel(const float* __restrict__ dy, float* __restrict__ db, int B, int H, int W, int P) {
+// db[c] = sum over (b, h, w) of dy: grid (splits, 32 channels), a warp walks a row; part[split][c] = the block's sum, added
+// up in split order by reduce_parts
+constexpr int EMB_BIAS_SPLITS = 32;
+__global__ void emb_bias_grad_kernel(const float* __restrict__ dy, float* __restrict__ part, int B, int H, int W, int P) {
   __shared__ float red[8];
   const int c = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rows = B * H;
@@ -402,7 +395,7 @@ __global__ void emb_bias_grad_kernel(const float* __restrict__ dy, float* __rest
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int w = 0; w < 8; w++) t += red[w];
-    atomicAdd(db + c, t);
+    part[blockIdx.x * EC + c] = t;
   }
 }
 
@@ -438,11 +431,11 @@ static int make_shifted(const float* src, float* dst, int B, int H, int W, int P
 
 // [N, 32, H, .] (row pitch P, W valid columns) seen as the 4-D tensor (w, c, h, n): a box {32 w, 32 c, 1, 1} is one 32 x 32
 // window of a row across all channels.  For the shifted copies N = 4 * B (index s * B + b) and every column is valid.
-static int nchw_map(CUtensorMap* m, const float* base, int W, int P, int H, int N, bool atom32) {
+static int nchw_map(CUtensorMap* m, const float* base, int W, int P, int H, int N) {
   uint64_t dims[4] = {(uint64_t)W, (uint64_t)EC, (uint64_t)H, (uint64_t)N};
   uint64_t strides[3] = {(uint64_t)H * P, (uint64_t)P, (uint64_t)EC * H * P};
   uint32_t box[4] = {32, EC, 1, 1};
-  return make_tensor_map_f32(m, base, 4, dims, strides, box, atom32, false);
+  return make_tensor_map_f32(m, base, 4, dims, strides, box, false);
 }
 
 static inline int emb1_pitch(int W) { return ((W + 1) / 2 + 3 + 3) / 4 * 4; }
@@ -457,7 +450,7 @@ static int emb1_geom(Emb1G& g, const char* who, int B, int H, int W, int Co, int
 }
 
 // the de-interleaved, shifted copies and the overlapping (w, kh, oh, n) view of them
-static int emb1_prepare(CUtensorMap* m, const float* x, float* copies, const Emb1G& g, bool atom32, cudaStream_t st) {
+static int emb1_prepare(CUtensorMap* m, const float* x, float* copies, const Emb1G& g, cudaStream_t st) {
   const long long R = (long long)g.B * g.H, n = R * (g.pd / 4);
   emb1_prep_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(x, copies, R, g.W, g.pd);
   note_launch(1);
@@ -465,7 +458,7 @@ static int emb1_prepare(CUtensorMap* m, const float* x, float* copies, const Emb
   uint64_t dims[4] = {(uint64_t)g.pd, (uint64_t)g.KH, (uint64_t)g.OH, (uint64_t)8 * g.B};
   uint64_t strides[3] = {(uint64_t)g.pd, (uint64_t)2 * g.pd, (uint64_t)g.H * g.pd};
   uint32_t box[4] = {32, 32, 1, 1};
-  return make_tensor_map_f32(m, copies, 4, dims, strides, box, atom32, false);
+  return make_tensor_map_f32(m, copies, 4, dims, strides, box, false);
 }
 
 template <bool DGRAD>
@@ -515,11 +508,11 @@ int b200asr_conv2d_tc_fwd(const float* x, const float* w, const float* bias, flo
   CUtensorMap ma, mb;
   float* xs = (float*)ws + weight_floats(KH, KW);
   if (int rc = make_shifted(x, xs, B, H, W, x_pitch, st)) return rc;
-  if (int rc = nchw_map(&ma, xs, shift_pitch(W), shift_pitch(W), H, 4 * B, true)) return rc;
+  if (int rc = nchw_map(&ma, xs, shift_pitch(W), shift_pitch(W), H, 4 * B)) return rc;
   {
     uint64_t dims[2] = {(uint64_t)EC, (uint64_t)(precision == 2 ? 1 : 2) * KH * KW * EC}, strides[1] = {(uint64_t)EC};
     uint32_t box[2] = {EC, EC};
-    int rc = precision == 3 ? make_tensor_map_f32(&mb, ws, 2, dims, strides, box, false, false) : make_tensor_map_bf16(&mb, ws, 2, dims, strides, box);
+    int rc = precision == 3 ? make_tensor_map_f32(&mb, ws, 2, dims, strides, box, false) : make_tensor_map_bf16(&mb, ws, 2, dims, strides, box);
     if (rc) return rc;
   }
   EmbConvP e{y, bias, g, g.OH, g.OW, y_pitch, ceil_div(g.OW, 128), KH * KW * EC};
@@ -540,11 +533,11 @@ int b200asr_conv2d_tc_bwd_data(const float* dy, const float* w, float* dx, void*
   CUtensorMap ma, mb;
   float* dys = (float*)ws + weight_floats(KH, KW);
   if (int rc = make_shifted(dy, dys, B, g.OH, g.OW, y_pitch, st)) return rc;
-  if (int rc = nchw_map(&ma, dys, shift_pitch(g.OW), shift_pitch(g.OW), g.OH, 4 * B, true)) return rc;
+  if (int rc = nchw_map(&ma, dys, shift_pitch(g.OW), shift_pitch(g.OW), g.OH, 4 * B)) return rc;
   {
     uint64_t dims[2] = {(uint64_t)EC, (uint64_t)(precision == 2 ? 1 : 2) * KH * KW * EC}, strides[1] = {(uint64_t)EC};
     uint32_t box[2] = {EC, EC};
-    int rc = precision == 3 ? make_tensor_map_f32(&mb, ws, 2, dims, strides, box, false, false) : make_tensor_map_bf16(&mb, ws, 2, dims, strides, box);
+    int rc = precision == 3 ? make_tensor_map_f32(&mb, ws, 2, dims, strides, box, false) : make_tensor_map_bf16(&mb, ws, 2, dims, strides, box);
     if (rc) return rc;
   }
   EmbConvP e{dx, nullptr, g, H, W, x_pitch, ceil_div(W, 128), KH * KW * EC};
@@ -558,24 +551,27 @@ int b200asr_conv2d_tc_bwd_weight(const float* dy, const float* x, float* dw, flo
   if (int rc = emb_geom(g, "conv2d_tc_bwd_weight", B, Ci, H, W, Co, KH, KW, SH, x_pitch, y_pitch)) return rc;
   B200_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(ws), B200ASR_BAD_ALIGN, "conv2d_tc_bwd_weight: alignment");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)EC * EC * KH * KW, st);
   CUtensorMap mx, mdy;
   float* xs = (float*)ws + weight_floats(KH, KW);
   if (int rc = make_shifted(x, xs, B, H, W, x_pitch, st)) return rc;
-  if (int rc = nchw_map(&mx, xs, shift_pitch(W), shift_pitch(W), H, 4 * B, false)) return rc;          // K-major tiles: plain 128B swizzle
-  if (int rc = nchw_map(&mdy, dy, g.OW, y_pitch, g.OH, B, false)) return rc;
-  EmbWgP e{dw, g, ceil_div(KW, 4), 1, B * g.OH, ceil_div(g.OW, 32)};
+  if (int rc = nchw_map(&mx, xs, shift_pitch(W), shift_pitch(W), H, 4 * B)) return rc;
+  if (int rc = nchw_map(&mdy, dy, g.OW, y_pitch, g.OH, B)) return rc;
+  EmbWgP e{nullptr, g, ceil_div(KW, 4), 1, B * g.OH, ceil_div(g.OW, 32)};
   const int base = KH * e.m_tiles, rows = B * g.OH;
   int splits = max(1, (3 * device_sm_count()) / base);
   e.rows_per_split = max(8, ceil_div(rows, splits));
   e.splits = ceil_div(rows, e.rows_per_split);
+  const size_t wn = (size_t)EC * EC * KH * KW;
+  e.part = (float*)stream_scratch(sizeof(float) * ((size_t)e.splits * wn + EMB_BIAS_SPLITS * EC), st);
+  if (!e.part) return B200ASR_CUDA_ERROR;
   EmbWgradPolicy::Params p{e};
   int rc = launch_engine<EmbWgradPolicy, 3>(mx, mdy, p, base * e.splits, st, "conv2d_tc_wgrad");
-  if (rc) return rc;
+  if (rc || (rc = reduce_parts(e.part, e.splits, (long long)wn, (long long)wn, dw, 0, st))) return rc;
   if (dbias) {
-    cudaMemsetAsync(dbias, 0, sizeof(float) * EC, st);
-    emb_bias_grad_kernel<<<dim3(32, EC), 256, 0, st>>>(dy, dbias, B, g.OH, g.OW, y_pitch);
-    return check_launch("conv2d_tc_bias_grad");
+    float* bpart = e.part + (size_t)e.splits * wn;
+    emb_bias_grad_kernel<<<dim3(EMB_BIAS_SPLITS, EC), 256, 0, st>>>(dy, bpart, B, g.OH, g.OW, y_pitch);
+    if ((rc = check_launch("conv2d_tc_bias_grad"))) return rc;
+    return reduce_parts(bpart, EMB_BIAS_SPLITS, EC, EC, dbias, 0, st);
   }
   return B200ASR_OK;
 }
@@ -597,11 +593,11 @@ int b200asr_conv2d_c1_tc_fwd(const float* x, const float* w, const float* bias, 
   emb1_repack_kernel<<<ceil_div(rows * 32, 256), 256, 0, st>>>(w, ws, KH, KW, nkblk, precision);
   note_launch(1);
   CUtensorMap ma, mb;
-  if (int rc = emb1_prepare(&ma, x, (float*)ws + emb1_weight_floats(KH, KW), g, true, st)) return rc;
+  if (int rc = emb1_prepare(&ma, x, (float*)ws + emb1_weight_floats(KH, KW), g, st)) return rc;
   {
     uint64_t dims[2] = {32, (uint64_t)(precision == 2 ? 1 : 2) * rows}, strides[1] = {32};
     uint32_t box[2] = {32, EC};
-    int rc = precision == 3 ? make_tensor_map_f32(&mb, ws, 2, dims, strides, box, false, false) : make_tensor_map_bf16(&mb, ws, 2, dims, strides, box);
+    int rc = precision == 3 ? make_tensor_map_f32(&mb, ws, 2, dims, strides, box, false) : make_tensor_map_bf16(&mb, ws, 2, dims, strides, box);
     if (rc) return rc;
   }
   Emb1ConvPolicy::Params p{Emb1ConvP{y, bias, g, y_pitch, ceil_div(g.OW, 128), nkblk}};
@@ -620,22 +616,25 @@ int b200asr_conv2d_c1_tc_bwd_weight(const float* dy, const float* x, float* dw, 
   B200_REQUIRE(y_pitch >= g.OW && y_pitch % 4 == 0 && aligned16(dy) && aligned16(ws), B200ASR_BAD_ALIGN,
                "conv2d_c1_tc_bwd_weight: dy needs a 16-byte aligned base and a row pitch that is a multiple of 4 floats (TMA)");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)EC * KH * KW, st);
   CUtensorMap mx, mdy;
-  if (int rc = emb1_prepare(&mx, x, (float*)ws + emb1_weight_floats(KH, KW), g, false, st)) return rc;
-  if (int rc = nchw_map(&mdy, dy, g.OW, y_pitch, g.OH, B, false)) return rc;
-  Emb1WgP e{dw, g, ceil_div(KW, 4), ceil_div(KH, 32), 1, B * g.OH, ceil_div(g.OW, 32)};
+  if (int rc = emb1_prepare(&mx, x, (float*)ws + emb1_weight_floats(KH, KW), g, st)) return rc;
+  if (int rc = nchw_map(&mdy, dy, g.OW, y_pitch, g.OH, B)) return rc;
+  Emb1WgP e{nullptr, g, ceil_div(KW, 4), ceil_div(KH, 32), 1, B * g.OH, ceil_div(g.OW, 32)};
   const int base = e.nkblk * e.m_tiles, rows = B * g.OH;
   int splits = max(1, (3 * device_sm_count()) / base);
   e.rows_per_split = max(8, ceil_div(rows, splits));
   e.splits = ceil_div(rows, e.rows_per_split);
+  const size_t wn = (size_t)EC * KH * KW;
+  e.part = (float*)stream_scratch(sizeof(float) * ((size_t)e.splits * wn + EMB_BIAS_SPLITS * EC), st);
+  if (!e.part) return B200ASR_CUDA_ERROR;
   Emb1WgradPolicy::Params p{e};
   int rc = launch_engine<Emb1WgradPolicy, 3>(mx, mdy, p, base * e.splits, st, "conv2d_c1_tc_wgrad");
-  if (rc) return rc;
+  if (rc || (rc = reduce_parts(e.part, e.splits, (long long)wn, (long long)wn, dw, 0, st))) return rc;
   if (dbias) {
-    cudaMemsetAsync(dbias, 0, sizeof(float) * EC, st);
-    emb_bias_grad_kernel<<<dim3(32, EC), 256, 0, st>>>(dy, dbias, B, g.OH, g.OW, y_pitch);
-    return check_launch("conv2d_c1_tc_bias_grad");
+    float* bpart = e.part + (size_t)e.splits * wn;
+    emb_bias_grad_kernel<<<dim3(EMB_BIAS_SPLITS, EC), 256, 0, st>>>(dy, bpart, B, g.OH, g.OW, y_pitch);
+    if ((rc = check_launch("conv2d_c1_tc_bias_grad"))) return rc;
+    return reduce_parts(bpart, EMB_BIAS_SPLITS, EC, EC, dbias, 0, st);
   }
   return B200ASR_OK;
 }

@@ -1,12 +1,16 @@
-// Persistent tcgen05 tile engine shared by the GEMM and the implicit-GEMM convolutions.
+// Persistent wgmma tile engine shared by the GEMM and the implicit-GEMM convolutions (sm_90a).
 //
-// One CTA per SM loops over output tiles (static round-robin).  Warp roles:
-//   warp 0      TMA producer            -- runs ahead across tiles through a ring of smem stages
-//   warp 1      MMA issuer + TMEM owner -- accumulates tile i into TMEM buffer (i & 1)
-//   warps 2-5   epilogue                -- drain buffer (i & 1) with tcgen05.ld while tile i+1 is being multiplied
-//   warps 6-13  3xTF32 operand split    -- A: smem -> (hi, lo) in TMEM; B: hi in place / lo in smem (only when NSPLIT == 3);
-//               two groups of 4 warps take alternating k-blocks
-// so per-tile prologue/epilogue latency is hidden behind the next tile's mainloop instead of being paid 200+ times per SM.
+// One CTA per SM loops over 128 x BN output tiles (static round-robin).  Roles (384 threads):
+//   warp 0               TMA producer -- runs ahead across tiles through a ring of shared-memory stages
+//   warps 1-3            idle (they complete the producer warpgroup, so that the consumers are whole warpgroups)
+//   warpgroups 1 and 2   consumers, rows 0-63 and 64-127 of the tile.  Per k-block (32 deep) they
+//                          * read their rows of the raw fp32 A tile from the stage and round / split them into wgmma
+//                            register fragments (A never needs a tensor-core layout, so either major works);
+//                          * make B the K-major operand wgmma reads from shared memory when it did not arrive that way
+//                            (MN-major tiles are transposed, fp32 operands split into hi | lo or converted to bf16);
+//                          * issue the MMAs and release the stage;
+//                        after the last k-block they stage the accumulators through shared memory and hand 32-column row
+//                        pieces to Policy::store, a warp covering 32 consecutive rows.
 //
 // A Policy supplies the problem-specific parts:
 //   static constexpr int  BN, kABytes, kBBytes;  static constexpr bool kSplitA, kSplitB (operand needs the in-kernel split);
@@ -15,15 +19,21 @@
 //   struct Tile;  static __device__ Tile tile(p, tile);       // tile coordinates, decoded ONCE per tile (integer divisions)
 //   static __device__ void load(p, Tile&, mapA, mapB, sa, sb, sb_lo, bar, leader);   // TMA for the next k-block of the tile
 //                              // (fixed tx bytes, issued by the leader lane only); every lane advances the k cursor in Tile
-//   static __device__ uint64_t a_desc(uint32_t saddr, int ks); static __device__ uint64_t b_desc(uint32_t saddr, int ks);
+//   static __device__ void load16(..., halves);               // the same for the bf16 modes with a pre-converted B
 //   static __device__ void store(p, const Tile&, row, col0, const float (&v)[32]);     // 32 accumulator columns of one row
-//   static constexpr bool kSumA, kSumB;   // fused reductions over the contraction index done by the split warps (3xTF32
-//       only): kSumA = row sums of an MN-major A tile, kSumB = column sums of an MN-major B tile (bias gradients of the
-//       weight-gradient GEMMs -- the operand is in shared memory anyway, a separate column-sum pass re-reads it from HBM)
-//   static __device__ bool want_sums(p, Tile);  void sum_a_store(p, Tile, row, v);  void sum_b_store(p, Tile, col, float4 v);
-// The producer is ONE thread: anything it does per k-block is on the critical path of the whole SM (the first version
-// re-derived (b, t, f, tap) with integer divisions for every k-block -- ~1000 clk each -- and that, not the tensor pipe,
-// set the pace; see profiles/engine_ConvPolicy_r1.md).
+//   static constexpr bool kSumA, kSumB;   // fused reductions over the contraction index, taken from the fp32 operand tiles
+//       the consumers read anyway: kSumA = row sums of A, kSumB = column sums of an MN-major B tile (bias gradients of the
+//       weight-gradient GEMMs -- a separate column-sum pass would re-read the operand from HBM)
+//   static __device__ bool want_sums(p, Tile);  void sum_a_store(p, Tile, row, v);  void sum_b_store1(p, Tile, col, v);
+//       each called once per row / column and tile, with sums taken in a fixed order (no atomics: run-to-run reproducible)
+// The producer is ONE thread: anything it does per k-block is on the critical path of the whole SM, so tile coordinates are
+// decoded once per tile and k-blocks advance a cursor.
+//
+// Shared-memory tile layouts (TMA, 128-byte swizzle):
+//   K-major fp32 tile (rows x 32 k): row r = 128 B, 16-byte chunk c stored at chunk c ^ (r & 7)
+//   MN-major fp32 tile: chunks of 32 rows (4 KB) of 32 k-lines x 128 B; within a k-line, chunk c ^ (k & 7)
+//   MN-major bf16 tile ("pairs"): chunks of 64 rows (4 KB) of 32 k-lines x 128 B; within a k-line, chunk c ^ (k & 7)
+//   K-major bf16 tile (rows x 32 k): row r = 64 B, chunk c stored at c ^ ((r >> 1) & 3) (64-byte swizzle)
 #pragma once
 #include <type_traits>
 
@@ -33,77 +43,160 @@
 namespace b200asr {
 namespace tc {
 
-// NSPLIT selects the arithmetic: 1 = TF32 (SS-MMA), 3 = 3xTF32 (A split into TMEM, TS-MMA), and the kind::f16 modes
-// 2 = bf16 (A converted to bf16 into TMEM, one TS-MMA) and 6 = bf16x3 (2-term bf16 split, three TS-MMAs at twice the tf32
-// rate).  In the bf16 modes the fp32 A tile (K- or MN-major) is converted by the split warps on its way into TMEM, and B is
+// NSPLIT selects the arithmetic: 1 = TF32, 3 = 3xTF32 (hi*hi + hi*lo + lo*hi over x = hi + lo), 2 = bf16 and
+// 6 = bf16x3 (2-term bf16 split, three MMAs at twice the tf32 rate).  In the bf16 modes B is
 //   * either a PRE-CONVERTED K-major bf16 operand ([hi] or [hi | lo], 64-byte rows, SWIZZLE_64B; Policy::load16) -- weights,
 //   * or (Policy::kSplitB, both operands MN-major: the weight-gradient GEMMs, whose operands are activations) the raw fp32
-//     MN-major tile, which the split warps convert into bf16 MN-major tiles (64 columns = 128 bytes per k-line, SWIZZLE_128B)
-//     in a second shared-memory region of the stage.
+//     MN-major tile, which the consumers convert into K-major bf16 tiles in a second shared-memory region of the stage,
 //   * or (Policy::kBMN without kSplitB) MN-major bf16 hi | lo tiles that the PRODUCER of the activation already wrote next to
-//     the fp32 tensor ("pairs"): loaded by TMA like the weights, no conversion at all (convolution weight gradient).
-// Policy::b_desc16 describes the bf16 B tile in every case.
-constexpr bool eng_is_bf16(int nsplit) { return nsplit == 2 || nsplit == 6; }
-constexpr bool eng_has_split_warps(int nsplit) { return nsplit != 1; }
+//     the fp32 tensor ("pairs"): loaded by TMA like the weights and transposed in place.
+__host__ __device__ constexpr bool eng_is_bf16(int nsplit) { return nsplit == 2 || nsplit == 6; }
 
-constexpr int ENG_THREADS_X1 = 192;     // TMA, MMA, 4 epilogue warps
-constexpr int ENG_THREADS_X3 = 448;     // + 8 split warps
-constexpr int ENG_SPLIT_THREADS = 256;
-#ifndef ENG_SPLIT_GROUPS
-#define ENG_SPLIT_GROUPS 2              // the 8 split warps work as this many groups on alternating k-blocks
-#endif
+constexpr int ENG_THREADS = 384;
+constexpr int ENG_CONSUMERS = 256;
+constexpr int ENG_BAR = 1;                 // named barrier of the consumer threads
+constexpr int ENG_SMEM_CAP = 227 * 1024;   // dynamic shared memory per block on sm_90
 
-// 3xTF32 keeps the A operand in TENSOR MEMORY: the split warps read the raw fp32 tile from smem once and write
-// hi / lo straight into TMEM (tcgen05.st), and the MMAs run in the TS form (A from TMEM, B from smem).  Shared memory then
-// holds only [A_raw | B_hi | B_lo] per stage (48 KB instead of 64 KB for a 128x128 tile -> one more stage in flight) and the
-// tensor core no longer competes with the split for smem bandwidth on the A side (an SS 128x128x8 MMA reads 8 KB of smem
-// per 64 cycles = the full 128 B/clk of the SM).
-// A policy may opt in (static constexpr bool kCat = true) to the "concatenated" form of the 3xTF32 products at BN = 64: the
-// tensor core is markedly less efficient at N = 64 than at N = 128 (see tc_conv_halo.cu), so hi*hi and hi*lo become ONE N = 128
-// MMA against the adjacent [B_hi ; B_lo] tiles of the stage into a 128-column accumulator, lo*hi an N = 64 MMA into its first
-// half, and the epilogue adds the halves.  Costs accumulator columns: 4 stages of A in tensor memory instead of 6.
-template <class P, class = void> struct policy_cat : std::false_type {};
-template <class P> struct policy_cat<P, std::void_t<decltype(P::kCat)>> : std::bool_constant<P::kCat> {};
+enum EngBMode { B_READY, B_SPLIT_K, B_T32, B_T16_FROM32, B_T16 };
+// accumulator staging buffer of the epilogue: 128 rows of min(BN, 64) + 4 floats (+4: conflict-free row reads)
+constexpr int epilogue_bytes(int BN) { return 128 * ((BN < 64 ? BN : 64) + 4) * 4; }
 
 template <class Policy, int NSPLIT> struct EngineCfg {
   static constexpr bool kBf16 = eng_is_bf16(NSPLIT);
-  static constexpr bool kCat = policy_cat<Policy>::value && Policy::BN == 64 && NSPLIT == 3;
-  static constexpr int kAccW = kCat ? 128 : Policy::BN;                                      // accumulator columns per buffer
+  static constexpr int BN = Policy::BN;
   static constexpr int kBHalves = (NSPLIT == 3 || NSPLIT == 6) ? 2 : 1;                     // B tiles per stage (hi | lo)
-  static constexpr int kBTile = kBf16 ? Policy::BN * 64 : Policy::kBBytes;                   // bf16: 32 k x 2 B = 64-byte rows
-  static constexpr int kACols = NSPLIT == 3 ? 64 : (NSPLIT == 6 ? 32 : (NSPLIT == 2 ? 16 : 0));   // TMEM columns of A per stage
+  static constexpr int kBTile = kBf16 ? BN * 64 : Policy::kBBytes;                           // bf16: 32 k x 2 B = 64-byte rows
   static constexpr int kBRaw = (kBf16 && Policy::kSplitB) ? Policy::kBBytes : 0;             // bf16 + in-kernel B conversion: raw fp32 tile
   static constexpr int kStageBytes = Policy::kABytes + kBRaw + kBHalves * kBTile;
-  static constexpr int kMaxByTmem = NSPLIT == 1 ? 8 : (512 - 2 * kAccW) / kACols;
-  static constexpr int kBySmem = (200 * 1024) / kStageBytes;
-#ifndef ENG_MAX_STAGES
-#define ENG_MAX_STAGES 8
-#endif
-  static constexpr int kStagesRaw = kBySmem < kMaxByTmem ? kBySmem : kMaxByTmem;
-  static constexpr int kStagesCap = kStagesRaw > ENG_MAX_STAGES ? ENG_MAX_STAGES : kStagesRaw;
-  static constexpr int kStages = NSPLIT == 1 ? kStagesCap : kStagesCap - kStagesCap % ENG_SPLIT_GROUPS;
   static constexpr int kOffBraw = Policy::kABytes;
   static constexpr int kOffBhi = Policy::kABytes + kBRaw;
   static constexpr int kOffBlo = kOffBhi + kBTile;
-  static constexpr int kBarOff = kStages * kStageBytes;
-  static constexpr int kSmemBytes = kBarOff + 512 + 1024;
-  static constexpr int kAccCols = 2 * kAccW;
-  static constexpr int kTmemCols = NSPLIT != 1 ? 512 : (kAccCols <= 32 ? 32 : (kAccCols <= 64 ? 64 : (kAccCols <= 128 ? 128 : 256)));
+  static constexpr int kBMode = kBf16 ? (Policy::kSplitB ? B_T16_FROM32 : (Policy::kBMN ? B_T16 : B_READY))
+                                      : (Policy::kBMN ? B_T32 : ((NSPLIT == 3 && Policy::kSplitB) ? B_SPLIT_K : B_READY));
+  static constexpr bool kBSplit = NSPLIT == 3 && Policy::kSplitB;     // B_T32: fp32 B split into hi | lo while transposed
   static constexpr int kTxBytes = kBf16 ? Policy::kABytes + (Policy::kSplitB ? Policy::kBBytes : kBHalves * kBTile)
                                         : Policy::kABytes + Policy::kBBytes +
                                           (NSPLIT == 3 && !Policy::kSplitB ? Policy::kBBytes : 0);   // pre-split B arrives as hi+lo
+  static constexpr int kEpiBytes = epilogue_bytes(BN);
+  static constexpr int kBySmem = (ENG_SMEM_CAP - 1024 - kEpiBytes - 256) / kStageBytes;
+  static constexpr int kStages = kBySmem > 8 ? 8 : kBySmem;
+  static constexpr int kOffEpi = kStages * kStageBytes;
+  static constexpr int kBarOff = kOffEpi + kEpiBytes;
+  static constexpr int kSmemBytes = kBarOff + 256 + 1024;
   static_assert(!kBf16 || !Policy::kSplitB || (Policy::kAMN && Policy::kBMN),
                 "bf16 modes: a pre-converted bf16 B (K-major weights, or MN-major activation pairs), or both operands MN-major fp32 "
                 "with B converted in the kernel");
+  static_assert(!Policy::kSumB || Policy::kBMN, "column sums need an MN-major B tile");
+  static_assert(BN == 32 || BN == 64 || BN == 128, "BN");
   static_assert(kStages >= 2, "stage too large");
-  // Each split group must see EVERY phase of the full barriers it waits on: mbarrier parity waits only distinguish the
-  // current phase from the one before, so a group that skipped a phase of a stage could take a stale completion for the
-  // one it is waiting for.  With the stage count a multiple of the group count a stage always belongs to one group.
-  static_assert(NSPLIT == 1 || kStages % ENG_SPLIT_GROUPS == 0, "stage count must be a multiple of the split-group count");
+  static_assert(kSmemBytes <= ENG_SMEM_CAP, "shared memory");
 };
 
+// byte offset of fp32 element (row r, k) of an A tile
+template <bool MN> __device__ __forceinline__ uint32_t a_off(int r, int k) {
+  if constexpr (!MN) return r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4;
+  else return (r >> 5) * 4096 + k * 128 + ((((r & 31) >> 2) ^ (k & 7)) << 4) + (r & 3) * 4;
+}
+// K-major targets: fp32 (row n, k) in 128-byte rows, bf16 (row n, k) in 64-byte rows
+__device__ __forceinline__ uint32_t kmaj32_off(int n, int k) { return n * 128 + (((k >> 2) ^ (n & 7)) << 4) + (k & 3) * 4; }
+__device__ __forceinline__ uint32_t kmaj16_off(int n, int k) { return n * 64 + (((k >> 3) ^ ((n >> 1) & 3)) << 4) + (k & 7) * 2; }
+
+// One 32-deep k-block of a 128 x BN tile: this thread's A rows r0 / r1 (fp32 in shared memory at a_ptr(r, k)) rounded or
+// split into wgmma register fragments per NSPLIT, times the K-major B tile(s) at bhi (| blo); returns once the MMAs have
+// completed, so the caller may release the stage.  KPAIR: elements (r, k) and (r, k + 1) are adjacent (8-byte loads).
+// SUMS: asum0 / asum1 += the fp32 A values of rows r0 / r1 this thread read (a quarter of each row; the caller reduces).
+template <int NSPLIT, int BN, bool KPAIR, bool SUMS, class APtr>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], APtr a_ptr, int r0, int r1, int q, uint32_t bhi, uint32_t blo,
+                                           float& asum0, float& asum1) {
+  if constexpr (!eng_is_bf16(NSPLIT)) {
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) {
+      const int k0 = ks * 8 + q, k1 = k0 + 4;
+      const float x[4] = {*a_ptr(r0, k0), *a_ptr(r1, k0), *a_ptr(r0, k1), *a_ptr(r1, k1)};
+      if constexpr (SUMS) { asum0 += x[0] + x[2]; asum1 += x[1] + x[3]; }
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const float h = tf32_rn(x[i]);
+        ah[ks][i] = __float_as_uint(h);
+        al[ks][i] = __float_as_uint(x[i] - h);
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) {
+      if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
+        wgmma_tf32<BN>(acc, al[ks], kmajor_desc_tf32(bhi + ks * 32));
+        wgmma_tf32<BN>(acc, ah[ks], kmajor_desc_tf32(blo + ks * 32));
+      }
+      wgmma_tf32<BN>(acc, ah[ks], kmajor_desc_tf32(bhi + ks * 32));
+    }
+  } else {
+    uint32_t ah[2][4], al[2][4];
+#pragma unroll
+    for (int ks = 0; ks < 2; ks++) {
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int r = (i & 1) ? r1 : r0, k = ks * 16 + (i >> 1) * 8 + 2 * q;
+        float x0, x1;
+        if constexpr (KPAIR) {
+          const float2 v = *reinterpret_cast<const float2*>(a_ptr(r, k));
+          x0 = v.x; x1 = v.y;
+        } else {
+          x0 = *a_ptr(r, k);
+          x1 = *a_ptr(r, k + 1);
+        }
+        if constexpr (SUMS) { if (i & 1) asum1 += x0 + x1; else asum0 += x0 + x1; }
+        if constexpr (NSPLIT == 6) split_bf16_pair(x0, x1, ah[ks][i], al[ks][i]);
+        else ah[ks][i] = pack_bf16_pair(x0, x1);
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ks++) {
+      if constexpr (NSPLIT == 6) {
+        wgmma_bf16<BN>(acc, al[ks], kmajor_desc_bf16(bhi + ks * 32));
+        wgmma_bf16<BN>(acc, ah[ks], kmajor_desc_bf16(blo + ks * 32));
+      }
+      wgmma_bf16<BN>(acc, ah[ks], kmajor_desc_bf16(bhi + ks * 32));
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+}
+
+// Accumulators of a 128 x BN tile (this thread: rows r0 / r1) staged through shared memory `epi` (128 rows of EC + 4 floats)
+// and handed out as 32-column row pieces: out(row, col0, v[32]) with row = ctid % 128, so a warp covers 32 consecutive rows.
+// All ENG_CONSUMERS threads call it.
+template <int BN, class Out>
+__device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], float* epi, int ctid, int r0, int r1, int q, Out out) {
+  constexpr int EC = BN < 64 ? BN : 64, EP = EC + 4;
+#pragma unroll
+  for (int cc = 0; cc < BN / EC; cc++) {
+    named_bar_sync(ENG_BAR, ENG_CONSUMERS);           // the previous chunk's readers are done with the buffer
+#pragma unroll
+    for (int j = 0; j < EC / 8; j++) {
+      const int jj = cc * (EC / 8) + j, col = j * 8 + 2 * q;
+      *reinterpret_cast<float2*>(epi + r0 * EP + col) = make_float2(acc[4 * jj], acc[4 * jj + 1]);
+      *reinterpret_cast<float2*>(epi + r1 * EP + col) = make_float2(acc[4 * jj + 2], acc[4 * jj + 3]);
+    }
+    named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+    const int row = ctid & 127, piece = ctid >> 7;
+    if (piece < EC / 32) {
+      float v[32];
+#pragma unroll
+      for (int j = 0; j < 8; j++) {
+        const float4 t = *reinterpret_cast<const float4*>(epi + row * EP + piece * 32 + j * 4);
+        v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
+      }
+      out(row, cc * EC + piece * 32, v);
+    }
+  }
+}
+
 template <class Policy, int NSPLIT>
-__global__ void __launch_bounds__(eng_has_split_warps(NSPLIT) ? ENG_THREADS_X3 : ENG_THREADS_X1, 1)
+__global__ void __launch_bounds__(ENG_THREADS, 1)
 tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                  const typename Policy::Params p) {
   using Cfg = EngineCfg<Policy, NSPLIT>;
@@ -114,27 +207,18 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
   uint8_t* gen_base = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + Cfg::kBarOff;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto xfm_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (2 * S + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (3 * S + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (3 * S + 2 + b); };
-  const uint32_t tmem_slot = bar_base + 8u * (3 * S + 4);
+  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = Policy::num_tiles(p);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; s++) { mbar_init(full_bar(s), 1); mbar_init(xfm_bar(s), ENG_SPLIT_THREADS / ENG_SPLIT_GROUPS); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; b++) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), 128); }
+    for (int s = 0; s < S; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), ENG_CONSUMERS / 32); }
     fence_barrier_init();
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(gen_base + (tmem_slot - smem_base));
   griddep_launch();      // the next kernel in the stream may start its own prologue as our CTAs retire ...
   griddep_wait();        // ... and ours ran under the predecessor's tail: from here on its results are visible (common.cuh)
 
@@ -156,349 +240,184 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         __syncwarp();
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (whole warp loops, one lane issues)
-    // The issuing thread's own instruction stream is on the critical path: the tensor pipe's queue holds only a few MMAs,
-    // so whatever it executes between the last MMA of one k-block and the first of the next (barrier poll, descriptor
-    // arithmetic) must be shorter than the time that queue takes to drain -- ~130 clk with N = 64.  Descriptors are
-    // therefore built ONCE per CTA and advanced by adding to their 14-bit address field (shared memory is < 256 KB, so
-    // the field never carries into the stride fields above it); stage index and phase are running counters.
-    const bool leader = elect_one();
-    constexpr uint32_t idesc = make_idesc_tf32(128, BN, Policy::kAMN, Policy::kBMN);
-    constexpr uint32_t idesc_ts = make_idesc_tf32(128, BN, false, Policy::kBMN);
-    constexpr uint32_t idesc_cat = make_idesc_tf32(128, 128, false, Policy::kBMN);
-    constexpr bool kNeedXfm = NSPLIT != 1;
-    constexpr uint32_t idesc_bf = make_idesc_bf16(128, BN, false, Policy::kBMN);
-    constexpr uint32_t kStageStep = Cfg::kStageBytes >> 4, kLoStep = Cfg::kBTile >> 4;
-    uint64_t bd0, ad0;
-    uint32_t b_ks, a_ks;
-    if constexpr (Cfg::kBf16) {
-      bd0 = Policy::b_desc16(smem_base + Cfg::kOffBhi, 0); ad0 = 0;
-      b_ks = (uint32_t)(Policy::b_desc16(0, 1) - Policy::b_desc16(0, 0)); a_ks = 0;   // address-field step per 16-deep k-step
-    } else {
-      bd0 = Policy::b_desc(smem_base + Cfg::kOffBhi, 0); ad0 = Policy::a_desc(smem_base, 0);
-      b_ks = (uint32_t)(Policy::b_desc(0, 1) - Policy::b_desc(0, 0));     // address-field step per 8-deep k-step
-      a_ks = (uint32_t)(Policy::a_desc(0, 1) - Policy::a_desc(0, 0));
-    }
-    const uint32_t bd_hi = (uint32_t)(bd0 >> 32), ad_hi = (uint32_t)(ad0 >> 32);
-    auto mk = [](uint32_t hi, uint32_t lo) { return ((uint64_t)hi << 32) | lo; };
-    uint32_t s = 0, ph = 0, tcount = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, tcount++) {
-      const int nkb = Policy::num_kb(p, tile);
-      const uint32_t buf = tcount & 1;
-      mbar_wait(tempty_bar(buf), ((tcount >> 1) & 1) ^ 1);       // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * Cfg::kAccW;
-      for (int kb = 0; kb < nkb; kb++) {
-        mbar_wait(kNeedXfm ? xfm_bar(s) : full_bar(s), ph);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t b_lo32 = (uint32_t)bd0 + s * kStageStep, a_lo32 = (uint32_t)ad0 + s * kStageStep;
-          const uint32_t a_t = tmem_base + Cfg::kAccCols + s * Cfg::kACols;
-#pragma unroll
-          for (int ks = 0; ks < (Cfg::kBf16 ? 2 : 4); ks++) {
-            const uint64_t b_hi = mk(bd_hi, b_lo32 + ks * b_ks);
-            const uint32_t acc0 = (kb | ks) != 0 ? 1u : 0u;
-            if constexpr (NSPLIT == 1) {
-              umma_tf32(d_tmem, mk(ad_hi, a_lo32 + ks * a_ks), b_hi, idesc, acc0);
-            } else if constexpr (NSPLIT == 2) {
-              umma_bf16_ts(d_tmem, a_t + ks * 8, b_hi, idesc_bf, acc0);          // 16 k = 8 packed columns per step
-            } else if constexpr (NSPLIT == 6) {
-              const uint64_t b_lo = mk(bd_hi, b_lo32 + kLoStep + ks * b_ks);
-              const uint32_t a_hi = a_t + ks * 8, a_lo = a_hi + 16;
-              umma_bf16_ts(d_tmem, a_lo, b_hi, idesc_bf, acc0);
-              umma_bf16_ts(d_tmem, a_hi, b_lo, idesc_bf, 1u);
-              umma_bf16_ts(d_tmem, a_hi, b_hi, idesc_bf, 1u);
-            } else {
-              const uint64_t b_lo = mk(bd_hi, b_lo32 + kLoStep + ks * b_ks);
-              const uint32_t a_hi = a_t + ks * 8, a_lo = a_hi + 32;
-              if constexpr (Cfg::kCat) {
-                umma_tf32_ts(d_tmem, a_hi, b_hi, idesc_cat, acc0);             // [hi*hi | hi*lo]: B_lo follows B_hi in the stage
-                umma_tf32_ts(d_tmem, a_lo, b_hi, idesc_ts, 1u);                // + lo*hi into the first 64 columns
-              } else {
-                umma_tf32_ts(d_tmem, a_lo, b_hi, idesc_ts, acc0);
-                umma_tf32_ts(d_tmem, a_hi, b_lo, idesc_ts, 1u);
-                umma_tf32_ts(d_tmem, a_hi, b_hi, idesc_ts, 1u);
-              }
-            }
-          }
-          umma_commit(empty_bar(s));
-        }
-        __syncwarp();
-        if (++s == S) { s = 0; ph ^= 1; }
-      }
-      if (leader) umma_commit(tfull_bar(buf));
-      __syncwarp();
-    }
-  } else if (warp < 6) {
-    // ------------------------------------------------------------------ epilogue (warps 2-5: TMEM lane quarters 2,3,0,1)
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, tcount++) {
-      const uint32_t buf = tcount & 1;
-      const int nkb = Policy::num_kb(p, tile);
-      const typename Policy::Tile tc = Policy::tile(p, tile);
-      mbar_wait(tfull_bar(buf), (tcount >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; c++) {
-        float v[32];
-        if (nkb > 0) {
-          tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * Cfg::kAccW + (uint32_t)(c * 32), v);
-          if constexpr (Cfg::kCat) {
-            float w[32];
-            tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * Cfg::kAccW + (uint32_t)(64 + c * 32), w);
-#pragma unroll
-            for (int j = 0; j < 32; j++) v[j] += w[j];
-          }
-        } else
-#pragma unroll
-          for (int j = 0; j < 32; j++) v[j] = 0.f;
-        if (c == BN / 32 - 1) {            // all TMEM reads of this buffer are done: hand it back before the global stores
-          tc_fence_before();
-          mbar_arrive(tempty_bar(buf));
-        }
-        Policy::store(p, tc, row, c * 32, v);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ operand split warps (3xTF32 only)
-    if constexpr (Cfg::kBf16) {
-      // bf16 modes: the thread that owns A-tile row r reads its 32 fp32 k-values (K-major: one 128B-swizzled row; MN-major:
-      // one element per k-line), converts them to bf16 (NSPLIT == 6: hi and lo of the 2-term split) and stores them PACKED,
-      // two k per 32-bit column, into TMEM.  With Policy::kSplitB the group also converts the raw fp32 MN-major B tile into
-      // the bf16 MN-major tile(s) the tensor core reads.
-      constexpr int G = ENG_SPLIT_GROUPS, WPG = 8 / G, NT = ENG_SPLIT_THREADS / G;
-      static_assert(WPG == 4, "bf16 split: one thread per A row and group");
-      const int group = (warp - 6) / WPG;
-      const int t = threadIdx.x - 192 - group * NT;
-      const int quarter = warp & 3;
-      const int row = quarter * 32 + lane;
-      uint32_t kbg = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int nkb = Policy::num_kb(p, tile);
-        constexpr bool kSums = Policy::kSumA || Policy::kSumB;
-        typename Policy::Tile stc;
-        bool want = false;
-        if constexpr (kSums) { stc = Policy::tile(p, tile); want = Policy::want_sums(p, stc); }
-        float asum = 0.f;
-        float4 bsum[BN / 32];
-#pragma unroll
-        for (int c = 0; c < BN / 32; c++) bsum[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int kb = 0; kb < nkb; kb++, kbg++) {
-          if ((int)(kbg % G) != group) continue;
-          const int s = kbg % S;
-          mbar_wait(full_bar(s), (kbg / S) & 1);
-          uint8_t* stage = gen_base + s * Cfg::kStageBytes;
-          const uint8_t* araw = stage;
-          uint32_t hi[16], lo[16];
-          if constexpr (!Policy::kAMN) {
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-              const float4 x = *reinterpret_cast<const float4*>(araw + row * 128 + ((j ^ (row & 7)) << 4));
-              if constexpr (NSPLIT == 6) {
-                split_bf16_pair(x.x, x.y, hi[2 * j], lo[2 * j]);
-                split_bf16_pair(x.z, x.w, hi[2 * j + 1], lo[2 * j + 1]);
-              } else {
-                hi[2 * j] = pack_bf16_pair(x.x, x.y);
-                hi[2 * j + 1] = pack_bf16_pair(x.z, x.w);
-              }
-            }
-          } else {
-            // MN-major tile: chunk (row/32) of 32 k-lines x 128 B; 32-byte atom a = (row%32)/8 stored at atom (a ^ (k & 3))
-            const uint8_t* cbase = araw + (row >> 5) * 4096 + (row & 7) * 4;
-            const int atom = (row & 31) >> 3;
-#pragma unroll
-            for (int j = 0; j < 16; j++) {
-              const float x0 = *reinterpret_cast<const float*>(cbase + (2 * j) * 128 + ((atom ^ ((2 * j) & 3)) << 5));
-              const float x1 = *reinterpret_cast<const float*>(cbase + (2 * j + 1) * 128 + ((atom ^ ((2 * j + 1) & 3)) << 5));
-              if constexpr (NSPLIT == 6) split_bf16_pair(x0, x1, hi[j], lo[j]);
-              else hi[j] = pack_bf16_pair(x0, x1);
-              if constexpr (Policy::kSumA) asum += x0 + x1;
-            }
-          }
-          const uint32_t acol = tmem_base + ((uint32_t)(quarter * 32) << 16) + Cfg::kAccCols + s * Cfg::kACols;
-          tmem_st16u(acol, hi);
-          if constexpr (NSPLIT == 6) tmem_st16u(acol + 16, lo);
-          if constexpr (Policy::kSumB && !Policy::kSplitB) {
-            // column sums of a bf16 MN-major B tile that arrived by TMA (hi + lo = the 16-bit value the MMAs use): thread t
-            // owns column t -- 64-column chunks of 4 KB, k-line k at k * 128, 16-byte unit u stored at u ^ (k & 7)
-            if (want && t < BN) {
-              const uint8_t* bh = stage + Cfg::kOffBhi + ((t >> 6) << 12) + ((t & 7) << 1);
-              const int unit = (t & 63) >> 3;
-              float sum = 0.f;
-#pragma unroll 8
-              for (int k = 0; k < 32; k++) {
-                const uint8_t* q = bh + (k << 7) + ((unit ^ (k & 7)) << 4);
-                sum += __uint_as_float((uint32_t)(*reinterpret_cast<const uint16_t*>(q)) << 16);
-                if constexpr (NSPLIT == 6) sum += __uint_as_float((uint32_t)(*reinterpret_cast<const uint16_t*>(q + Cfg::kBTile)) << 16);
-              }
-              bsum[0].x += sum;
-            }
-          }
-          if constexpr (Policy::kSplitB) {
-            // raw tile: float4 i sits in 4 KB chunk i / 256 (32 columns), k-line (i % 256) / 8, 16-byte slot i % 8, and the
-            // logical 32-byte atom is (slot / 2) ^ (k & 3) (SWIZZLE_128B_ATOM_32B).  bf16 tile: 64-column chunks of 4 KB, k-line
-            // k at k * 128, 16-byte unit (8 columns) u stored at unit u ^ (k & 7) (SWIZZLE_128B).
-            const float4* braw = reinterpret_cast<const float4*>(stage + Cfg::kOffBraw);
-            uint8_t* bhi = stage + Cfg::kOffBhi;
-            uint8_t* blo = stage + Cfg::kOffBlo;
-            constexpr int NF4 = Policy::kBBytes / 16;
-#pragma unroll
-            for (int j = 0; j < NF4 / NT; j++) {
-              const int idx = t + j * NT;
-              const float4 x = braw[idx];
-              const int k = (idx & 255) >> 3, slot = idx & 7;
-              const int n = ((idx >> 8) << 5) + ((((slot >> 1) ^ (k & 3))) << 3) + ((slot & 1) << 2);
-              const int off = ((n >> 6) << 12) + (k << 7) + (((((n & 63) >> 3) ^ (k & 7))) << 4) + ((n & 7) << 1);
-              uint2 h, l;
-              if constexpr (NSPLIT == 6) {
-                split_bf16_pair(x.x, x.y, h.x, l.x);
-                split_bf16_pair(x.z, x.w, h.y, l.y);
-                *reinterpret_cast<uint2*>(blo + off) = l;
-              } else {
-                h.x = pack_bf16_pair(x.x, x.y);
-                h.y = pack_bf16_pair(x.z, x.w);
-              }
-              *reinterpret_cast<uint2*>(bhi + off) = h;
-              if constexpr (Policy::kSumB) {
-                float4& acc = bsum[(j * NT) / 256];
-                acc.x += x.x; acc.y += x.y; acc.z += x.z; acc.w += x.w;
-              }
-            }
-            fence_proxy_async_smem();
-          }
-          tmem_wait_st();
-          tc_fence_before();
-          mbar_arrive(xfm_bar(s));
-        }
-        if constexpr (kSums) {
-          if (want) {
-            if constexpr (Policy::kSumA) Policy::sum_a_store(p, stc, row, asum);
-            if constexpr (Policy::kSumB && Policy::kSplitB) {
-              const int slot = t & 7, kph = (t >> 3) & 3;
-              const int col_in_chunk = (((slot >> 1) ^ kph) << 3) + ((slot & 1) << 2);
-#pragma unroll
-              for (int c = 0; c < BN / 32; c++) Policy::sum_b_store(p, stc, c * 32 + col_in_chunk, bsum[c]);
-            }
-            if constexpr (Policy::kSumB && !Policy::kSplitB) {
-              if (t < BN) Policy::sum_b_store1(p, stc, t, bsum[0].x);
-            }
-          }
-        }
-      }
-    } else if (NSPLIT == 3) {
-      // The smem -> registers -> TMEM chain of one k-block is a serial latency (LDS, tcgen05.st, wait::st, arrive), so the
-      // warps are divided into groups that take alternating k-blocks: each thread handles a wider slice less often and the
-      // chains of consecutive k-blocks overlap.
-      constexpr int G = ENG_SPLIT_GROUPS, WPG = 8 / G, KPT = 128 / WPG;   // warps per group, k columns per thread
-      const int group = (warp - 6) / WPG;
-      const int kpart = ((warp - 6) % WPG) >> 2;    // which KPT-wide slice of the 32-deep block
-      const int t = threadIdx.x - 192 - group * WPG * 32;
-      const int quarter = warp & 3;                 // TMEM lanes this warp may touch
-      const int row = quarter * 32 + lane;          // A-tile row owned by this thread
-      uint32_t kbg = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int nkb = Policy::num_kb(p, tile);
-        constexpr bool kSums = Policy::kSumA || Policy::kSumB;
-        static_assert(!Policy::kSumA || Policy::kAMN, "row sums need an MN-major A tile (thread = row)");
-        static_assert(!Policy::kSumB || (Policy::kBMN && Policy::kSplitB), "column sums need an MN-major B tile split in the kernel");
-        typename Policy::Tile stc;
-        bool want = false;
-        if constexpr (kSums) { stc = Policy::tile(p, tile); want = Policy::want_sums(p, stc); }
-        float asum = 0.f;
-        float4 bsum[BN / 32];
-#pragma unroll
-        for (int c = 0; c < BN / 32; c++) bsum[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int kb = 0; kb < nkb; kb++, kbg++) {
-          if ((int)(kbg % G) != group) continue;
-          const int s = kbg % S;
-          mbar_wait(full_bar(s), (kbg / S) & 1);
-          const uint8_t* araw = gen_base + s * Cfg::kStageBytes;
-          float hi[KPT], lo[KPT];
-          if (!Policy::kAMN) {
-            // K-major tile: row = 128 B, 16-byte chunk j stored at chunk (j ^ (row & 7)) (128B swizzle)
-#pragma unroll
-            for (int j = 0; j < KPT / 4; j++) {
-              const int chunk = (kpart * (KPT / 4) + j) ^ (row & 7);
-              const float4 x = *reinterpret_cast<const float4*>(araw + row * 128 + chunk * 16);
-              hi[j * 4 + 0] = tf32_rn(x.x); lo[j * 4 + 0] = x.x - hi[j * 4 + 0];
-              hi[j * 4 + 1] = tf32_rn(x.y); lo[j * 4 + 1] = x.y - hi[j * 4 + 1];
-              hi[j * 4 + 2] = tf32_rn(x.z); lo[j * 4 + 2] = x.z - hi[j * 4 + 2];
-              hi[j * 4 + 3] = tf32_rn(x.w); lo[j * 4 + 3] = x.w - hi[j * 4 + 3];
-            }
-          } else {
-            // MN-major tile: chunk (row/32) of 32 k-lines x 128 B; 32-byte atom a = (row%32)/8 stored at atom (a ^ (k & 3))
-            const uint8_t* cbase = araw + (row >> 5) * 4096 + (row & 7) * 4;
-            const int atom = (row & 31) >> 3;
-#pragma unroll
-            for (int j = 0; j < KPT; j++) {
-              const int k = kpart * KPT + j;
-              const float x = *reinterpret_cast<const float*>(cbase + k * 128 + ((atom ^ (k & 3)) << 5));
-              hi[j] = tf32_rn(x); lo[j] = x - hi[j];
-              if constexpr (Policy::kSumA) asum += x;
-            }
-          }
-          const uint32_t acol = tmem_base + ((uint32_t)(quarter * 32) << 16) + Cfg::kAccCols + s * 64 + kpart * KPT;
-#pragma unroll
-          for (int i = 0; i < KPT / 16; i++) {
-            tmem_st16(acol + i * 16, hi + i * 16);
-            tmem_st16(acol + 32 + i * 16, lo + i * 16);
-          }
-          if (Policy::kSplitB) {
-            float4* stage = reinterpret_cast<float4*>(gen_base + s * Cfg::kStageBytes);
-            if constexpr (Policy::kSumB) {
-              // same elementwise split, plus per-thread partial column sums: float4 i of the tile sits in 4 KB chunk i / 256
-              // (32 columns), k-line (i % 256) / 8, 16-byte slot i % 8; with NT threads striding by NT (a divisor of 256)
-              // a thread keeps its slot and its k & 3, hence its 4 columns within every chunk (see sum_b_col below)
-              constexpr int NT = ENG_SPLIT_THREADS / G, NF4 = Policy::kBBytes / 16;
-              float4* bh = stage + Cfg::kOffBhi / 16;
-              float4* bl = stage + Cfg::kOffBlo / 16;
-#pragma unroll
-              for (int j = 0; j < NF4 / NT; j++) {
-                const int idx = t + j * NT;
-                const float4 x = bh[idx];
-                float4 h, l;
-                h.x = tf32_rn(x.x); l.x = x.x - h.x;
-                h.y = tf32_rn(x.y); l.y = x.y - h.y;
-                h.z = tf32_rn(x.z); l.z = x.z - h.z;
-                h.w = tf32_rn(x.w); l.w = x.w - h.w;
-                bh[idx] = h;
-                bl[idx] = l;
-                float4& acc = bsum[(j * NT) / 256];
-                acc.x += x.x; acc.y += x.y; acc.z += x.z; acc.w += x.w;
-              }
-            } else {
-              split_tf32_inplace(stage + Cfg::kOffBhi / 16, stage + Cfg::kOffBlo / 16, Policy::kBBytes / 16, t, ENG_SPLIT_THREADS / G);
-            }
-            fence_proxy_async_smem();
-          }
-          tmem_wait_st();
-          tc_fence_before();
-          mbar_arrive(xfm_bar(s));
-        }
-        if constexpr (kSums) {
-          if (want) {
-            if constexpr (Policy::kSumA) Policy::sum_a_store(p, stc, row, asum);
-            if constexpr (Policy::kSumB) {
-              // logical 32-byte atom = physical atom ^ (k & 3) (SWIZZLE_128B_ATOM_32B); k & 3 = (t / 8) & 3 for every j
-              const int slot = t & 7, kph = (t >> 3) & 3;
-              const int col_in_chunk = (((slot >> 1) ^ kph) << 3) + ((slot & 1) << 2);
-#pragma unroll
-              for (int c = 0; c < BN / 32; c++) Policy::sum_b_store(p, stc, c * 32 + col_in_chunk, bsum[c]);
-            }
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
+  if (warp < 4) return;
+
+  // -------------------------------------------------------------------- consumers
+  const int ctid = threadIdx.x - 128;                 // 0 .. 255
+  const int wg = ctid >> 7, cw = (ctid >> 5) & 3;
+  const int g = lane >> 2, q = lane & 3;
+  const int r0 = wg * 64 + cw * 16 + g, r1 = r0 + 8;  // the two A / accumulator rows of this thread
+  // B conversion: thread owns 4 consecutive columns n0..n0+3 and KR consecutive k from kk0
+  constexpr int NG = BN / 4, KSPL = ENG_CONSUMERS / NG, KR = 32 / KSPL;
+  const int n0 = (ctid % NG) * 4, kk0 = (ctid / NG) * KR;
+  float* epi = reinterpret_cast<float*>(gen_base + Cfg::kOffEpi);
+
+  uint32_t s = 0, ph = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int nkb = Policy::num_kb(p, tile);
+    const typename Policy::Tile tc = Policy::tile(p, tile);
+    constexpr bool kSums = Policy::kSumA || Policy::kSumB;
+    bool want = false;
+    if constexpr (kSums) want = Policy::want_sums(p, tc);
+    float asum0 = 0.f, asum1 = 0.f;
+    float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+
+    for (int kb = 0; kb < nkb; kb++) {
+      mbar_wait(full_bar(s), ph);
+      uint8_t* stage = gen_base + s * Cfg::kStageBytes;
+      const uint32_t stage_s = smem_base + s * Cfg::kStageBytes;
+
+      // ---- B as the K-major operand
+      if constexpr (Cfg::kBMode == B_SPLIT_K) {
+        // elementwise, so the (swizzled) layout does not matter: hi in place, lo into the lo tile
+        float4* bh = reinterpret_cast<float4*>(stage + Cfg::kOffBhi);
+        float4* bl = reinterpret_cast<float4*>(stage + Cfg::kOffBlo);
+#pragma unroll 4
+        for (int i = ctid; i < Policy::kBBytes / 16; i += ENG_CONSUMERS) {
+          const float4 x = bh[i];
+          float4 h, l;
+          h.x = tf32_rn(x.x); l.x = x.x - h.x;
+          h.y = tf32_rn(x.y); l.y = x.y - h.y;
+          h.z = tf32_rn(x.z); l.z = x.z - h.z;
+          h.w = tf32_rn(x.w); l.w = x.w - h.w;
+          bh[i] = h;
+          bl[i] = l;
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+      } else if constexpr (Cfg::kBMode == B_T32 || Cfg::kBMode == B_T16_FROM32) {
+        // fp32 MN-major tile -> K-major (tf32: as is, or hi | lo; bf16: hi (| lo)); thread: 4 columns x KR k-lines
+        const uint8_t* src = stage + (Cfg::kBMode == B_T32 ? Cfg::kOffBhi : Cfg::kOffBraw);
+        constexpr int NH = (Cfg::kBMode == B_T32 && !Cfg::kBSplit) ? Cfg::kBHalves : 1;    // pre-split halves transposed as they are
+        float x[NH][KR][4];
+#pragma unroll
+        for (int hf = 0; hf < NH; hf++)
+#pragma unroll
+          for (int i = 0; i < KR; i++) {
+            const int k = kk0 + i;
+            const float4 v = *reinterpret_cast<const float4*>(src + hf * Cfg::kBTile + (n0 >> 5) * 4096 + k * 128 +
+                                                              ((((n0 & 31) >> 2) ^ (k & 7)) << 4));
+            x[hf][i][0] = v.x; x[hf][i][1] = v.y; x[hf][i][2] = v.z; x[hf][i][3] = v.w;
+            if (hf == 0) { bsum.x += v.x; bsum.y += v.y; bsum.z += v.z; bsum.w += v.w; }
+          }
+        if constexpr (Cfg::kBMode == B_T32) named_bar_sync(ENG_BAR, ENG_CONSUMERS);     // in place: every thread has read the tile
+#pragma unroll
+        for (int c = 0; c < 4; c++) {
+          const int n = n0 + c;
+          if constexpr (Cfg::kBMode == B_T32) {
+#pragma unroll
+            for (int hf = 0; hf < (Cfg::kBSplit ? 2 : NH); hf++) {
+              float o[KR];
+#pragma unroll
+              for (int i = 0; i < KR; i++) {
+                const float v = x[Cfg::kBSplit ? 0 : hf][i][c];
+                o[i] = Cfg::kBSplit ? (hf == 0 ? tf32_rn(v) : v - tf32_rn(v)) : v;
+              }
+              uint8_t* dst = stage + Cfg::kOffBhi + hf * Cfg::kBTile + kmaj32_off(n, kk0);
+              if constexpr (KR == 4) *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
+              else if constexpr (KR == 2) *reinterpret_cast<float2*>(dst) = make_float2(o[0], o[1]);
+              else *reinterpret_cast<float*>(dst) = o[0];
+            }
+          } else {
+            uint32_t hi[(KR + 1) / 2], lo[(KR + 1) / 2];
+#pragma unroll
+            for (int i = 0; i < KR; i += 2) {
+              const float v0 = x[0][i][c], v1 = KR > 1 ? x[0][i + 1 < KR ? i + 1 : i][c] : 0.f;
+              if constexpr (NSPLIT == 6) split_bf16_pair(v0, v1, hi[i / 2], lo[i / 2]);
+              else hi[i / 2] = pack_bf16_pair(v0, v1);
+            }
+            uint8_t* dh = stage + Cfg::kOffBhi + kmaj16_off(n, kk0);
+            uint8_t* dl = stage + Cfg::kOffBlo + kmaj16_off(n, kk0);
+            if constexpr (KR == 4) {
+              *reinterpret_cast<uint2*>(dh) = make_uint2(hi[0], hi[1]);
+              if constexpr (NSPLIT == 6) *reinterpret_cast<uint2*>(dl) = make_uint2(lo[0], lo[1]);
+            } else if constexpr (KR == 2) {
+              *reinterpret_cast<uint32_t*>(dh) = hi[0];
+              if constexpr (NSPLIT == 6) *reinterpret_cast<uint32_t*>(dl) = lo[0];
+            } else {
+              *reinterpret_cast<uint16_t*>(dh) = (uint16_t)hi[0];
+              if constexpr (NSPLIT == 6) *reinterpret_cast<uint16_t*>(dl) = (uint16_t)lo[0];
+            }
+          }
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+      } else if constexpr (Cfg::kBMode == B_T16) {
+        // bf16 MN-major hi | lo tiles (64-column chunks) -> K-major bf16 tiles, in place; column sums of hi + lo
+        uint32_t hv[KR][2], lv[KR][2];
+#pragma unroll
+        for (int i = 0; i < KR; i++) {
+          const int k = kk0 + i;
+          const uint32_t off = (n0 >> 6) * 4096 + k * 128 + ((((n0 & 63) >> 3) ^ (k & 7)) << 4) + (n0 & 7) * 2;
+          const uint2 h = *reinterpret_cast<const uint2*>(stage + Cfg::kOffBhi + off);
+          uint2 l = make_uint2(0u, 0u);
+          if constexpr (NSPLIT == 6) l = *reinterpret_cast<const uint2*>(stage + Cfg::kOffBlo + off);
+          hv[i][0] = h.x; hv[i][1] = h.y; lv[i][0] = l.x; lv[i][1] = l.y;
+          bsum.x += __uint_as_float(h.x << 16) + __uint_as_float(l.x << 16);
+          bsum.y += __uint_as_float(h.x & 0xFFFF0000u) + __uint_as_float(l.x & 0xFFFF0000u);
+          bsum.z += __uint_as_float(h.y << 16) + __uint_as_float(l.y << 16);
+          bsum.w += __uint_as_float(h.y & 0xFFFF0000u) + __uint_as_float(l.y & 0xFFFF0000u);
+        }
+        named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+#pragma unroll
+        for (int c = 0; c < 4; c++) {
+          const int n = n0 + c;
+#pragma unroll
+          for (int hf = 0; hf < (NSPLIT == 6 ? 2 : 1); hf++) {
+            uint8_t* dst = stage + (hf ? Cfg::kOffBlo : Cfg::kOffBhi) + kmaj16_off(n, kk0);
+            uint32_t e[KR];     // column c of the 4: 16-bit half (c & 1) of word (c >> 1)
+#pragma unroll
+            for (int i = 0; i < KR; i++) e[i] = ((hf ? lv[i][c >> 1] : hv[i][c >> 1]) >> ((c & 1) * 16)) & 0xFFFFu;
+            if constexpr (KR == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(e[0] | (e[1] << 16), e[2] | (e[3] << 16));
+            else if constexpr (KR == 2) *reinterpret_cast<uint32_t*>(dst) = e[0] | (e[1] << 16);
+            else *reinterpret_cast<uint16_t*>(dst) = (uint16_t)e[0];
+          }
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+      }
+
+      // ---- A fragments + MMAs
+      const uint8_t* araw = stage;
+      mma_kblock<NSPLIT, BN, !Policy::kAMN, Policy::kSumA>(
+          acc, [&](int r, int k) { return reinterpret_cast<const float*>(araw + a_off<Policy::kAMN>(r, k)); }, r0, r1, q,
+          stage_s + Cfg::kOffBhi, stage_s + Cfg::kOffBlo, asum0, asum1);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s));
+      if (++s == S) { s = 0; ph ^= 1; }
+    }
+
+    // ---- fused reductions
+    if constexpr (kSums) {
+      if (want) {
+        if constexpr (Policy::kSumA) {
+          asum0 += __shfl_xor_sync(0xffffffffu, asum0, 1);
+          asum0 += __shfl_xor_sync(0xffffffffu, asum0, 2);
+          asum1 += __shfl_xor_sync(0xffffffffu, asum1, 1);
+          asum1 += __shfl_xor_sync(0xffffffffu, asum1, 2);
+          if (q == 0) { Policy::sum_a_store(p, tc, r0, asum0); Policy::sum_a_store(p, tc, r1, asum1); }
+        }
+        if constexpr (Policy::kSumB) {
+          // the KSPL threads of a column group hold sums over their k-lines: add them in a fixed order
+          named_bar_sync(ENG_BAR, ENG_CONSUMERS);         // the previous tile's epilogue is done with the buffer
+          *reinterpret_cast<float4*>(epi + (ctid / NG) * BN + n0) = bsum;
+          named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+          if (ctid < BN) {
+            float s = 0.f;
+            for (int j = 0; j < KSPL; j++) s += epi[j * BN + ctid];
+            Policy::sum_b_store1(p, tc, ctid, s);
+          }
+        }
+      }
+    }
+
+    // ---- epilogue
+    epilogue_rows<BN>(acc, epi, ctid, r0, r1, q, [&](int row, int col0, const float (&v)[32]) { Policy::store(p, tc, row, col0, v); });
   }
 }
 
@@ -511,7 +430,7 @@ int launch_engine(const CUtensorMap& ma, const CUtensorMap& mb, const typename P
   if (int rc = ensure_dynamic_smem((const void*)kern, Cfg::kSmemBytes, attr_set, what)) return rc;
   if (ntiles <= 0) return B200ASR_OK;
   const int grid = min(ntiles, device_sm_count());
-  launch_pdl(kern, dim3(grid), dim3(eng_has_split_warps(NSPLIT) ? ENG_THREADS_X3 : ENG_THREADS_X1), Cfg::kSmemBytes, st, ma, mb, p);
+  launch_pdl(kern, dim3(grid), dim3(ENG_THREADS), Cfg::kSmemBytes, st, ma, mb, p);
   return check_launch(what);
 }
 

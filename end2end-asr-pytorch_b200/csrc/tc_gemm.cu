@@ -1,17 +1,18 @@
-// tcgen05 GEMM for sm_100a: C[M,N] = sum_k A(m,k) B(k,n), fp32 in HBM, TF32 tensor-core math, fp32 accumulators in TMEM.
+// Tensor-core GEMM for sm_90a: C[M,N] = sum_k A(m,k) B(k,n), fp32 in HBM, TF32 / bf16 tensor-core math, fp32 accumulators.
 // A policy of the persistent tile engine (tc_engine.cuh):
 //
-//   * operands arrive by TMA (cp.async.bulk.tensor; 128B swizzle, 32-byte-atom variant for MN-major tiles) straight from
-//     the fp32 row-major tensors; either operand may be K-major (contraction contiguous) or MN-major (rows contiguous) --
-//     forward, data-gradient and weight-gradient GEMMs all run without a transpose pass;
+//   * operands arrive by TMA (cp.async.bulk.tensor, 128B swizzle) straight from the fp32 row-major tensors; either operand
+//     may be K-major (contraction contiguous) or MN-major (rows contiguous) -- forward, data-gradient and weight-gradient
+//     GEMMs all run without a transpose pass in HBM;
 //   * 128x128 output tiles, 32-deep k-blocks; tile = (m-tile, n-tile, k-split), n fastest so that the CTAs that run
 //     concurrently share the same A rows through L2;
-//   * NSPLIT = 1: kind::tf32 once; the tensor maps use the TFLOAT32 data type, so the copy engine rounds fp32 -> tf32
+//   * NSPLIT = 1: tf32 once; the tensor maps use the TFLOAT32 data type, so the copy engine rounds fp32 -> tf32
 //     to nearest in flight (measured: 4-5x lower error than letting the tensor core truncate the fp32 operands);
 //     NSPLIT = 3: "3xTF32" -- hi = rn_tf32(x), lo = x - hi, and lo*hi + hi*lo + hi*hi per k-step, which recovers
 //     fp32-grade products (error ~2^-21 relative) at three MMAs per step; weights can arrive pre-split (PRESPLIT);
-//   * epilogue: tcgen05.ld (32 lanes x 32 columns per warp) -> bias / ReLU / ReLU-mask / accumulate -> global;
-//     split-K with fp32 atomics for the skinny weight-gradient shapes; the weight-gradient instantiation (both operands
+//   * epilogue: 32-column row pieces (tc_engine.cuh) -> bias / ReLU / ReLU-mask / accumulate -> global;
+//     split-K for the skinny weight-gradient shapes (each split writes its partial tile, gemm_splitk_reduce sums them in
+//     split order); the weight-gradient instantiation (both operands
 //     MN-major) also produces the bias gradient = row sums of its A operand dy^T from the tiles it stages anyway.
 #include "../../include/b200asr.h"
 #include "common.cuh"
@@ -37,7 +38,7 @@ EncodeTiledFn get_encode_tiled() {
 }
 
 int make_tensor_map_f32(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                        const uint32_t* box, bool atom32b, bool tf32_dtype) {
+                        const uint32_t* box, bool tf32_dtype) {
   EncodeTiledFn enc = get_encode_tiled();
   if (!enc) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return B200ASR_CUDA_ERROR; }
   cuuint64_t gdim[5], gstride[4];
@@ -49,7 +50,7 @@ int make_tensor_map_f32(CUtensorMap* map, const void* base, int rank, const uint
   static thread_local bool ctx_bound = false;
   if (!ctx_bound) { cudaFree(nullptr); ctx_bound = true; }
   CUresult r = enc(map, tf32_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstride, bdim, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, atom32b ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return B200ASR_CUDA_ERROR; }
@@ -83,6 +84,8 @@ struct EpiP {
   const float* relu_mask;
   int relu, accumulate, splits, klen;
   float* rowsum;           // [M] += sum_k A(m,k) (bias gradient of the weight-gradient GEMM), or nullptr
+  float* part;             // splits > 1: partial tiles [splits][M][N] (scratch), summed by gemm_splitk_reduce
+  float* rowpart;          // splits > 1 with rowsum: partial row sums [splits][M]
 };
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -138,21 +141,12 @@ struct GemmPolicy {
     tma_load_2d(sb, mapB, bar, k0, n0);
     if (halves == 2) tma_load_2d(sb_lo, mapB, bar, k0, n0 + p.b_rows);
   }
-  // bf16 B tile: K-major (pre-converted weights): 64-byte rows, SWIZZLE_64B, a 16-deep k-step = 32 B along the row;
-  // MN-major (converted in the kernel): 64-column chunks of 4 KB, 8-k-line swizzle groups of 1 KB, a k-step = 16 k-lines = 2 KB
-  static __device__ __forceinline__ uint64_t b_desc16(uint32_t s, int ks) {
-    return B_MN ? make_smem_desc(s + ks * 2048, 4096, 1024, kLayoutSW128) : make_smem_desc(s + ks * 32, 16, 512, kLayoutSW64);
-  }
   // every (row, k) of A is staged once by the n-tile-0 tiles (over all k-splits)
   static __device__ __forceinline__ bool want_sums(const Params& p, const Tile& t) { return p.e.rowsum != nullptr && t.n0 == 0; }
   static __device__ __forceinline__ void sum_a_store(const Params& p, const Tile& t, int r, float v) {
-    if (t.m0 + r < p.e.M) atomicAdd(p.e.rowsum + t.m0 + r, v);
-  }
-  static __device__ __forceinline__ uint64_t a_desc(uint32_t s, int ks) {
-    return A_MN ? make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B) : make_smem_desc(s + ks * 32, 16, 1024);
-  }
-  static __device__ __forceinline__ uint64_t b_desc(uint32_t s, int ks) {
-    return B_MN ? make_smem_desc(s + ks * 1024, 4096, 512, kLayoutSW128Base32B) : make_smem_desc(s + ks * 32, 16, 1024);
+    if (t.m0 + r >= p.e.M) return;
+    if (p.e.splits > 1) p.e.rowpart[(size_t)t.z * p.e.M + t.m0 + r] = v;
+    else p.e.rowsum[t.m0 + r] += v;                      // one tile per row when K is not split
   }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const EpiP& e = p.e;
@@ -162,18 +156,16 @@ struct GemmPolicy {
     const int col0 = n0 + c0;
     float* crow = e.C + (size_t)row * e.ldc;
     const float* mrow = e.relu_mask ? e.relu_mask + (size_t)row * e.ldc : nullptr;
-    if (e.splits > 1) {
-      if (((e.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(e.C) & 15) == 0) && col0 + 32 <= e.N && !(e.bias && z == 0)) {
-        // a TMEM lane is a row, so the 32 lanes of a reduction instruction touch 32 rows whatever we do: make each one carry 16 bytes
+    if (e.splits > 1) {                                   // this split's partial tile
+      float* prow = e.part + ((size_t)z * e.M + row) * e.N;
+      if ((e.N & 3) == 0 && col0 + 32 <= e.N) {
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) red_add_v4(crow + col0 + j, v[j], v[j + 1], v[j + 2], v[j + 3]);
+        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(prow + col0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
         return;
       }
 #pragma unroll
-      for (int j = 0; j < 32; j++) {
-        const int col = col0 + j;
-        if (col < e.N) atomicAdd(crow + col, v[j] + ((e.bias && z == 0) ? e.bias[col] : 0.f));
-      }
+      for (int j = 0; j < 32; j++)
+        if (col0 + j < e.N) prow[col0 + j] = v[j];
       return;
     }
     const bool vec_ok = ((e.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(e.C) & 15) == 0);
@@ -230,6 +222,18 @@ struct GemmPolicy {
   }
 };
 
+// C = (accumulate ? C : 0) + bias + sum of the split partials in split order (split-K never carries ReLU or a mask)
+__global__ void gemm_splitk_reduce_kernel(const float* __restrict__ part, int splits, int M, int N, float* __restrict__ C, int ldc,
+                                          const float* __restrict__ bias, int accumulate) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)M * N) return;
+  const int row = (int)(i / N), col = (int)(i - (long long)row * N);
+  float s = 0.f;
+  for (int z = 0; z < splits; z++) s += part[(size_t)z * M * N + i];
+  float* c = C + (size_t)row * ldc + col;
+  *c = (accumulate ? *c : 0.f) + (bias ? bias[col] : 0.f) + s;
+}
+
 template <bool A_MN, bool B_MN, int NSPLIT, bool PRESPLIT = false>
 static int launch_persistent(const CUtensorMap& ma, const CUtensorMap& mb, const EpiP& e, cudaStream_t st, int b_rows = 0) {
   using Pol = GemmPolicy<A_MN, B_MN, PRESPLIT>;
@@ -239,6 +243,9 @@ static int launch_persistent(const CUtensorMap& ma, const CUtensorMap& mb, const
 
 }  // namespace tc
 
+static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const tc::EpiP& e, cudaStream_t st, bool a_kmaj,
+                       bool b_kmaj, int nsplit);
+
 bool gemm_tc_fuses_rowsum(bool a_kmaj, bool b_kmaj, int nsplit) { return !a_kmaj && !b_kmaj && (nsplit == 3 || nsplit == 6 || nsplit == 2); }
 
 int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, int ldb, float* C, int ldc, int M, int N,
@@ -247,7 +254,7 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
   using namespace tc;
   if (M <= 0 || N <= 0) return B200ASR_OK;
   if (eng_is_bf16(nsplit) && !(!a_kmaj && !b_kmaj)) {
-    // kind::f16 modes: fp32 K-major A converted in the kernel, pre-converted K-major bf16 B
+    // bf16 modes: fp32 K-major A converted in the kernel, pre-converted K-major bf16 B
     B200_REQUIRE(a_kmaj && b_split && b_rows >= N, B200ASR_BAD_ARG, "gemm_tc (bf16): needs a K-major A and the bf16 operand from b200asr_split_bf16");
     B200_REQUIRE(aligned16(A) && aligned16(b_split) && lda % 4 == 0 && ldb % 8 == 0, B200ASR_BAD_SHAPE,
                  "gemm_tc (bf16): TMA needs 16-byte row pitches (lda=%d must be a multiple of 4, ldb=%d of 8)", lda, ldb);
@@ -256,7 +263,7 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
     {
       uint64_t dims[2] = {(uint64_t)K, (uint64_t)M}, strides[1] = {(uint64_t)lda};
       uint32_t box[2] = {GBK, GBM};
-      if (int rc = make_tensor_map_f32(&ma, A, 2, dims, strides, box, false, false)) return rc;
+      if (int rc = make_tensor_map_f32(&ma, A, 2, dims, strides, box, false)) return rc;
     }
     {
       uint64_t dims[2] = {(uint64_t)K, (uint64_t)(nsplit == 6 ? 2 : 1) * b_rows}, strides[1] = {(uint64_t)ldb};
@@ -281,7 +288,7 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
     uint32_t box[2];
     if (a_kmaj) { dims[0] = (uint64_t)K; dims[1] = (uint64_t)M; box[0] = GBK; box[1] = GBM; }
     else        { dims[0] = (uint64_t)M; dims[1] = (uint64_t)K; box[0] = 32;  box[1] = GBK; }
-    rc = make_tensor_map_f32(&ma, A, 2, dims, strides, box, !a_kmaj, nsplit == 1);
+    rc = make_tensor_map_f32(&ma, A, 2, dims, strides, box, nsplit == 1);
     if (rc) return rc;
   }
   {
@@ -290,7 +297,7 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
     // pre-split B = [hi | lo] stacked along the row axis of the weight matrix (b_rows rows each)
     if (b_kmaj) { dims[0] = (uint64_t)K; dims[1] = (uint64_t)(presplit ? 2 * b_rows : N); box[0] = GBK; box[1] = GBN; }
     else        { dims[0] = (uint64_t)N; dims[1] = (uint64_t)(presplit ? 2 * b_rows : K); box[0] = 32;  box[1] = GBK; }
-    rc = make_tensor_map_f32(&mb, B, 2, dims, strides, box, !b_kmaj, nsplit == 1);
+    rc = make_tensor_map_f32(&mb, B, 2, dims, strides, box, nsplit == 1);
     if (rc) return rc;
   }
   B200_REQUIRE(!rowsum || gemm_tc_fuses_rowsum(a_kmaj, b_kmaj, nsplit), B200ASR_BAD_ARG, "gemm_tc: row sums are fused only into the MN/MN 3xTF32 kernel");
@@ -298,8 +305,8 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
   const int tiles = ceil_div(M, GBM) * ceil_div(N, GBN);
   if (!relu && !relu_mask && K >= 1024 && tiles * 2 <= device_sm_count()) {
     // Split-K only for skinny outputs (weight gradients: few tiles, long contraction).  A general "split against wave
-    // quantisation" rule was measured and lost: the zero-fill plus the per-element atomic epilogue cost more than the
-    // idle SMs of the last round (linear fwd 3.5 -> 4.9 ms per step at cfg2).
+    // quantisation" rule does not pay: writing and re-reading the partial tiles costs more than the idle SMs of the last
+    // round.
     const int sms = device_sm_count();
     int splits = min(min(sms / tiles, K / 256), 16);
     if (splits > 1) {
@@ -307,13 +314,30 @@ int gemm_tc(const float* A, bool a_kmaj, int lda, const float* B, bool b_kmaj, i
       e.splits = ceil_div(K, e.klen);
     }
   }
-  if (e.splits > 1 && !accumulate) cudaMemsetAsync(C, 0, sizeof(float) * (size_t)M * ldc, st);
+  if (e.splits > 1) {
+    const size_t n = (size_t)e.splits * M * N + (rowsum ? (size_t)e.splits * M : 0);
+    e.part = (float*)stream_scratch(sizeof(float) * n, st);
+    if (!e.part) return B200ASR_CUDA_ERROR;
+    e.rowpart = rowsum ? e.part + (size_t)e.splits * M * N : nullptr;
+    rc = presplit ? (b_kmaj ? launch_persistent<false, false, 3, true>(ma, mb, e, st, b_rows)
+                            : launch_persistent<false, true, 3, true>(ma, mb, e, st, b_rows))
+                  : launch_gemm(ma, mb, e, st, a_kmaj, b_kmaj, nsplit);
+    if (rc) return rc;
+    gemm_splitk_reduce_kernel<<<(unsigned)ceil_div_ll((long long)M * N, 256), 256, 0, st>>>(e.part, e.splits, M, N, C, ldc, bias, accumulate);
+    if ((rc = check_launch("gemm_splitk_reduce"))) return rc;
+    return rowsum ? reduce_parts(e.rowpart, e.splits, M, M, rowsum, 1, st) : B200ASR_OK;
+  }
+  if (presplit) return b_kmaj ? launch_persistent<false, false, 3, true>(ma, mb, e, st, b_rows)
+                              : launch_persistent<false, true, 3, true>(ma, mb, e, st, b_rows);
+  return launch_gemm(ma, mb, e, st, a_kmaj, b_kmaj, nsplit);
+}
+
+// the non-presplit fp32-map instantiations, by operand majors and arithmetic
+static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const tc::EpiP& e, cudaStream_t st, bool a_kmaj,
+                       bool b_kmaj, int nsplit) {
+  using namespace tc;
 #define GO(AM, BM_, NS) return launch_persistent<AM, BM_, NS>(ma, mb, e, st)
   const bool a_mn = !a_kmaj, b_mn = !b_kmaj;
-  if (presplit) {
-    if (!b_mn) return launch_persistent<false, false, 3, true>(ma, mb, e, st, b_rows);
-    return launch_persistent<false, true, 3, true>(ma, mb, e, st, b_rows);
-  }
   if (nsplit == 6) GO(true, true, 6);
   if (nsplit == 2) GO(true, true, 2);
   if (nsplit == 1) {

@@ -4,7 +4,7 @@ Mirrors `SpectrogramParser.parse_audio` (utils/data_loader.py:60-91) + the padde
 STFT (n_fft = sample_rate * window_size, hop = sample_rate * window_stride, symmetric Hamming window -- the reference
 passes the callable scipy.signal.hamming, which librosa evaluates as window(n_fft), i.e. sym=True --, centred frames),
 magnitude, log1p, per-utterance mean / unbiased-std normalisation, zero padding to the longest utterance.  One C-ABI call
-(`b200asr_stft_features`): the STFT of the whole batch is a single 3xTF32 tcgen05 GEMM over overlapping frame rows.
+(`b200asr_stft_features`): the STFT of the whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
 """
 from __future__ import annotations
 

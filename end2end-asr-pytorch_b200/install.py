@@ -1,4 +1,4 @@
-"""Drop-in installer: bind the B200 forwards onto the UNMODIFIED reference classes (class-level patch).
+"""Drop-in installer: bind the GPU forwards onto the UNMODIFIED reference classes (class-level patch).
 
     import b200asr; b200asr.install()      # after `utils.constant` has parsed its flags
 

@@ -20,22 +20,18 @@ _BF16_PRECS = (L.PREC_BF16, L.PREC_BF16X3)
 class _Config:
     """Arithmetic mode per kernel family (include/b200asr.h `precision`).
 
-    Default = the fp32-grade mix, everything on tcgen05 with a 2-term operand split and three MMAs per product:
-    "bf16x3" (kind::f16, x ~ bf16 hi + bf16 lo, twice the tf32 MMA rate) for the linear and convolution forward / data
-    gradient, "tf32x3" (kind::tf32) for the weight gradients and the attention contractions.  Measured at the TRUE cfg2
-    dims against the fp64 oracle (tests/test_gpu_fullsize_parity.py): logits 1.7e-5, every gradient tensor < 7e-5 in the
-    max norm at the path's own ReLU / pooling decisions (3xTF32 everywhere: 1.2e-5 / 5e-5; fp32 CUDA cores: 1.5e-6 / 4e-5).
+    Default = the fp32-grade mix, everything on the tensor cores with a 2-term operand split and three MMAs per product:
+    "bf16x3" (x ~ bf16 hi + bf16 lo, twice the tf32 MMA rate) for the linear and convolution forward / data gradient,
+    "tf32x3" for the weight gradients and the attention contractions; tests/test_gpu_fullsize_parity.py holds it to the fp64
+    oracle at the TRUE cfg2 dims (every gradient tensor in the max norm at the path's own ReLU / pooling decisions).
     Attention: the default "tf32x3" is the materialised path (batched 3xTF32 GEMMs around exact fp32 softmax kernels; at
-    these shapes -- T <= 250, 256 heads -- the 41 MB score tensor stays in the 126 MB L2); "bf16x3" selects the fused
-    kind::f16 kernels (tc_attention16.cu: QK^T / PV with masks, softmax and dropout on the accumulator in tensor memory, the
-    backward recomputing the probabilities).  Measured at cfg2: outputs and gradients ~1e-5 at kernel level, but the
-    flash-style delta = rowsum(dO o O) injects a row-constant error into dS that the near-uniform attention of this model
-    amplifies (Q/K projection gradients: up to 1.7e-3 at cfg4 against 3e-5 for the materialised path), and its softmax runs
-    on 4 warps per SM (fwd 131 us vs 60 us per call): opt-in, not default.
+    these shapes -- T <= 250, 256 heads -- the 41 MB score tensor fits the 50 MB L2); "bf16x3" selects the fused kernels
+    (tc_flash.cu: QK^T / PV with masks, softmax and dropout on the score fragments in registers, the backward
+    recomputing the probabilities), opt-in: its flash-style delta = rowsum(dO o O) injects a row-constant error into dS that
+    the near-uniform attention of this model amplifies in the Q/K projection gradients.
     Alternatives per family: "fp32" = CUDA-core kernels (exact fp32; attention = the flash-style kernel, which is also
-    what shapes outside the tensor-core shape rules run on), "tf32" = single-pass TF32 (convolutions: logits 3e-4 but
-    gradients ~6e-3; attention = the single-kernel flash forward/backward with S/P resident in TMEM, gradients ~3e-3
-    because dP - delta cancels in TF32) -- neither meets the 1e-3 gradient bar, so they are opt-in only."""
+    what shapes outside the tensor-core shape rules run on), "tf32" = single-pass TF32 (attention = the flash forward /
+    backward kernels) -- neither meets the 1e-3 gradient bar, so they are opt-in only."""
 
     def __init__(self):
         self.linear = _PREC_NAMES[os.environ.get("B200ASR_LINEAR", "bf16x3")]
@@ -318,11 +314,11 @@ class _WgradStream:
     """Weight-gradient GEMMs of the dense layers are off the critical path of the backward pass (nothing downstream reads
     them before the optimizer).  When `enabled` (parallel.DataParallelStep turns it on around loss.backward()) the ones that
     accumulate straight into the flat gradient buffer are queued on a second stream: their CTAs fill the SMs that the
-    data-gradient GEMMs of the main stream leave idle in their last, partial wave (100 / 200 / 300-tile problems on 148 SMs)
-    and run under the small LayerNorm / softmax kernels.  sync() makes the current stream wait for all of them.
-    MEASURED AND REJECTED as a default (cfg2: 18.0 -> 20.1 ms/step): the engine kernels are persistent (one CTA per SM for
-    the whole tile list, ~200 KB of shared memory each), so a weight-gradient kernel that got the SMs first holds them until
-    its last tile and the critical-path data-gradient kernel queues behind it.  Kept behind B200ASR_ASYNC_WGRAD=1."""
+    data-gradient GEMMs of the main stream leave idle in their last, partial wave and run under the small LayerNorm /
+    softmax kernels.  sync() makes the current stream wait for all of them.  Not the default: the engine kernels are
+    persistent (one CTA per SM for the whole tile list, most of the shared memory each), so a weight-gradient kernel that
+    got the SMs first holds them until its last tile and the critical-path data-gradient kernel queues behind it.  Kept
+    behind B200ASR_ASYNC_WGRAD=1."""
 
     def __init__(self):
         self.enabled, self.stream, self.used = False, None, False
@@ -370,7 +366,7 @@ def linear_bwd_weight(dy2, x2, want_bias, prec, w_sink=None, b_sink=None):
 def _linear_prec(N, K):
     """Shape rule (documented in DESIGN.md, not a fallback): TMA needs 16-byte row pitches, i.e. N % 4 == 0 and
     K % 4 == 0 for fp32 operands (other shapes, e.g. dim_input = 161 with feat_extractor='', run on the fp32 CUDA-core
-    GEMM) and additionally K % 8 == 0 for the bf16 weight operand of the kind::f16 modes (else the matching tf32 grade)."""
+    GEMM) and additionally K % 8 == 0 for the bf16 weight operand of the bf16 modes (else the matching tf32 grade)."""
     if not (N % 4 == 0 and K % 4 == 0):
         return L.PREC_FP32
     prec = config.linear
@@ -533,11 +529,11 @@ def _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop, head
     seed, off = rng.next() if p_drop > 0.0 else (0, 0)
     qs, ks, vs, os_ = _bhtd_strides(q), _bhtd_strides(k), _bhtd_strides(v), _bhtd_strides(out)
     # shape rules (not fallbacks; DESIGN.md section 4): the materialised 3xTF32 path needs head dims that are whole
-    # 32-float k-blocks and rows of at most 2048 keys; the TF32 flash kernel keeps the score row in TMEM
-    # (Tk <= 448, d in {32,64}); everything else runs on the fp32 CUDA-core kernel
+    # 32-float k-blocks and rows of at most 2048 keys; the TF32 flash kernels take Tk <= 448 and d in {32,64};
+    # everything else runs on the fp32 CUDA-core kernel
     prec = config.attn
     if prec == L.PREC_BF16X3 and not (dk == 64 and dv == 64 and Tk <= 448 and not head_major_out):
-        prec = L.PREC_TF32X3     # the fused kind::f16 kernels keep the score row in TMEM (Tk <= 448) and take 64-wide heads
+        prec = L.PREC_TF32X3     # the fused bf16x3 kernels take Tk <= 448 and 64-wide heads
     if prec == L.PREC_BF16:
         prec = L.PREC_TF32       # "bf16" (cfg5) attention = the single-pass TF32 flash kernels
     if prec == L.PREC_BF16X3:
@@ -571,7 +567,7 @@ def _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop, head
                                     float(p_drop), seed, off, prec, _stream()), "sdpa_fwd")
     bwd_prec = config.attn_bwd if (dk in (32, 64) and dv in (32, 64)) else L.PREC_FP32
     if bwd_prec == L.PREC_TF32X3:
-        bwd_prec = L.PREC_FP32       # the flash-style backward exists as fp32 (CUDA cores) and TF32 (tcgen05) only
+        bwd_prec = L.PREC_FP32       # the flash-style backward exists as fp32 (CUDA cores) and TF32 (tensor cores) only
     return out, dict(mat=False, tensors=(q, k, v, out, lse, key_pad, dense_mask),
                      meta=(int(causal), float(scale), float(p_drop), seed, off, bwd_prec))
 
@@ -661,7 +657,7 @@ class AttnProjFn(torch.autograd.Function):
 
     When the three projection weights (and biases, and their .grad) lie back to back in memory -- optim.FlatParams
     arranges that -- the projections of a common input run as one GEMM with N = 3*H*d (self-attention) or N = 2*H*d (K and
-    V of encoder-decoder attention): 200-tile problems on 148 SMs become 600-tile ones, the three data gradients become one
+    V of encoder-decoder attention): 200-tile problems on 132 SMs become 600-tile ones, the three data gradients become one
     GEMM with K = 3*H*d (no gradient-accumulation adds), the three weight gradients one split-K GEMM.  The attention kernels
     read Q/K/V as column slices of the packed projection output and write dQ/dK/dV into column slices of one packed
     buffer, all through strides.  Any other memory arrangement runs the same arithmetic as three GEMMs."""
@@ -805,9 +801,8 @@ class VggFrontendFn(torch.autograd.Function):
         y2 = new(B, T, F, C1)
         T2, F2 = T // 2, F // 2
         p1 = new(B, T2, F2, C1)
-        # (pool_idx = None: letting the epilogue also write the arg-max bytes for b200asr_maxpool2x2_bwd_idx was measured -- the
-        # pooling backward gets 0.2 ms cheaper, the convolution epilogue 1.0 ms dearer: it is the kernel's critical path)
-        # conv + ReLU + MaxPool2d(2, 2): in the kind::f16 modes the pooling is the convolution's epilogue
+        # (pool_idx = None: asking for the arg-max bytes of b200asr_maxpool2x2_bwd_idx runs the stand-alone pooling kernel)
+        # conv + ReLU + MaxPool2d(2, 2): in the bf16 modes the pooling is the convolution's epilogue
         L.check(lib.b200asr_conv3x3_fwd_pool(L.ptr(y1), L.ptr(_f32c(w2)), L.ptr(b2), L.ptr(y2), L.ptr(p1), None, L.ptr(ws), B, T, F, C1, C1, 1,
                                              prec, st), "conv2+pool1")
         y3 = new(B, T2, F2, C2)

@@ -1,7 +1,7 @@
 """Data-parallel training step: one process per GPU, replicated parameters, ONE all-reduce per step.
 
 Mirrors the reference's `--parallel` nn.DataParallel path (utils/functions.py:154-160, SURVEY.md §3.4) with the
-B200-native strategy of SURVEY.md §5.8: each rank runs forward/backward on its shard of the utterance batch with the
+strategy of SURVEY.md §5.8: each rank runs forward/backward on its shard of the utterance batch with the
 UN-normalised token-loss sum, the flat gradient buffer (+ [sum-loss, n_tokens]) is all-reduced once over
 NCCL/NVLink, and the optimizer divides by the GLOBAL token count -- exactly the reference's normalisation over the
 gathered global batch (trainer.py:84 + metrics.py:127-130).

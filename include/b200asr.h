@@ -1,4 +1,4 @@
-/* libb200asr -- C ABI of the B200-native speech-Transformer training hot path.
+/* libb200asr -- C ABI of the H100-native (sm_90a) speech-Transformer training hot path.
  *
  * The reference (gentaiscool/end2end-asr-pytorch) is pure Python on PyTorch and has NO FFI / operator
  * plugin interface (SURVEY.md §8b): its seams are nn.Module.forward methods and two free functions.  Each
@@ -8,13 +8,15 @@
  * Conventions
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless stated; fp32 data,
  *     int64 token ids (torch.long), uint8 masks (1 = masked / padded).
- *   - the caller owns all memory (including workspaces); the library never allocates, frees or keeps
- *     device pointers after the call returns.
+ *   - the caller owns all memory it passes (including workspaces); the library keeps one scratch buffer per
+ *     (device, stream) of its own, for the partial results of reductions summed in a fixed order, so that the same
+ *     inputs give the same bits every run (the fp32 CUDA-core GEMM / convolution / attention backward variants and
+ *     the im2col convolution path still accumulate with atomics).
  *   - every function enqueues work on `stream` (a cudaStream_t passed as void*) and returns without
  *     synchronising.  Return value: 0 on success, <0 on error (B200ASR_* below);
  *     b200asr_last_error() gives a thread-local message.  No C++ exception crosses the ABI.
- *   - `precision`: 0 = fp32 FMA on CUDA cores (exact-order fp32 accumulate); 1 = tcgen05 kind::tf32,
- *     one pass; 3 = tcgen05 3xTF32 split (fp32-grade).  An unsupported (shape, precision) pair is an
+ *   - `precision`: 0 = fp32 FMA on CUDA cores (exact-order fp32 accumulate); 1 = TF32 tensor cores,
+ *     one pass; 3 = 3xTF32 split (fp32-grade).  An unsupported (shape, precision) pair is an
  *     error -- there is no silent fallback of any kind (and no CPU path).
  *   - dropout: `p_drop` in [0,1); decisions come from a counter-based generator keyed by
  *     (seed, offset, element index), so *_bwd regenerates the mask of the matching *_fwd call when it is
@@ -39,7 +41,7 @@ extern "C" {
 #define B200ASR_PREC_FP32 0
 #define B200ASR_PREC_TF32 1
 #define B200ASR_PREC_TF32X3 3
-/* kind::f16 tensor-core modes (fp32 in HBM, operands converted on the way into the tensor core, fp32 accumulate):
+/* bf16 tensor-core modes (fp32 in HBM, operands converted on the way into the tensor core, fp32 accumulate):
  * BF16 = one bf16 MMA per product (BASELINE.json cfg5 asks for bf16); BF16X3 = 2-term bf16 split x ~ hi + lo (16 significant
  * bits) with hi*hi + hi*lo + lo*hi -- three MMAs at twice the TF32 rate, product error ~2^-17 (between TF32 and 3xTF32). */
 #define B200ASR_PREC_BF16 2
@@ -49,7 +51,7 @@ typedef void* b200asr_stream_t; /* cudaStream_t */
 
 int b200asr_version(void);
 const char* b200asr_last_error(void);
-/* 0 iff the current device is an sm_100 part (B200).  Called by the loader; everything else assumes it. */
+/* 0 iff the current device is an sm_90 part (H100).  Called by the loader; everything else assumes it. */
 int b200asr_device_check(void);
 /* Number of CUDA kernels this library has launched in the process so far (bench.py reports the per-step delta). */
 unsigned long long b200asr_launch_count(void);
@@ -73,7 +75,7 @@ int b200asr_linear_bwd_data(const float* dy, const float* w, const float* relu_o
  * w_split, precisions 2 / 6 (REQUIRED): the weight converted to bf16 by b200asr_split_bf16 -- linear_fwd takes `dst`
  * ([terms][N][K], needs K % 8 == 0), linear_bwd_data takes the transposed `dst_t` ([terms][K][N8], N8 = N rounded up to 8). */
 int b200asr_split_tf32(const float* src, float* dst_hi_lo, long long n, b200asr_stream_t stream);
-/* w [N,K] fp32 -> bf16 operands of the kind::f16 GEMMs: terms = 1: hi = bf16(w); terms = 2: hi followed by lo = bf16(w - hi).
+/* w [N,K] fp32 -> bf16 operands of the bf16 GEMMs: terms = 1: hi = bf16(w); terms = 2: hi followed by lo = bf16(w - hi).
  * dst [terms][N][K] (K-major for y = x w^T) and/or dst_t [terms][K][N8] (K-major for dx = dy w; zero padded columns);
  * either may be NULL. */
 int b200asr_split_bf16(const float* w, void* dst, void* dst_t, int N, int K, int terms, b200asr_stream_t stream);
@@ -136,12 +138,13 @@ int b200asr_sdpa_bwd(const float* dout, const float* q, const float* k, const fl
                      uint64_t seed, uint64_t offset, int precision, b200asr_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused attention at fp32 grade (the default path): ScaledDotProductAttention.forward, models/common_layers.py:211-225,
- * as ONE forward kernel (QK^T and PV on tcgen05 kind::f16 with the 2-term bf16 split, masks + softmax + dropout on the
- * accumulator in tensor memory) and TWO backward kernels that recompute the probabilities from Q, K and the forward's
+ * Fused attention at fp32 grade (opt-in): ScaledDotProductAttention.forward, models/common_layers.py:211-225,
+ * as ONE forward kernel (QK^T and PV on the tensor cores with the 2-term bf16 split, masks + softmax + dropout on the
+ * score fragments in registers) and TWO backward kernels that recompute the probabilities from Q, K and the forward's
  * log-sum-exp.  Same view / mask / dropout conventions as b200asr_sdpa_fwd.  Needs dk = dv = 64 and (forward) Tk <= 448.
- * ws16: b200asr_sdpa_fused_ws_bytes(B,H,Tq,Tk) bytes -- the bf16 hi / lo copies of q, k, v the forward makes; the SAME
- * buffer must be handed to the backward.  ws_bwd: b200asr_sdpa_fused_bwd_ws_bytes(B,H,Tq) bytes of scratch.
+ * ws16: b200asr_sdpa_fused_ws_bytes(B,H,Tq,Tk) bytes of workspace the caller keeps from the forward to the backward (the
+ * current kernels split the fp32 operands as they load them and leave it unused).  ws_bwd:
+ * b200asr_sdpa_fused_bwd_ws_bytes(B,H,Tq) bytes of scratch.
  */
 size_t b200asr_sdpa_fused_ws_bytes(int B, int H, int Tq, int Tk);
 size_t b200asr_sdpa_fused_bwd_ws_bytes(int B, int H, int Tq);
@@ -161,7 +164,7 @@ int b200asr_sdpa_fused_bwd(const float* dout, const float* q, const float* k, co
 /* Materialised attention (precision 1 = TF32, 3 = 3xTF32): the same contract as b200asr_sdpa_fwd/_bwd
  * (models/common_layers.py:211-225; head views addressed by strides; dropout drawn from the same counter stream, so
  * both paths produce identical masks), computed op for op like the reference -- bmm, masked softmax, dropout, bmm --
- * with the bmm's as batched tcgen05 GEMMs and the softmax (and its backward) as exact fp32 row kernels.
+ * with the bmm's as batched tensor-core GEMMs and the softmax (and its backward) as exact fp32 row kernels.
  * probs / probs_drop / dp_ws: caller-owned [B,H,Tq,round_up(Tk,4)] float buffers of b200asr_sdpa_mat_ws_bytes bytes;
  * probs (softmax output) and, when p_drop > 0, probs_drop (after dropout) must be kept for the backward call;
  * probs_drop may be NULL when p_drop == 0.  dk, dv multiples of 32; Tk <= 2048. */
@@ -196,7 +199,7 @@ int b200asr_conv3x3_c1_bwd_weight(const float* x, const float* dy, float* dw, fl
 int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int T,
                         int F, int Ci, int Co, int relu, int precision, b200asr_stream_t stream);
 /* The same convolution followed by MaxPool2d(2, stride 2) (models/asr/transformer.py:44-52: conv, ReLU, pool): y as above AND
- * pooled [B,T/2,F/2,Co] (floor mode).  In the kind::f16 modes the 2x2 maximum is taken in the convolution's epilogue (four
+ * pooled [B,T/2,F/2,Co] (floor mode).  In the bf16 modes the 2x2 maximum is taken in the convolution's epilogue (four
  * lanes of a warp hold a window), so the activation is not read back; other precisions run the two kernels.
  * pool_idx (optional) [B,T/2,F/2,Co] bytes: which element of each window holds the maximum (ATen's scan order, first maximum;
  * bit 2 set when the maximum is not positive) -- what b200asr_maxpool2x2_bwd_idx routes the gradient by; asking for it runs
@@ -259,9 +262,9 @@ int b200asr_bn_clamp_bwd(const float* dy, const float* x, const float* y, const 
                          int B, int C, int H, int W, int dy_pitch, int x_pitch, int y_pitch, int dx_pitch, int training,
                          float lo, float hi, b200asr_stream_t stream);
 /* The second emb_cnn convolution (models/asr/transformer.py:37, Conv2d(32, 32, (KH, KW), stride (SH, 1)), no padding) as
- * implicit GEMMs on tcgen05 -- no im2col matrix.  x / dx [B,32,H,W] with row pitch x_pitch, y / dy [B,32,OH,OW] with row
+ * implicit GEMMs on the tensor cores -- no im2col matrix.  x / dx [B,32,H,W] with row pitch x_pitch, y / dy [B,32,OH,OW] with row
  * pitch y_pitch (floats, multiples of 4: TMA); w [32,32,KH,KW].  precision 6 (bf16x3), 3 (3xTF32) or 2 (bf16) for forward
- * and data gradient; the weight gradient runs 3xTF32 and accumulates with atomics (dw is zeroed here).
+ * and data gradient; the weight gradient runs 3xTF32, one partial per row split, summed in split order.
  * ws: b200asr_conv2d_tc_ws_bytes(B, H, W, KH, KW) bytes -- the repacked weight slices, and four copies of the tensor whose
  * windows slide (x, or dy for the data gradient) shifted by 0..3 floats, because a TMA box must start on a 16-byte
  * boundary; each call rebuilds what it needs (one HBM-bound pass), so the same buffer may serve all three. */

@@ -2,7 +2,7 @@
 
 The reference parses its command line when `utils.constant` is first imported (utils/constant.py:99) and imports
 `Levenshtein` at module import (utils/metrics.py:3).  Neither is edited: this module
-  * finds the checkout (/root/reference in the build container, oracle/_ref on the GPU box -- see oracle/make_ref.py),
+  * finds the checkout ($B200ASR_REFERENCE, or the copy oracle/make_ref.py stages in oracle/_ref),
   * registers a tiny pure-Python `Levenshtein.distance` (python-Levenshtein is not installed; it is only called by
     calculate_cer / calculate_wer, which the Trainer loop uses for logging),
   * sets sys.argv for the first import and, on later calls, re-parses the flags into `constant.args` (every reference
@@ -19,7 +19,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def reference_root():
-    for cand in (os.environ.get("B200ASR_REFERENCE"), "/root/reference", os.path.join(HERE, "_ref")):
+    for cand in (os.environ.get("B200ASR_REFERENCE"), os.path.join(HERE, "_ref")):
         if cand and os.path.isdir(os.path.join(cand, "models", "asr")):
             return cand
     return None
@@ -44,7 +44,7 @@ def load(flags=(), q12_shim=False):
     optimizer.  `flags` are the reference's own command-line flags (utils/constant.py)."""
     root = reference_root()
     if root is None:
-        raise RuntimeError("reference checkout not found (neither /root/reference nor oracle/_ref: run oracle/make_ref.py)")
+        raise RuntimeError("reference checkout not found (neither $B200ASR_REFERENCE nor oracle/_ref: run oracle/make_ref.py)")
     if root not in sys.path:
         sys.path.insert(0, root)
     if "Levenshtein" not in sys.modules:

@@ -1,6 +1,6 @@
 """CPU-side checks of the C ABI: the in-tree library loads, exports every symbol include/b200asr.h declares, the ctypes
 prototypes agree with the header's parameter counts, and entry points fail with an error code (never crash, never
-compute on the CPU) when no B200 is present."""
+compute on the CPU) when no H100 is present."""
 import ctypes
 import re
 

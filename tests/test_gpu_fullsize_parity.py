@@ -158,16 +158,16 @@ def test_oracle_parity_at_true_baseline_dims(name):
 
 @pytest.mark.parametrize("name", ["cfg2", "cfg4"])
 def test_oracle_parity_3xtf32_everywhere(name):
-    """The kind::tf32 3xTF32 split for every contraction (the package default uses the kind::f16 bf16x3 split for the linear
+    """The 3xTF32 split for every contraction (the package default uses the bf16x3 split for the linear
     and convolution forward / data gradient)."""
     _check(name, dict(linear="tf32x3", conv="tf32x3", conv_wgrad="tf32x3", attn="tf32x3"))
 
 
 def test_cfg5_in_bf16_as_baseline_json_asks():
-    """BASELINE.json configs[4] is quoted in bf16: one kind::f16 MMA per product (bf16 operands, fp32 accumulate, fp32 master
+    """BASELINE.json configs[4] is quoted in bf16: one bf16 MMA per product (bf16 operands, fp32 accumulate, fp32 master
     weights and activations in HBM) for every linear / convolution GEMM incl. the weight gradients, single-pass TF32 flash
-    attention.  Tolerance stated separately, as SURVEY.md 8d asks -- bf16 cannot meet 1e-3: measured logits 9e-3, loss 2e-4,
-    gradients 2e-2 (max norm, at the path's own decisions); bars 3e-2 / 3e-2 / 6e-2."""
+    attention.  Tolerance stated separately, as SURVEY.md 8d asks -- bf16 cannot meet 1e-3: bars 3e-2 (logits) / 3e-2
+    (loss) / 6e-2 (gradients, max norm, at the path's own decisions)."""
     _check("cfg5", dict(linear="bf16", conv="bf16", conv_wgrad="bf16", attn="tf32", attn_bwd="tf32"), tol=3e-2, tol_grad=6e-2,
            fp32_grade=False)
 

@@ -24,7 +24,7 @@ def b200_mod():
 
 @pytest.fixture(params=["fp32", "default"])
 def b200(request, b200_mod):
-    """Every test runs twice: on the exact-fp32 CUDA-core kernels and on the package default (tcgen05 3xTF32 GEMM/conv).
+    """Every test runs twice: on the exact-fp32 CUDA-core kernels and on the package default (tensor-core GEMM/conv).
     `b200.k` scales the per-kernel tolerances (set for exact fp32) for the tensor-core mode; the end-to-end 1e-3 bar is
     the same in both."""
     import importlib

@@ -1,4 +1,4 @@
-"""-m gpu tests of the tcgen05 kernels against the exact-fp32 CUDA-core kernels and the CPU oracle.
+"""-m gpu tests of the tensor-core kernels against the exact-fp32 CUDA-core kernels and the CPU oracle.
 
 precision 1 (TF32, one pass) is checked at TF32 tolerance; precision 3 (3xTF32 split) must meet fp32-grade error."""
 import ctypes
@@ -115,7 +115,7 @@ def test_conv3x3_forward_and_dgrad_tensor_core(L, B, T, F_, Ci, Co, prec, tol):
 ])
 @pytest.mark.parametrize("bwd", ["fp32", "tf32"])
 def test_attention_tensor_core(L, B, H, Tq, Tk, dk, dv, mode, bwd):
-    """tcgen05 forward with either the fp32 CUDA-core backward or the tcgen05 backward (dK/dV kernel + dQ kernel)."""
+    """TF32 tensor-core forward with either the fp32 CUDA-core backward or the TF32 backward (dK/dV kernel + dQ kernel)."""
     import importlib
     import b200asr
     from tests.test_gpu_parity import _attention_case
@@ -160,8 +160,8 @@ def test_attention_materialised_3xtf32(L, B, H, Tq, Tk, dk, dv, mode):
     (2, 2, 100, 100, "causal"), (1, 1, 200, 200, "keypad"), (1, 2, 300, 448, "keypad"), (2, 2, 257, 400, "none"), (1, 2, 129, 65, "none"),
 ])
 def test_attention_fused_bf16x3(L, B, H, Tq, Tk, mode):
-    """The fused kind::f16 attention (tc_attention16.cu: one forward kernel, two backward kernels, scores / probabilities
-    only ever in tensor memory): fp32-grade against the oracle -- 3e-5 (the 2-term bf16 split carries 16 significant bits)."""
+    """The fused bf16x3 attention (tc_flash.cu: one forward kernel, two backward kernels, scores / probabilities
+    only ever in registers): fp32-grade against the oracle -- 3e-5 (the 2-term bf16 split carries 16 significant bits)."""
     import importlib
     import b200asr
     from tests.test_gpu_parity import _attention_case
@@ -276,7 +276,7 @@ def test_conv3x3_weight_gradient_tensor_core(L, B, T, F_, Ci, Co, prec, tol):
 @pytest.mark.parametrize("prec,tol", [(6, 1e-4), (2, 1e-2)])
 @pytest.mark.parametrize("B,T,F_,Ci,Co", [(2, 16, 32, 64, 64), (1, 9, 21, 64, 128), (3, 24, 41, 128, 128), (2, 10, 23, 128, 64), (1, 40, 161, 64, 64)])
 def test_conv3x3_weight_gradient_bf16_modes_and_pairs(L, B, T, F_, Ci, Co, prec, tol):
-    """kind::f16 weight gradient: (a) dy converted inside the kernel, (b) dy arriving as the bf16 hi | lo pairs its producers
+    """bf16 weight gradient: (a) dy converted inside the kernel, (b) dy arriving as the bf16 hi | lo pairs its producers
     write (max-pool backward with the ReLU mask, incl. the odd-F tail) -- B tiles by TMA, bias gradient from the bf16 tiles."""
     lib = L.load()
     g = torch.Generator().manual_seed(B * 11 + T)
@@ -399,7 +399,7 @@ def test_conv2d_first_layer_implicit_gemm(L, B, H, W, prec, tol):
 @pytest.mark.parametrize("prec", [6, 2, 3, 0])
 @pytest.mark.parametrize("B,T,F_,Ci,Co", [(2, 32, 16, 64, 64), (1, 37, 21, 64, 128), (2, 18, 161, 128, 128)])
 def test_conv3x3_with_fused_max_pool(L, B, T, F_, Ci, Co, prec):
-    """b200asr_conv3x3_fwd_pool == b200asr_conv3x3_fwd followed by b200asr_maxpool2x2_fwd, bit for bit (the kind::f16 modes take
+    """b200asr_conv3x3_fwd_pool == b200asr_conv3x3_fwd followed by b200asr_maxpool2x2_fwd, bit for bit (the bf16 modes take
     the 2x2 maximum in the convolution's epilogue; odd T / F exercise the floor-mode edges and partial tiles)."""
     lib = L.load()
     g = torch.Generator().manual_seed(B + T)

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import b200asr
-from oracle import asr_oracle as O
+from oracle import asr_oracle as O, ref_shim
 from tests.helpers import GOLDEN_CASES, load_golden
 
 
@@ -96,13 +96,11 @@ def test_cpu_tensors_are_rejected_not_computed():
         b200asr.calculate_metrics(torch.randn(2, 3, 8), torch.ones(2, 3, dtype=torch.long))
 
 
-REF = "/root/reference"
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout only exists in the build container")
+@pytest.mark.skipif(ref_shim.reference_root() is None, reason="reference checkout not staged (oracle/make_ref.py)")
 def test_install_rebinds_reference_classes_and_keeps_module_tree():
     """Runs in a subprocess because the reference parses flags at import (utils/constant.py:99)."""
     import subprocess
+    REF = ref_shim.reference_root()
     code = r'''
 import sys, types
 sys.path.insert(0, %r); sys.path.insert(0, %r)

@@ -10,7 +10,10 @@ from tests.helpers import GOLDEN_CASES, load_golden, rel_err, grads_rel_err
 @pytest.mark.parametrize("case", GOLDEN_CASES)
 def test_forward_loss_and_grads_match_reference(case):
     cfg, P, G, io, smoothing = load_golden(case)
-    pred, gold, hyp, loss, n_word, grads = O.forward_backward(P, cfg, io["in.src"], io["in.lengths"],
+    # the oracle runs in float64: in float32 its own rounding noise depends on the host's CPU thread count, and for gradients
+    # that are mathematically zero (a conv bias in front of BatchNorm) noise is all there is to compare
+    P = {k: v.double() for k, v in P.items()}
+    pred, gold, hyp, loss, n_word, grads = O.forward_backward(P, cfg, io["in.src"].double(), io["in.lengths"],
                                                               io["in.tgt"], smoothing)
     assert torch.equal(gold, io["out.gold"])
     assert rel_err(pred, io["out.pred"]) < 2e-5

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GPU check of the kind::f16 GEMM modes (precision 2 = bf16, 6 = bf16x3) against float64: y = x w^T + b and dx = dy w for
+"""GPU check of the bf16 GEMM modes (precision 2 = bf16, 6 = bf16x3) against float64: y = x w^T + b and dx = dy w for
 shapes with M / N / K tails.  Prints max|err| / max|ref| per (shape, precision); 3xTF32 (3) and TF32 (1) for comparison."""
 import importlib
 import sys

@@ -10,9 +10,9 @@ mkdir -p "$OBJ"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 pids=()
 for f in "$SRC"/*.cu; do
-  $NVCC -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC $defs -c "$f" -o "$OBJ/$(basename "${f%.cu}").o" &
+  $NVCC -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC $defs -c "$f" -o "$OBJ/$(basename "${f%.cu}").o" &
   pids+=($!)
 done
 for p in "${pids[@]}"; do wait "$p"; done
-$NVCC -shared -o "$SRC/build/variants/libb200asr_$name.so" "$OBJ"/*.o -gencode arch=compute_100a,code=sm_100a
+$NVCC -shared -o "$SRC/build/variants/libb200asr_$name.so" "$OBJ"/*.o -gencode arch=compute_90a,code=sm_90a
 echo "built $SRC/build/variants/libb200asr_$name.so"

@@ -41,7 +41,7 @@ def overheads(prec):
     dev = torch.device("cuda:0")
     for N in (128, 256):
         for K in (32, 256, 512, 2048, 8192):
-            M = 128 * 148
+            M = 128 * 132
             x = torch.randn(M, K, device=dev)
             w = torch.randn(N, K, device=dev) * 0.05
             b = torch.randn(N, device=dev)

@@ -4,7 +4,7 @@ shape is supported end to end (finite loss, no shape/alignment rejection) and pr
 (CUDA-event timed, 10 warm-up + 20 timed steps).  Usage:
     python tools/run_configs.py [cfg1 cfg2 ...] [--batch N] [--mode default|bf16|tf32x3|fp32]
 Modes: default = package default (bf16x3 linear/conv fwd+dgrad, tf32x3 conv wgrad + attention); bf16 = BASELINE cfg5's
-"bf16" (one kind::f16 MMA per product everywhere, TF32 flash attention); tf32x3 = 3xTF32 everywhere; fp32 = CUDA cores."""
+"bf16" (one bf16 MMA per product everywhere, TF32 flash attention); tf32x3 = 3xTF32 everywhere; fp32 = CUDA cores."""
 import importlib
 import json
 import sys
