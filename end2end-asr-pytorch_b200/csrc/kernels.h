@@ -44,5 +44,9 @@ int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, 
                      cudaStream_t st, float* dbias = nullptr, int* dbias_done = nullptr, const void* dy16 = nullptr);
 // dy16 (bf16 modes only): dy as bf16 hi | lo pairs [2][B,T,F,Co] written by its producer -> B tiles arrive by TMA
 // dbias: optional [Co] bias gradient; *dbias_done = 1 when the kernel produced it (3xTF32), else the caller must
+// Weight gradient at precision 3 / 1 with all nine taps of a 64-channel slice from one x patch per pixel block
+// (tc_conv_wgrad.cu); conv3x3_wgrad_tc dispatches to it for those precisions.  Same arguments as conv3x3_wgrad_tc.
+int conv3x3_wgrad_tc_halo(const float* x, const float* dy, float* dwr, int B, int T, int F, int Ci, int Co, int precision,
+                          cudaStream_t st, float* dbias, int* dbias_done);
 
 }  // namespace b200asr

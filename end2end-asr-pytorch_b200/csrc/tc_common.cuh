@@ -51,6 +51,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// The same bound without the message, for code that waits while its own wgmma are in flight: the printf is a function
+// call, and ptxas serializes every wgmma of a kernel whose MMA pipeline crosses a call.
+__device__ __forceinline__ void mbar_wait_inflight(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 4000000000LL) __trap();
+}
 // named barrier over `count` threads (a multiple of 32); id 0 is __syncthreads
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
@@ -139,6 +147,12 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 template <int N> __device__ __forceinline__ void acc_fence(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// register-A fragments of wgmma still in flight: a use here keeps the compiler from reusing their registers before the
+// wait that retires those MMAs (call it right after that wait)
+__device__ __forceinline__ void keep_live(const uint32_t (&a)[4]) {
+  asm volatile("" ::"r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]) : "memory");
 }
 
 // D[64 x N] += A[64 x k] (registers) * B[k x N] (shared memory, K-major), fp32 accumulate; k = 8 (tf32) or 16 (bf16).

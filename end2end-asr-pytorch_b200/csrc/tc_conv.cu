@@ -9,7 +9,8 @@
 // The box lands in shared memory as 128 rows x 128 B (K-major, 128B swizzle).
 // The B operand is the repacked weight wk[tap][n][c] (K-major, one 2-D box), pre-split into hi | lo for 3xTF32.
 //
-// Weight gradient:  dwr[tap][ci][co] += sum_p x[p + off(tap)][ci] * dy[p][co]
+// Weight gradient (bf16 modes; tf32 / 3xTF32 run on the halo weight-gradient kernel, tc_conv_wgrad.cu):
+//   dwr[tap][ci][co] += sum_p x[p + off(tap)][ci] * dy[p][co]
 // GEMM with the PIXEL axis as the contraction: both operands are MN-major (channels contiguous, pixels strided), i.e.
 // exactly the channels-last activations as they lie in HBM -- no transpose.  One k-block = a 2 (time) x 16 (freq) patch
 // of 32 pixels; the A tile is four 32-channel chunks {32 ch, 16, 2, 1} fetched at the tap-shifted coordinate (zero fill
@@ -253,7 +254,7 @@ int conv3x3_tc(const float* in, const float* wk, const float* bias, const float*
   return precision == 1 ? launch_conv_persistent<128, 1>(ma, mb, e, st) : launch_conv_persistent<128, 3>(ma, mb, e, st);
 }
 
-// dbias (optional, 3xTF32 only): [Co], zeroed here and accumulated by the kernel; returns with *dbias_done = 1 when the
+// dbias (optional, not at precision 1): [Co], produced by the kernel; returns with *dbias_done = 1 when the
 // kernel took care of it (the caller runs the separate column-sum pass otherwise)
 int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, int F, int Ci, int Co, int precision,
                      cudaStream_t st, float* dbias, int* dbias_done, const void* dy16) {
@@ -265,13 +266,14 @@ int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, 
   B200_REQUIRE((Ci == 64 || Ci == 128) && (Co == 64 || Co == 128), B200ASR_BAD_SHAPE,
                "conv3x3_wgrad_tc: needs Ci, Co in {64,128} (Ci=%d Co=%d)", Ci, Co);
   B200_REQUIRE(aligned16(x) && aligned16(pairs ? dy16 : (const void*)dy) && aligned16(dwr), B200ASR_BAD_ALIGN, "conv3x3_wgrad_tc: alignment");
+  // tf32 / 3xTF32: all nine taps per x patch (tc_conv_wgrad.cu); the tap-shifted policies below serve the bf16 modes
+  if (precision == 1 || precision == 3) return conv3x3_wgrad_tc_halo(x, dy, dwr, B, T, F, Ci, Co, precision, st, dbias, dbias_done);
   CUtensorMap mx, mdy;
-  const bool tf32 = precision == 1;
   {
     uint64_t dims[4] = {(uint64_t)Ci, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Ci, (uint64_t)F * Ci, (uint64_t)T * F * Ci};
     uint32_t box[4] = {32, WG_PF, WG_PT, 1};
-    if (int rc = make_tensor_map_f32(&mx, x, 4, dims, strides, box, tf32 && !pairs)) return rc;
+    if (int rc = make_tensor_map_f32(&mx, x, 4, dims, strides, box)) return rc;
   }
   if (pairs) {
     uint64_t dims[4] = {(uint64_t)Co, (uint64_t)F, (uint64_t)T, (uint64_t)2 * B};
@@ -282,9 +284,9 @@ int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, 
     uint64_t dims[4] = {(uint64_t)Co, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Co, (uint64_t)F * Co, (uint64_t)T * F * Co};
     uint32_t box[4] = {32, WG_PF, WG_PT, 1};
-    if (int rc = make_tensor_map_f32(&mdy, dy, 4, dims, strides, box, tf32)) return rc;
+    if (int rc = make_tensor_map_f32(&mdy, dy, 4, dims, strides, box)) return rc;
   }
-  const bool fuse_bias = dbias != nullptr && (pairs || precision != 1);
+  const bool fuse_bias = dbias != nullptr;
   WgP e{nullptr, nullptr, B, T, F, Ci, Co, ceil_div(F, WG_PF), ceil_div(T, WG_PT), 0, 0};
   const long long total = (long long)B * e.nft * e.ntt;
   B200_REQUIRE(total < (1LL << 31), B200ASR_BAD_SHAPE, "conv3x3_wgrad_tc: too many pixel blocks");
@@ -298,8 +300,6 @@ int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, 
 #define WGP(CIv, BNv)                                                                                                  \
   if (pairs) rc = precision == 6 ? launch_wgrad<CIv, BNv, 6, WgradPairPolicy<CIv, BNv>>(mx, mdy, e, splits, st)        \
                                  : launch_wgrad<CIv, BNv, 2, WgradPairPolicy<CIv, BNv>>(mx, mdy, e, splits, st);       \
-  else if (precision == 1) rc = launch_wgrad<CIv, BNv, 1>(mx, mdy, e, splits, st);                                     \
-  else if (precision == 3) rc = launch_wgrad<CIv, BNv, 3>(mx, mdy, e, splits, st);                                     \
   else if (precision == 6) rc = launch_wgrad<CIv, BNv, 6>(mx, mdy, e, splits, st);                                     \
   else rc = launch_wgrad<CIv, BNv, 2>(mx, mdy, e, splits, st);
   if (Ci == 64 && Co == 64) { WGP(64, 64) }

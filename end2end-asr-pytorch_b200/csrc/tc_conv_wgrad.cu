@@ -1,0 +1,308 @@
+// 3x3 convolution weight gradient, "halo" variant: all nine taps of a 64-input-channel slice from ONE x patch per pixel
+// block, 3xTF32 or TF32 (wgmma, register A).
+//
+//   dwr[tap][ci][co] = sum_p x[p + off(tap)][ci] * dy[p][co]        (pixels p are the contraction axis)
+//
+// Why: the tap-shifted weight gradient (tc_conv.cu, WgradPolicy) covers 128 rows of (tap, ci) per tile, so a pixel block's
+// dy tile is fetched, transposed and split once per tap group (5 or 9 times) and its x data once per tap.  Here a tile is
+// 9 taps x 64 input channels (M = 576, nine m64 row blocks) x 32 output channels: per pixel block of 4 (time) x 8 (freq)
+// the CTA loads the x patch including its one-pixel halo -- 6 x 10 pixels x 64 channels, TMA zero fill = padding -- and
+// the dy tile once, converts dy once for all nine taps, and the taps are nine shifted row mappings of the patch, exactly
+// as in the halo forward convolution (tc_conv_halo.cu).
+//
+// Roles (416 threads, 1 CTA / SM, one tile per CTA):
+//   warpgroups 0, 1, 2     consumers: warpgroup w owns taps 3w .. 3w + 2 (df = w - 1, dt = -1 .. 1), i.e. three m64n32
+//                          accumulator blocks.  Per (tap, 8-pixel k-step) a thread reads its four patch elements, splits
+//                          them into tf32 hi | lo fragments and issues the MMAs asynchronously; fragments are double
+//                          buffered, so the next k-step is built while the previous one's MMAs run (wgmma.wait_group 1).
+//   warp 12                producer: TMA of the x patch + dy tile of each pixel block into a ring of stages, and the dy
+//                          conversion -- raw MN-major tile -> K-major hi | lo in the same stage, once for all nine taps,
+//                          with the bias-gradient column sums on the way; it signals the consumers through an mbarrier.
+//
+// Contraction order inside a k-step: MMA k position j of step ks is pixel (time ks, freq 2j) for j < 4 and (ks, 2j - 7)
+// for j >= 4, so the four lanes q of a quad read patch columns 2q (+1): distinct 128-byte swizzle phases, no bank conflicts.
+// The dy conversion writes B in the same order.
+//
+// Each tile reduces one contiguous range of pixel blocks (its split) and writes its 576 x 32 partial to the split's slot of
+// [splits][9][Ci][Co]; reduce_parts sums the splits in a fixed order (no floating-point atomics: bit-reproducible).
+#include "../../include/b200asr.h"
+#include "common.cuh"
+#include "kernels.h"
+#include "tc_common.cuh"
+#include "tc_engine.cuh"
+
+namespace b200asr {
+namespace tc {
+
+constexpr int WH_T = 4, WH_F = 8;                        // pixel block = one 32-deep k-block
+constexpr int WH_PT = WH_T + 2, WH_PF = WH_F + 2;        // x patch incl. halo: 6 x 10 pixels
+constexpr int WH_PATCH_BOX = WH_PT * WH_PF * 128;        // 7,680 B per 32-channel box
+constexpr int WH_PATCH_CHUNK = 8192;                     // boxes on 1024-byte boundaries (128B swizzle phase = row & 7)
+constexpr int WH_N = 32;                                 // output channels per tile
+// three consumer warpgroups (warps 0-11) and one producer warp.  13 warps put 4 on one SM sub-partition, which caps a
+// thread at 128 registers: a consumer's three m64n32 accumulator blocks (48) and double-buffered fragments fit, three
+// m64n64 blocks (96) do not.
+constexpr int WH_CONSUMERS = 384;
+constexpr int WH_THREADS = WH_CONSUMERS + 32;
+
+struct WgHaloP {
+  float* part;         // [splits][9][Ci][Co] partial weight gradients
+  float* bpart;        // [splits][Co] partial bias gradients, or nullptr
+  int Ci, Co, ncs, ncn, nft, ntt, blocks_per_cta, total_blocks;
+};
+
+// stage: x patch (two 32-channel boxes) | raw dy tile (32-channel chunks, MN-major) | dy hi (| lo) K-major WH_N x 32
+template <int NSPLIT> struct WgHaloCfg {
+  static constexpr int kOffRaw = 2 * WH_PATCH_CHUNK;
+  static constexpr int kOffHi = kOffRaw + (WH_N / 32) * 4096;
+  static constexpr int kOffLo = kOffHi + WH_N * 128;
+  static constexpr int kStageBytes = kOffHi + (NSPLIT == 3 ? 2 : 1) * WH_N * 128;
+  static constexpr int kTxBytes = 2 * WH_PATCH_BOX + (WH_N / 32) * 4096;
+  static constexpr int kBySmem = (ENG_SMEM_CAP - 1024 - 256) / kStageBytes;
+  static constexpr int kStages = kBySmem > 8 ? 8 : kBySmem;
+  static constexpr int kBarOff = kStages * kStageBytes;
+  static constexpr int kSmemBytes = kBarOff + 256 + 1024;
+  static_assert(kStages >= 3, "stage too large");
+  static_assert(3 * 8 * kStages <= 256, "barriers");
+  static_assert(kSmemBytes <= ENG_SMEM_CAP, "shared memory");
+};
+
+template <int NSPLIT>
+__global__ void __launch_bounds__(WH_THREADS, 1)
+tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapDy, const WgHaloP p) {
+  using Cfg = WgHaloCfg<NSPLIT>;
+  constexpr int S = Cfg::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* gen_base = smem_raw + (smem_base - smem_u32(smem_raw));
+  const uint32_t bar_base = smem_base + Cfg::kBarOff;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };              // x patch and raw dy of stage s landed
+  auto ready_bar = [&](int s) { return bar_base + 8u * (S + s); };       // dy hi | lo of stage s written
+  auto empty_bar = [&](int s) { return bar_base + 8u * (2 * S + s); };   // the MMAs of stage s completed
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // tile = split z, then (input-channel slice, output-channel slice): the tiles of one split are adjacent CTAs (shared L2)
+  const int groups = p.ncs * p.ncn;
+  const int z = blockIdx.x / groups, grp = blockIdx.x % groups;
+  const int ci0 = (grp / p.ncn) * 64, co0 = (grp % p.ncn) * WH_N;
+  const int blk0 = z * p.blocks_per_cta;
+  const int nkb = max(0, min(p.blocks_per_cta, p.total_blocks - blk0));
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; s++) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(ready_bar(s), 1);
+      mbar_init(empty_bar(s), WH_CONSUMERS / 32);
+    }
+    fence_barrier_init();
+    tma_prefetch_desc(&mapX);
+    tma_prefetch_desc(&mapDy);
+  }
+  __syncthreads();
+  griddep_launch();      // programmatic dependent launch, see common.cuh
+  griddep_wait();
+
+  if (warp == WH_CONSUMERS / 32) {
+    // ------------------------------------------------------------------ producer: TMA + dy conversion
+    // The loads run S - 1 pixel blocks ahead of the conversion.  (Not S: the stage of block kb + S is free only once the
+    // consumers have moved on to block kb + 1, which waits for this warp's conversion of it.)
+    const bool leader = elect_one();
+    int ft = blk0 % p.nft, tt = (blk0 / p.nft) % p.ntt, b = blk0 / (p.nft * p.ntt);   // pixel-block cursor, ft fastest
+    uint32_t ls = 0, lph = 0;                          // ring position / phase of the next load
+    int loaded = 0;
+    auto load_next = [&]() {
+      mbar_wait_inflight(empty_bar(ls), lph ^ 1);
+      if (leader) {
+        const uint32_t sa = smem_base + ls * Cfg::kStageBytes;
+        const int f0 = ft * WH_F, t0 = tt * WH_T;
+        mbar_expect_tx(full_bar(ls), Cfg::kTxBytes);
+#pragma unroll
+        for (int c = 0; c < 2; c++) tma_load_4d(sa + c * WH_PATCH_CHUNK, &mapX, full_bar(ls), ci0 + c * 32, f0 - 1, t0 - 1, b);
+#pragma unroll
+        for (int c = 0; c < WH_N / 32; c++) tma_load_4d(sa + Cfg::kOffRaw + c * 4096, &mapDy, full_bar(ls), co0 + c * 32, f0, t0, b);
+      }
+      __syncwarp();
+      if (++ft == p.nft) {
+        ft = 0;
+        if (++tt == p.ntt) { tt = 0; b++; }
+      }
+      if (++ls == S) { ls = 0; lph ^= 1; }
+      loaded++;
+    };
+    while (loaded < nkb && loaded < S - 1) load_next();
+    // dy conversion: lane = output channels n = lane (+ 32 ...); bias-gradient column sums on the way
+    float bs[WH_N / 32][4] = {};
+    uint32_t s = 0, ph = 0;
+    for (int kb = 0; kb < nkb; kb++) {
+      mbar_wait_inflight(full_bar(s), ph);
+      uint8_t* stage = gen_base + s * Cfg::kStageBytes;
+#pragma unroll
+      for (int c = 0; c < WH_N / 32; c++) {
+        const int n = c * 32 + lane;
+        const uint8_t* raw = stage + Cfg::kOffRaw + c * 4096 + (lane & 3) * 4;
+#pragma unroll
+        for (int kg = 0; kg < 8; kg++) {          // K-major k = 4 kg .. 4 kg + 3 (see the contraction order above)
+          float x[4], h[4], l[4];
+#pragma unroll
+          for (int i = 0; i < 4; i++) {
+            const int pix = (kg >> 1) * WH_F + 2 * i + (kg & 1);
+            x[i] = *reinterpret_cast<const float*>(raw + pix * 128 + (((lane >> 2) ^ (pix & 7)) << 4));
+            bs[c][i] += x[i];
+            h[i] = NSPLIT == 3 ? tf32_rn(x[i]) : x[i];
+            l[i] = x[i] - h[i];
+          }
+          *reinterpret_cast<float4*>(stage + Cfg::kOffHi + kmaj32_off(n, 4 * kg)) = make_float4(h[0], h[1], h[2], h[3]);
+          if constexpr (NSPLIT == 3)
+            *reinterpret_cast<float4*>(stage + Cfg::kOffLo + kmaj32_off(n, 4 * kg)) = make_float4(l[0], l[1], l[2], l[3]);
+        }
+      }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(ready_bar(s));
+      if (++s == S) { s = 0; ph ^= 1; }
+      if (loaded < nkb) load_next();
+    }
+    // every pixel block is visited once by the input-channel-slice-0 tiles (over all splits)
+    if (p.bpart && ci0 == 0)
+#pragma unroll
+      for (int c = 0; c < WH_N / 32; c++) p.bpart[(size_t)z * p.Co + co0 + c * 32 + lane] = (bs[c][0] + bs[c][1]) + (bs[c][2] + bs[c][3]);
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers
+  const int wg = threadIdx.x >> 7, cw = warp & 3;
+  const int g = lane >> 2, q = lane & 3;
+  // A rows of this thread in each tap block: input channels cw * 16 + g and + 8 (same 32-channel box, swizzle chunks cch
+  // and cch + 2); tap 3 * wg + j reads patch row R + pcol, R = (t + j) * WH_PF + h, for pixel (t, 2q + h).  Its 128B
+  // swizzle term depends on (R + pcol) & 7; byte m of sw[m / 4] holds it for R & 7 = m, so that with R known at compile
+  // time a load is a byte extract, an xor and an immediate offset.  (Offsets hoisted per row, or an 8-register table,
+  // would not fit in the register budget next to the accumulators.)
+  const int cch = ((cw * 16 + g) & 31) >> 2;
+  const int pcol = wg + 2 * q;
+  const int aoff = (cw >> 1) * WH_PATCH_CHUNK + (g & 3) * 4 + pcol * 128;
+  uint32_t sw[2] = {0u, 0u};
+#pragma unroll
+  for (int m = 0; m < 8; m++) sw[m >> 2] |= ((cch ^ ((m + pcol) & 7)) << 4) << (8 * (m & 3));
+  float acc[3][WH_N / 2];
+#pragma unroll
+  for (int j = 0; j < 3; j++)
+#pragma unroll
+    for (int i = 0; i < WH_N / 2; i++) acc[j][i] = 0.f;
+  uint32_t ah[2][4] = {}, al[2][4] = {};
+  uint32_t s = 0, ph = 0;
+  for (int kb = 0; kb < nkb; kb++) {
+    mbar_wait_inflight(full_bar(s), ph);
+    mbar_wait_inflight(ready_bar(s), ph);
+    const uint8_t* patch = gen_base + s * Cfg::kStageBytes + aoff;
+    const uint32_t bhi = smem_base + s * Cfg::kStageBytes + Cfg::kOffHi, blo = bhi + (Cfg::kOffLo - Cfg::kOffHi);
+    asm volatile("" : "+r"(sw[0]), "+r"(sw[1]));     // keeps the extracts below in the loop (see sw)
+    auto ld = [&](int r, int c2) {
+      const uint32_t x = (sw[(r >> 2) & 1] >> (8 * (r & 3))) & 0xFFu;
+      return *reinterpret_cast<const float*>(patch + r * 128 + (x ^ (c2 ? 32 : 0)));
+    };
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+#pragma unroll
+      for (int ks = 0; ks < 4; ks++) {
+        const int u = (j * 4 + ks) & 1;
+        const int r = (ks + j) * WH_PF;
+        // fragment: a0 = (row g, pixel 2q), a1 = (g + 8, 2q), a2 = (g, 2q + 1), a3 = (g + 8, 2q + 1) of time row ks
+        const float x[4] = {ld(r, 0), ld(r, 1), ld(r + 1, 0), ld(r + 1, 1)};
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          const float h = tf32_rn(x[i]);
+          ah[u][i] = __float_as_uint(h);
+          al[u][i] = __float_as_uint(x[i] - h);
+        }
+        wgmma_fence();
+        if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
+          wgmma_tf32<WH_N>(acc[j], al[u], kmajor_desc_tf32(bhi + ks * 32));
+          wgmma_tf32<WH_N>(acc[j], ah[u], kmajor_desc_tf32(blo + ks * 32));
+        }
+        wgmma_tf32<WH_N>(acc[j], ah[u], kmajor_desc_tf32(bhi + ks * 32));
+        wgmma_commit();
+        wgmma_wait<1>();                        // the previous k-step's MMAs are done: its fragment buffer is free
+        keep_live(ah[u ^ 1]);                   // (so far: the compiler must not reuse those registers while they run)
+        keep_live(al[u ^ 1]);
+        if (j == 0 && ks == 0 && kb > 0) {      // ... and they were the last ones to read the previous stage
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(s == 0 ? S - 1 : s - 1));
+        }
+      }
+    }
+    if (++s == S) { s = 0; ph ^= 1; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int j = 0; j < 3; j++) acc_fence(acc[j]);
+
+  // ---- partials: accumulator (row g (+8), col 8 jj + 2q (+1)) -> [z][tap][ci][co]; a warp stores full 32-byte sectors
+#pragma unroll
+  for (int j = 0; j < 3; j++) {
+    float* o = p.part + (((size_t)z * 9 + 3 * wg + j) * p.Ci + ci0 + cw * 16 + g) * p.Co + co0 + 2 * q;
+#pragma unroll
+    for (int jj = 0; jj < WH_N / 8; jj++) {
+      *reinterpret_cast<float2*>(o + 8 * jj) = make_float2(acc[j][4 * jj], acc[j][4 * jj + 1]);
+      *reinterpret_cast<float2*>(o + 8 * (size_t)p.Co + 8 * jj) = make_float2(acc[j][4 * jj + 2], acc[j][4 * jj + 3]);
+    }
+  }
+}
+
+template <int NSPLIT>
+static int launch_wgrad_halo(const CUtensorMap& mx, const CUtensorMap& mdy, const WgHaloP& p, int tiles, cudaStream_t st) {
+  using Cfg = WgHaloCfg<NSPLIT>;
+  auto* kern = tc_conv3x3_wgrad_kernel<NSPLIT>;
+  static bool attr_set[kMaxDevices] = {};
+  if (int rc = ensure_dynamic_smem((const void*)kern, Cfg::kSmemBytes, attr_set, "tc_conv3x3_wgrad")) return rc;
+  if (tiles <= 0) return B200ASR_OK;
+  launch_pdl(kern, dim3(tiles), dim3(WH_THREADS), Cfg::kSmemBytes, st, mx, mdy, p);
+  return check_launch("tc_conv3x3_wgrad");
+}
+
+}  // namespace tc
+
+// precision 3 (3xTF32) or 1 (TF32, operands rounded by the TMA copy); dwr: [9][Ci][Co]; dbias (3xTF32 only, may be null)
+int conv3x3_wgrad_tc_halo(const float* x, const float* dy, float* dwr, int B, int T, int F, int Ci, int Co, int precision,
+                          cudaStream_t st, float* dbias, int* dbias_done) {
+  using namespace tc;
+  if (dbias_done) *dbias_done = 0;
+  B200_REQUIRE(precision == 1 || precision == 3, B200ASR_BAD_ARG, "conv3x3_wgrad_tc_halo: precision must be 1 or 3");
+  B200_REQUIRE((Ci == 64 || Ci == 128) && (Co == 64 || Co == 128), B200ASR_BAD_SHAPE,
+               "conv3x3_wgrad_tc_halo: needs Ci, Co in {64,128} (Ci=%d Co=%d)", Ci, Co);
+  B200_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(dwr), B200ASR_BAD_ALIGN, "conv3x3_wgrad_tc_halo: alignment");
+  const bool tf32 = precision == 1;
+  CUtensorMap mx, mdy;
+  {
+    uint64_t dims[4] = {(uint64_t)Ci, (uint64_t)F, (uint64_t)T, (uint64_t)B};
+    uint64_t strides[3] = {(uint64_t)Ci, (uint64_t)F * Ci, (uint64_t)T * F * Ci};
+    uint32_t box[4] = {32, WH_PF, WH_PT, 1};
+    if (int rc = make_tensor_map_f32(&mx, x, 4, dims, strides, box, tf32)) return rc;
+  }
+  {
+    uint64_t dims[4] = {(uint64_t)Co, (uint64_t)F, (uint64_t)T, (uint64_t)B};
+    uint64_t strides[3] = {(uint64_t)Co, (uint64_t)F * Co, (uint64_t)T * F * Co};
+    uint32_t box[4] = {32, WH_F, WH_T, 1};
+    if (int rc = make_tensor_map_f32(&mdy, dy, 4, dims, strides, box, tf32)) return rc;
+  }
+  const bool fuse_bias = dbias != nullptr && !tf32;
+  WgHaloP p{nullptr, nullptr, Ci, Co, Ci / 64, Co / WH_N, ceil_div(F, WH_F), ceil_div(T, WH_T), 0, 0};
+  const long long total = (long long)B * p.nft * p.ntt;
+  B200_REQUIRE(total < (1LL << 31), B200ASR_BAD_SHAPE, "conv3x3_wgrad_tc_halo: too many pixel blocks");
+  p.total_blocks = (int)total;
+  // one wave: about one tile per SM over the channel groups, at least 32 pixel blocks per tile
+  const int groups = p.ncs * p.ncn;
+  p.blocks_per_cta = max(32, ceil_div(p.total_blocks, max(1, device_sm_count() / groups)));
+  const int splits = ceil_div(p.total_blocks, p.blocks_per_cta);
+  const long long wn = 9LL * Ci * Co;
+  p.part = (float*)stream_scratch(sizeof(float) * (size_t)splits * (wn + (fuse_bias ? Co : 0)), st);
+  if (!p.part) return B200ASR_CUDA_ERROR;
+  p.bpart = fuse_bias ? p.part + (size_t)splits * wn : nullptr;
+  int rc = tf32 ? launch_wgrad_halo<1>(mx, mdy, p, groups * splits, st) : launch_wgrad_halo<3>(mx, mdy, p, groups * splits, st);
+  if (rc) return rc;
+  if ((rc = reduce_parts(p.part, splits, wn, wn, dwr, 0, st))) return rc;
+  if (!fuse_bias) return B200ASR_OK;
+  if (dbias_done) *dbias_done = 1;
+  return reduce_parts(p.bpart, splits, Co, Co, dbias, 0, st);
+}
+
+}  // namespace b200asr
