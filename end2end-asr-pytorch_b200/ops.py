@@ -176,7 +176,9 @@ class WeightOperandCache:
     from the next refresh on its operands are views of one bf16 buffer.  Freshness: the Adam kernel writes through raw
     pointers, so FusedAdam.step() calls refresh() itself; any other in-place change of a weight (torch optimizers,
     load_state_dict, manual edits) moves that tensor's autograd version counter away from the one recorded at the last
-    conversion, and get() then converts again (once: a refresh records the versions of all registered weights)."""
+    conversion, and get() then converts again (once: a refresh records the versions of all registered weights).  A write
+    through the flat buffer itself (flat.flat.copy_(snapshot), a broadcast into it) moves only the BUFFER's version counter --
+    the parameters were re-homed with `p.data = view`, which keeps their own counters -- so that one is tracked as well."""
 
     def __init__(self, flat):
         self.flat = flat                      # optim.FlatParams
@@ -185,6 +187,7 @@ class WeightOperandCache:
         self.tiles = 0
         self.tensors = {}                     # key -> the weight (a view of the flat buffer) as last seen
         self.converted_at = {}                # key -> its version counter when its operands were last converted
+        self.flat_converted_at = None         # the flat buffer's version counter at the last conversion
 
     def owns(self, w2):
         f = self.flat.flat
@@ -215,6 +218,7 @@ class WeightOperandCache:
                                                       len(self.entries), self.tiles, _stream()), "split_bf16_batched")
             for key, w2 in self.tensors.items():
                 self.converted_at[key] = w2._version
+            self.flat_converted_at = self.flat.flat._version
 
     def after_optimizer_step(self):
         if self.entries or self.pending:
@@ -229,8 +233,8 @@ class WeightOperandCache:
             self.pending.setdefault(key, w2)
             return None
         self.tensors[key] = w2
-        if self.converted_at.get(key) != w2._version:       # changed in place since the last conversion (not by our optimizer)
-            self.refresh()
+        if self.converted_at.get(key) != w2._version or self.flat.flat._version != self.flat_converted_at:
+            self.refresh()                                  # changed in place since the last conversion (not by our optimizer)
         _, _, _, _, do, dto = e
         n8 = (N + 7) // 8 * 8
         return WSplit(self.buf[do:do + terms * N * K].view(terms, N, K), self.buf[dto:dto + terms * K * n8].view(terms, K, n8))

@@ -44,7 +44,8 @@ def test_linear_forward_tensor_core(L, M, N, K, prec, tol):
 @pytest.mark.parametrize("prec,tol", [(1, 2e-3), (3, 1e-4)])   # 3xTF32: operands exact to ~2^-22; the residual is the
 @pytest.mark.parametrize("M,N,K", SHAPES)                      # tensor core's own fp32 accumulation over long K
 def test_linear_backward_tensor_core(L, M, N, K, prec, tol):
-    """bwd_data exercises an MN-major B operand, bwd_weight MN-major A and B (plus split-K atomics)."""
+    """bwd_data exercises an MN-major B operand, bwd_weight MN-major A and B.  Every contraction here is below 1024 rows, so
+    the weight gradients run unsplit; the split-K path is tested in test_gpu_default_precision.py."""
     lib = L.load()
     g = torch.Generator().manual_seed(M * 3 + N + K)
     x = torch.randn(M, K, generator=g).cuda()
@@ -88,10 +89,19 @@ def _conv_case(L, B, T, F_, Ci, Co, seed=0):
     return nhwc(x).cuda(), w.cuda(), b.cuda(), nhwc(y), nhwc(dy).cuda(), nhwc(dx)
 
 
-@pytest.mark.parametrize("prec,tol", [(1, 2e-3), (3, 2e-5)])
+# short time axes (T = 17 is one past a 16-row halo tile) and the cfg2 layer shapes (F = 161: 64 -> 64; F = 80: 64 -> 128, 128 -> 128)
+CONV_EDGE_SHAPES = [(2, 1, 41, 64, 64), (2, 2, 23, 64, 128), (1, 3, 80, 128, 128), (2, 17, 21, 64, 64), (2, 33, 161, 64, 64),
+                    (2, 25, 80, 64, 128), (2, 25, 80, 128, 128)]
+
+
+@pytest.mark.parametrize("prec,tol", [(1, 2e-3), (3, 2e-5), (6, 2e-5), (2, 1e-2)])
 @pytest.mark.parametrize("B,T,F_,Ci,Co", [(2, 16, 32, 64, 64), (1, 9, 21, 64, 128), (3, 24, 41, 128, 128), (2, 10, 23, 64, 64),
-                                          (1, 40, 161, 64, 64)])
+                                          (1, 40, 161, 64, 64)] + CONV_EDGE_SHAPES)
 def test_conv3x3_forward_and_dgrad_tensor_core(L, B, T, F_, Ci, Co, prec, tol):
+    """Forward (with and without ReLU) and data gradient (through a ReLU mask) against float64.  In the bf16 modes (the halo
+    kernel: bf16x3 is the default, bf16 is cfg5's) the data gradient also writes the bf16 pairs the layer below's weight
+    gradient reads: they must be the round-to-nearest-even split of the returned dx, bit for bit.  Measured on one H100 80GB
+    HBM3: bf16x3 <= 6.7e-6 (bar 2e-5), bf16 <= 2.7e-3 (bar 1e-2)."""
     lib = L.load()
     x, w, b, y_ref, dy, dx_ref = _conv_case(L, B, T, F_, Ci, Co, seed=B + T)
     ws = torch.empty(lib.b200asr_conv3x3_ws_bytes(Ci, Co) // 4, device="cuda")
@@ -103,8 +113,15 @@ def test_conv3x3_forward_and_dgrad_tensor_core(L, B, T, F_, Ci, Co, prec, tol):
     assert rel_err(y2, y_ref.relu()) < tol
     dx = torch.full((B, T, F_, Ci), float("nan"), device="cuda")
     mask = torch.randn(B, T, F_, Ci, device="cuda")
-    L.check(lib.b200asr_conv3x3_bwd_data(L.ptr(dy), L.ptr(w), L.ptr(mask), L.ptr(dx), None, L.ptr(ws), B, T, F_, Ci, Co, prec, _stream()), "conv dgrad")
+    dx16 = torch.full((2, B, T, F_, Ci), float("nan"), device="cuda", dtype=torch.bfloat16) if prec in (2, 6) else None
+    L.check(lib.b200asr_conv3x3_bwd_data(L.ptr(dy), L.ptr(w), L.ptr(mask), L.ptr(dx), L.ptr(dx16), L.ptr(ws), B, T, F_, Ci, Co, prec,
+                                         _stream()), "conv dgrad")
     assert rel_err(dx, dx_ref.cuda() * (mask > 0)) < tol
+    if dx16 is not None:
+        hi = dx.to(torch.bfloat16)
+        lo = (dx - hi.float()).to(torch.bfloat16)
+        assert torch.equal(dx16[0].view(torch.int16), hi.view(torch.int16))
+        assert torch.equal(dx16[1].view(torch.int16), lo.view(torch.int16))
 
 
 # ------------------------------------------------------------------------------------------------ attention
@@ -256,7 +273,7 @@ def test_attention_tensor_core_rejects_long_keys(L):
 
 @pytest.mark.parametrize("prec,tol", [(1, 2e-3), (3, 1e-4)])
 @pytest.mark.parametrize("B,T,F_,Ci,Co", [(2, 16, 32, 64, 64), (1, 9, 21, 64, 128), (3, 24, 41, 128, 128), (2, 10, 23, 128, 64),
-                                          (1, 40, 161, 64, 64)])
+                                          (1, 40, 161, 64, 64)] + CONV_EDGE_SHAPES)
 def test_conv3x3_weight_gradient_tensor_core(L, B, T, F_, Ci, Co, prec, tol):
     lib = L.load()
     g = torch.Generator().manual_seed(B * 7 + T)
@@ -399,8 +416,10 @@ def test_conv2d_first_layer_implicit_gemm(L, B, H, W, prec, tol):
 @pytest.mark.parametrize("prec", [6, 2, 3, 0])
 @pytest.mark.parametrize("B,T,F_,Ci,Co", [(2, 32, 16, 64, 64), (1, 37, 21, 64, 128), (2, 18, 161, 128, 128)])
 def test_conv3x3_with_fused_max_pool(L, B, T, F_, Ci, Co, prec):
-    """b200asr_conv3x3_fwd_pool == b200asr_conv3x3_fwd followed by b200asr_maxpool2x2_fwd, bit for bit (the bf16 modes take
-    the 2x2 maximum in the convolution's epilogue; odd T / F exercise the floor-mode edges and partial tiles)."""
+    """b200asr_conv3x3_fwd_pool with the pooling index bytes == b200asr_conv3x3_fwd followed by b200asr_maxpool2x2_fwd, bit
+    for bit, in every precision: asking for the index bytes routes the call to the convolution followed by the stand-alone
+    pooling kernel (odd T / F exercise the floor-mode edges).  The bf16 modes' epilogue pooling, taken when no index bytes are
+    asked for, is tested by test_gpu_default_precision.py::test_conv3x3_pool_in_epilogue."""
     lib = L.load()
     g = torch.Generator().manual_seed(B + T)
     x = torch.randn(B, T, F_, Ci, generator=g).cuda()

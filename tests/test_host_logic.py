@@ -161,7 +161,8 @@ def test_weight_operand_cache_converts_once_per_change(monkeypatch):
     """ops.WeightOperandCache bookkeeping with the conversion kernel stubbed out (no GPU): a weight is registered on first use,
     converted by the refresh of the optimizer step, NOT converted again by the first get() after that (the regression: every
     weight's first get() re-converted all of them -- 46 launches in the step after registration), and converted again when
-    the tensor changes in place behind the optimizer's back."""
+    the tensor changes in place behind the optimizer's back, including a write through the flat buffer into a parameter
+    re-homed by `p.data = view` (the regression: the stale operands of the previous weights fed the next forward)."""
     ops = importlib.import_module(b200asr.__name__ + ".ops")
     L = importlib.import_module(b200asr.__name__ + "._lib")
     calls = []
@@ -196,3 +197,12 @@ def test_weight_operand_cache_converts_once_per_change(monkeypatch):
     cache.get(w1, L.PREC_BF16X3)
     cache.get(w2, L.PREC_BF16X3)                 # w2 shares the buffer's version counter: its view changed version too, but
     assert calls == [2, 2, 2]                    # the refresh that followed the edit already covers it
+    p = torch.nn.Parameter(torch.empty(16, 32))
+    p.data = Flat.flat[2048:2560].view(16, 32)   # re-homed as optim.FlatParams does it: p keeps its own version counter
+    assert cache.get(p, L.PREC_BF16X3) is None
+    cache.after_optimizer_step()
+    assert calls == [2, 2, 2, 3]
+    Flat.flat.copy_(torch.ones(4096))            # a write through the buffer (a snapshot restored, a broadcast into it) ...
+    assert p._version == 0
+    cache.get(p, L.PREC_BF16X3)
+    assert calls == [2, 2, 2, 3, 3]              # ... is seen although the parameter's counter did not move
