@@ -117,6 +117,7 @@ __global__ void __launch_bounds__(256) softmax_bwd_kernel(SoftP p, const float* 
   float* drow = dpd + row * p.ldp;
   float4 pv[NV], dv[NV];
   float delta = 0.f;
+  bool all_nan = true;
 #pragma unroll
   for (int i = 0; i < NV; i++) {
     const int col = 4 * (lane + 32 * i);
@@ -124,6 +125,7 @@ __global__ void __launch_bounds__(256) softmax_bwd_kernel(SoftP p, const float* 
     dv[i] = pv[i];
     if (col < p.ldp) {
       pv[i] = *reinterpret_cast<const float4*>(prow + col);
+      all_nan = all_nan && isnan(pv[i].x) && isnan(pv[i].y) && isnan(pv[i].z) && isnan(pv[i].w);
       float4 d = *reinterpret_cast<const float4*>(drow + col);
       if (p.thresh) {
         bool kp[4];
@@ -136,10 +138,14 @@ __global__ void __launch_bounds__(256) softmax_bwd_kernel(SoftP p, const float* 
     }
   }
   delta = warp_sum(delta);
+  // A fully masked row (the forward's probabilities are all NaN) gets dS = 0: in the reference, masked_fill's backward
+  // zeroes the gradient of every masked score, so its NaN reaches dV (through P) but neither dQ nor dK.
+  const bool dead = __all_sync(0xffffffffu, all_nan);
 #pragma unroll
   for (int i = 0; i < NV; i++) {
     const int col = 4 * (lane + 32 * i);
     if (col >= p.ldp) continue;
+    if (dead) { *reinterpret_cast<float4*>(drow + col) = make_float4(0.f, 0.f, 0.f, 0.f); continue; }
     const float4 d = dv[i], q = pv[i];
     *reinterpret_cast<float4*>(drow + col) = make_float4(p.scale * q.x * (d.x - delta), p.scale * q.y * (d.y - delta),
                                                          p.scale * q.z * (d.z - delta), p.scale * q.w * (d.w - delta));

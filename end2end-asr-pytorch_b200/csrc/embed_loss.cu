@@ -165,10 +165,9 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restr
   __shared__ float bc[3];
   const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* x = logits + (size_t)row * V;
-  float bv = -INFINITY; int bi = 0x7fffffff; float sum = 0.f;
+  float bv = -INFINITY; int bi = 0x7fffffff;
   for (int c = tid; c < V; c += CE_THREADS) {
     float v = x[c];
-    sum += v;
     if (v > bv) { bv = v; bi = c; }
   }
 #pragma unroll
@@ -177,41 +176,45 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restr
     int oi = __shfl_xor_sync(0xffffffffu, bi, o);
     argmax_combine(bv, bi, ov, oi);
   }
-  sum = warp_sum(sum);
-  if (lane == 0) { sv[warp] = bv; si[warp] = bi; ss[warp] = sum; }
+  if (lane == 0) { sv[warp] = bv; si[warp] = bi; }
   __syncthreads();
   if (tid == 0) {
-    float v = sv[0]; int i = si[0]; float s = ss[0];
-    for (int w = 1; w < CE_THREADS / 32; w++) { argmax_combine(v, i, sv[w], si[w]); s += ss[w]; }
-    bc[0] = v; bc[1] = __int_as_float(i); bc[2] = s;
+    float v = sv[0]; int i = si[0];
+    for (int w = 1; w < CE_THREADS / 32; w++) argmax_combine(v, i, sv[w], si[w]);
+    bc[0] = v; bc[1] = __int_as_float(i);
   }
   __syncthreads();
   const float mx = bc[0];
   const int amax = __float_as_int(bc[1]);
-  const float sumx = bc[2];
-  float e = 0.f;
-  for (int c = tid; c < V; c += CE_THREADS) e += expf(x[c] - mx);
+  // sum of exp and the sum of the logits, both relative to the row maximum: the loss below is then a combination of
+  // terms of the size of the loss itself, whatever offset the logits share (lse - x_g with both ~ 200 would lose 8 bits)
+  float e = 0.f, sd = 0.f;
+  for (int c = tid; c < V; c += CE_THREADS) {
+    const float xs = x[c] - mx;
+    e += expf(xs);
+    sd += xs;
+  }
   e = warp_sum(e);
-  __syncthreads();
-  if (lane == 0) ss[warp] = e;
+  sd = warp_sum(sd);
+  if (lane == 0) { ss[warp] = e; sv[warp] = sd; }
   __syncthreads();
   if (tid == 0) {
-    float t = 0.f;
-    for (int w = 0; w < CE_THREADS / 32; w++) t += ss[w];
-    const float lse = mx + logf(t);
-    row_lse[row] = lse;
+    float t = 0.f, sumd = 0.f;
+    for (int w = 0; w < CE_THREADS / 32; w++) { t += ss[w]; sumd += sv[w]; }
+    const float lt = logf(t);                      // lse - mx
+    row_lse[row] = mx + lt;
     const int64_t g = gold[row];
     float* pr = part + (size_t)row * 3;            // (loss, 1, correct) of this row; zeros for PAD rows
     pr[0] = pr[1] = pr[2] = 0.f;
     if (g != TOK_PAD) {
-      const float xg = x[g];
+      const float xg = x[g] - mx;
       float loss;
       if (eps > 0.f) {
         const float off = eps / (float)V;
         const float wsum = (1.f - eps) + off * (float)(V - 1);
-        loss = wsum * lse - (off * (sumx - xg) + (1.f - eps) * xg);
+        loss = wsum * lt - (off * (sumd - xg) + (1.f - eps) * xg);
       } else {
-        loss = lse - xg;
+        loss = lt - xg;
       }
       pr[0] = loss;
       pr[1] = 1.f;

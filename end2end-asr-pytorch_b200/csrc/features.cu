@@ -18,8 +18,8 @@
 namespace b200asr {
 
 struct FeatWs {               // carve-up of the caller's workspace (all offsets in floats, 16-byte aligned)
-  size_t padded, basis, spec, stats, total;
-  int Lp, rows_per_utt, npad;
+  size_t padded, basis, spec, stats, parts, total;
+  int Lp, rows_per_utt, npad, max_tiles;
 };
 
 static FeatWs feat_ws(int B, int Lmax, int n_fft, int hop) {
@@ -32,7 +32,9 @@ static FeatWs feat_ws(int B, int Lmax, int n_fft, int hop) {
   w.basis = al((size_t)B * w.Lp + n_fft);                    // + n_fft: the last (ignored) rows still read in bounds
   w.spec = w.basis + al((size_t)w.npad * n_fft);
   w.stats = w.spec + al((size_t)B * w.rows_per_utt * w.npad);
-  w.total = w.stats + al((size_t)4 * B);                     // two doubles per utterance
+  w.parts = w.stats + al((size_t)4 * B);                     // two doubles per utterance
+  w.max_tiles = ceil_div(w.rows_per_utt, 32) * ceil_div(n_fft / 2 + 1, 32);   // feat_mag tiles per utterance at Tmax's bound
+  w.total = w.parts + al((size_t)4 * B * w.max_tiles);       // two doubles per tile
   return w;
 }
 
@@ -84,10 +86,12 @@ __global__ void feat_basis_kernel(float* __restrict__ basis, int n_fft, int nb, 
   basis[i] = v;
 }
 
-// spec [B*R, npad] (re | im) -> out [B, nb, Tmax] = log1p(|X|) for t < frames[b] (0 beyond), plus per-utterance sum / sum
-// of squares in double.  32 x 32 (frame x bin) tiles through shared memory so that both sides are coalesced.
+// spec [B*R, npad] (re | im) -> out [B, nb, Tmax] = log1p(|X|) for t < frames[b] (0 beyond), plus the tile's sum / sum of
+// squares in double, written to its own slot parts[b][tile][2] (feat_stats_kernel adds them up in tile order, so the
+// normalisation does not depend on the order in which tiles finish).  32 x 32 (frame x bin) tiles through shared memory so
+// that both sides are coalesced.
 __global__ void feat_mag_kernel(const float* __restrict__ spec, const int* __restrict__ lens, float* __restrict__ out,
-                                double* __restrict__ stats, int* __restrict__ frames_out, int R, int npad, int nb, int Tmax,
+                                double* __restrict__ parts, int* __restrict__ frames_out, int R, int npad, int nb, int Tmax,
                                 int hop) {
   __shared__ float tile[32][33];
   __shared__ double red[2][8];
@@ -118,9 +122,21 @@ __global__ void feat_mag_kernel(const float* __restrict__ spec, const int* __res
   if (threadIdx.x == 0) {
     double a = 0.0, c = 0.0;
     for (int i = 0; i < 8; i++) { a += red[0][i]; c += red[1][i]; }
-    atomicAdd(stats + 2 * b, a);
-    atomicAdd(stats + 2 * b + 1, c);
+    double* o = parts + ((size_t)b * gridDim.x * gridDim.y + (size_t)blockIdx.y * gridDim.x + blockIdx.x) * 2;
+    o[0] = a;
+    o[1] = c;
   }
+}
+
+// stats[b] = (sum, sum of squares) of utterance b: one warp per utterance, lane l takes tiles l, l + 32, ... in order, then a
+// fixed shuffle tree -- the same bits every run
+__global__ void feat_stats_kernel(const double* __restrict__ parts, double* __restrict__ stats, int tiles) {
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const double* p = parts + (size_t)b * tiles * 2;
+  double a = 0.0, c = 0.0;
+  for (int i = lane; i < tiles; i += 32) { a += p[2 * i]; c += p[2 * i + 1]; }
+  for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
+  if (lane == 0) { stats[2 * b] = a; stats[2 * b + 1] = c; }
 }
 
 // spect.add_(-mean); spect.div_(std) with torch's unbiased std (utils/data_loader.py:85-89), valid frames only
@@ -169,6 +185,7 @@ int b200asr_stft_features(const float* wave, const int* lens, float* out, int* f
   float* basis = base + w.basis;
   float* spec = base + w.spec;
   double* stats = (double*)(base + w.stats);
+  double* parts = (double*)(base + w.parts);
   const size_t total = (size_t)B * w.Lp + n_fft;
   feat_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(wave, lens, padded, B, Lmax, w.Lp, n_fft / 2, pad_reflect, total);
   int rc = check_launch("feat_pad");
@@ -183,12 +200,14 @@ int b200asr_stft_features(const float* wave, const int* lens, float* out, int* f
     rc = gemm_tc(padded, true, hop, basis, true, n_fft, spec, w.npad, M, w.npad, n_fft, nullptr, 0, nullptr, 0, precision, st);
   else { set_error("stft_features: unknown precision %d", precision); return B200ASR_BAD_ARG; }
   if (rc) return rc;
-  cudaMemsetAsync(stats, 0, sizeof(double) * 2 * (size_t)B, st);
   dim3 grid(ceil_div(Tmax, 32), ceil_div(nb, 32), B);
-  feat_mag_kernel<<<grid, 256, 0, st>>>(spec, lens, out, stats, frames_out, w.rows_per_utt, w.npad, nb, Tmax, hop);
+  feat_mag_kernel<<<grid, 256, 0, st>>>(spec, lens, out, parts, frames_out, w.rows_per_utt, w.npad, nb, Tmax, hop);
   rc = check_launch("feat_mag");
   if (rc) return rc;
   if (normalize) {
+    feat_stats_kernel<<<B, 32, 0, st>>>(parts, stats, (int)(grid.x * grid.y));
+    rc = check_launch("feat_stats");
+    if (rc) return rc;
     dim3 g2(ceil_div(nb * Tmax, 256), B);
     feat_norm_kernel<<<g2, 256, 0, st>>>(out, stats, lens, nb, Tmax, hop);
     rc = check_launch("feat_norm");
