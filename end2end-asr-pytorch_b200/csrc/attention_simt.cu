@@ -147,7 +147,8 @@ __global__ void __launch_bounds__(256) sdpa_fwd_simt_kernel(AttnP p) {
     const float inv = 1.f / l[i];   // l == 0 (fully masked row) -> inf * 0 = NaN, as the reference's softmax
 #pragma unroll
     for (int jj = 0; jj < DV / 16; jj++) og[(long long)q * p.o_rs + tx + 16 * jj] = o[i][jj] * inv;
-    if (tx == 0 && p.lse) p.lse[((size_t)b * p.H + h) * p.Tq + q] = m[i] + logf(l[i]);
+    // a fully masked row's log-sum-exp is NaN, as the tensor-core kernels write it; the backward reads it as "dead row"
+    if (tx == 0 && p.lse) p.lse[((size_t)b * p.H + h) * p.Tq + q] = m[i] == -INFINITY ? NAN : m[i] + logf(l[i]);
   }
 }
 
@@ -200,6 +201,11 @@ __global__ void __launch_bounds__(256) sdpa_bwd_simt_kernel(AttnP p, const float
   }
   const size_t row_base = ((size_t)b * p.H + h) * p.Tq;
   const int q_start = p.causal ? (k0 / TQ) * TQ : 0;   // queries before the key tile see none of it
+  // a fully masked query row (lse NaN) has a NaN row of P in the reference's masked_fill -> softmax, so dV = P^T dO is NaN
+  // for every key of the head, skipped query tiles included; masked_fill passes its scores no gradient, so dS stays 0
+  bool dead = false;
+  for (int i = tid; i < p.Tq; i += 256) dead |= isnan(p.lse[row_base + i]);
+  dead = __syncthreads_or(dead);
 
   for (int q0 = q_start; q0 < p.Tq; q0 += TQ) {
     __syncthreads();
@@ -313,7 +319,7 @@ __global__ void __launch_bounds__(256) sdpa_bwd_simt_kernel(AttnP p, const float
 #pragma unroll
     for (int jj = 0; jj < DK / 16; jj++) dkg[(long long)key * p.k_rs + tx + 16 * jj] = dka[i][jj];
 #pragma unroll
-    for (int jj = 0; jj < DV / 16; jj++) dvg[(long long)key * p.v_rs + tx + 16 * jj] = dva[i][jj];
+    for (int jj = 0; jj < DV / 16; jj++) dvg[(long long)key * p.v_rs + tx + 16 * jj] = dead ? NAN : dva[i][jj];
   }
 }
 
@@ -353,8 +359,8 @@ static int launch_bwd(const AttnP& p, const float* dout, float* dq, float* dk, f
 
 int sdpa_bwd_simt(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st) {
 #define CASE(a, b) if (p.dk == a && p.dv == b) return launch_bwd<a, b>(p, dout, dq, dk, dv, delta, st)
-  CASE(16, 16); CASE(16, 32); CASE(32, 16); CASE(32, 32); CASE(32, 64); CASE(64, 32); CASE(64, 64);
-  CASE(64, 128); CASE(128, 64); CASE(128, 128);
+  CASE(16, 16); CASE(16, 32); CASE(16, 64); CASE(16, 128); CASE(32, 16); CASE(32, 32); CASE(32, 64); CASE(32, 128);
+  CASE(64, 16); CASE(64, 32); CASE(64, 64); CASE(64, 128); CASE(128, 16); CASE(128, 32); CASE(128, 64); CASE(128, 128);
 #undef CASE
   set_error("sdpa_bwd: (dk=%d, dv=%d) unsupported", p.dk, p.dv);
   return B200ASR_BAD_SHAPE;

@@ -264,6 +264,11 @@ flash_bwd_dkdv_kernel(const AttnP p, const float* __restrict__ dout, const float
 #pragma unroll
   for (int i = 0; i < DV / 8; i++) dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
   const int qstart = p.causal ? k0 : 0;                     // with a causal mask, queries before the key block see none of it
+  // a fully masked query row (lse NaN) has a NaN row of P in the reference's masked_fill -> softmax, so dV = P^T dO is NaN
+  // for every key of the head, skipped query tiles included; masked_fill passes its scores no gradient, so dS stays 0
+  bool dead = false;
+  for (int i = threadIdx.x; i < p.Tq; i += FL_THREADS) dead |= isnan(p.lse[bh * p.Tq + i]);
+  dead = __syncthreads_or(dead);
 
   for (int qt = qstart; qt < p.Tq; qt += FL_ROWS) {
     __syncthreads();
@@ -319,7 +324,8 @@ flash_bwd_dkdv_kernel(const AttnP p, const float* __restrict__ dout, const float
     }
   }
   fl_store_rows<DK>(dk, dk_out, p.k_bs, p.k_hs, p.k_rs, b, h, k0 + warp * 16, p.Tk, g, q, 1.f, 1.f);
-  fl_store_rows<DV>(dv, dv_out, p.v_bs, p.v_hs, p.v_rs, b, h, k0 + warp * 16, p.Tk, g, q, 1.f, 1.f);
+  const float dv_s = dead ? NAN : 1.f;
+  fl_store_rows<DV>(dv, dv_out, p.v_bs, p.v_hs, p.v_rs, b, h, k0 + warp * 16, p.Tk, g, q, dv_s, dv_s);
 }
 
 template <int MODE, int DK, int DV>

@@ -119,8 +119,9 @@ size_t b200asr_add_ln_bwd_ws_bytes(int rows, int d);
  * key_pad   [B,Tk]     1 = key is padding for every query of that utterance (NULL = none)
  * dense_mask[B,Tq,Tk]  1 = masked (the reference's generic mask, broadcast over heads; NULL = none)
  * causal != 0 masks k > q (models/common_layers.py:66-74).  lse is [B,H,Tq] (log-sum-exp of the scaled,
- * masked scores).  A fully-masked row yields NaN exactly like the reference's softmax.
- * dk, dv in {16,32,64,128}.
+ * masked scores).  A fully-masked row yields NaN exactly like the reference's softmax: that row of out and lse
+ * are NaN; in the backward its dq row is 0, dk stays finite and dv is NaN for every key of that (b, h).
+ * dk, dv in {16,32,64,128} (precision 0: every pair, forward and backward).
  */
 int b200asr_sdpa_fwd(const float* q, const float* k, const float* v, long long q_bs, long long q_hs,
                      long long q_rs, long long k_bs, long long k_hs, long long k_rs, long long v_bs,
