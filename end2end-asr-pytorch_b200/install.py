@@ -4,7 +4,8 @@
 
 After this, the reference's own `Transformer` (models/asr/transformer.py), `Trainer` loop
 (trainer/asr/trainer.py) and `test.py` run on libb200asr kernels: module tree, parameter names and checkpoints are
-untouched; only `forward` attributes and the two loss functions are rebound (SURVEY.md §8b).
+untouched; only `forward` attributes, `Decoder.beam_search` and the two loss functions are rebound (SURVEY.md §8b).
+The replaced beam_search stays reachable through original(): LM rescoring still runs it.
 """
 from __future__ import annotations
 
@@ -32,6 +33,7 @@ def install(reference_root: str = None):
         (tr.DecoderLayer, "forward", modules.decoder_layer_forward),
         (tr.Encoder, "forward", modules.encoder_forward),
         (tr.Decoder, "forward", modules.decoder_forward),
+        (tr.Decoder, "beam_search", modules.beam_search),
         (tr.Transformer, "forward", modules.transformer_forward),
         (um, "calculate_loss", metrics.calculate_loss),
         (um, "calculate_metrics", metrics.calculate_metrics),
@@ -52,3 +54,12 @@ def uninstall():
     for obj, name, old in _PATCHED.values():
         setattr(obj, name, old)
     _PATCHED.clear()
+
+
+def original(cls, name):
+    """The reference's own attribute `name` of `cls` (or of the nearest patched base class) that install() replaced, or None."""
+    for c in getattr(cls, "__mro__", (cls,)):
+        hit = _PATCHED.get((id(c), name))
+        if hit is not None:
+            return hit[2]
+    return None

@@ -6,7 +6,9 @@ a composition of libb200asr kernels (ops.py).  The forward bodies are written ag
 exist in BOTH this mirror and the reference classes, so ``install()`` can bind the very same functions onto
 the reference's classes (class-level patch, SURVEY.md §8b).
 
-Not mirrored (out of scope, SURVEY.md §2): beam_search, LM rescoring, the Linear-variant FFN (dead code).
+Decoder.beam_search is mirrored without LM rescoring (beam_decode: batched, KV-cached, selection on the device); with
+lm_rescoring=True it runs the reference's own method.  Not mirrored (out of scope, SURVEY.md §2): LM rescoring, the
+Linear-variant FFN (dead code).
 """
 from __future__ import annotations
 
@@ -253,6 +255,137 @@ def greedy_decode_cached(self, encoder_padded_outputs, steps=300, stop_at_eos=Fa
     return ys
 
 
+PAD_CHAR, SOS_CHAR, EOS_CHAR = "\u00b6", "\u00a7", "\u00a4"     # utils/constant.py:105-107
+
+
+def word_records(id2label, V):
+    """Per-token word-count record of Decoder.beam_search's num_words (models/asr/transformer.py:490-492): with s the label
+    without the PAD/SOS/EOS characters, w = len(s.split()), head / tail = s starts / ends with a non-space character, empty =
+    s is "".  A hypothesis carries (words, tail); appending token v gives words += w - (tail and head), and tail = tail_v
+    unless s is empty -- exactly len(s.split()) of the joined string.  Returns [V] ints w * 8 + head * 4 + tail * 2 + empty."""
+    out = []
+    for v in range(V):
+        try:
+            lab = str(id2label[v])
+        except (KeyError, IndexError):
+            lab = ""
+        s = lab.replace(PAD_CHAR, "").replace(SOS_CHAR, "").replace(EOS_CHAR, "")
+        head = bool(s) and not s[0].isspace()
+        tail = bool(s) and not s[-1].isspace()
+        out.append(len(s.split()) * 8 + head * 4 + tail * 2 + (not s))
+    return out
+
+
+def _word_table(self, V, device):
+    """word_records of self.id2label as a device tensor, built once per label map (and device)."""
+    cached = self.__dict__.get("_b200_word_table")
+    if cached is None or cached[0] is not self.id2label or cached[1] != V or cached[2].device != device:
+        tab = torch.tensor(word_records(self.id2label, V), dtype=torch.int32, device=device)
+        cached = (self.id2label, V, tab)
+        self.__dict__["_b200_word_table"] = cached
+    return cached[2]
+
+
+def _check_beam_positions(self, Te, steps):
+    n = min(int(steps), int(Te))
+    if int(self.trg_max_length) < n:
+        raise ValueError(f"beam search decodes {n} positions (min(steps={steps}, T_e={Te})) but the decoder's positional table "
+                         f"covers trg_max_length={self.trg_max_length}: build the model with tgt_max_len >= {n}")
+
+
+def beam_decode(self, enc, beam_width, nbest=1, c_weight=1.0, steps=300, check_every=8):
+    """Batched, KV-cached Decoder.beam_search (models/asr/transformer.py:396-517, no LM rescoring) on the device.
+
+    All B utterances decode together as B * beam_width rows.  Per step only the new position is projected: its self-attention
+    K/V rows are written by the GEMM into step t of per-layer caches [steps, B*W, H*d], and each row attends over its own
+    history through an index table that the selection kernel reorders (no K/V moves).  Cross-attention runs over the encoder
+    K/V projected once per call (the W queries of an utterance share them).  Selection, the forced EOS at T_e - 1, word counts,
+    final scores and the n-best pools stay on the device; the host reads the live-utterance counter every `check_every` steps.
+
+    Returns device tensors (ids [B, nbest, S + 2] int64: SOS, tokens, EOS, then -1, with S = min(steps, T_e); lengths [B, nbest]
+    int64, 0 where an utterance has fewer than nbest ended hypotheses; score and final_score [B, nbest] fp32, NaN there),
+    ordered by final_score as the reference's stable sort orders them."""
+    B, Te, _ = enc.shape
+    _check_beam_positions(self, Te, steps)
+    dev = enc.device
+    S = min(int(steps), int(Te))
+    W = int(beam_width)
+    R = B * W
+    was_training = self.training
+    self.eval()
+    try:
+        with torch.no_grad():
+            tab = _word_table(self, self.output_linear.weight.shape[0], dev)
+            H = self.layers[0].self_attn.num_heads
+            dk, dv = self.layers[0].self_attn.dim_key, self.layers[0].self_attn.dim_value
+            cross, kc, vc = [], [], []
+            for layer in self.layers:
+                ca = layer.encoder_attn
+                k = ops.LinearFn.apply(enc, ca.key_linear.weight, ca.key_linear.bias).view(B, Te, H, dk).permute(0, 2, 1, 3)
+                v = ops.LinearFn.apply(enc, ca.value_linear.weight, ca.value_linear.bias).view(B, Te, H, dv).permute(0, 2, 1, 3)
+                cross.append((k, v))
+                kc.append(torch.empty((S, R, H * dk), device=dev, dtype=torch.float32))
+                vc.append(torch.empty((S, R, H * dv), device=dev, dtype=torch.float32))
+            buf = ops.BeamBuffers(B, W, int(nbest), S, dev)
+
+            def post(mod, o, x):
+                o = ops.LinearFn.apply(o, mod.output_linear.weight, mod.output_linear.bias).view(R, 1, -1)
+                return ops.AddLNFn.apply(o, x, mod.layer_norm.weight, mod.layer_norm.bias, None, None, mod.layer_norm.eps, 0.0)
+
+            for t in range(S):
+                pe = self.positional_encoding.pe[0, t:t + 1]
+                x = ops.EmbedFn.apply(buf.next_tok, self.trg_embedding.weight, pe, float(self.x_logit_scale), 0.0, PAD_TOKEN)
+                idx = buf.idx[t % 2]
+                for li, layer in enumerate(self.layers):
+                    sa, ca = layer.self_attn, layer.encoder_attn
+                    x2 = x.view(R, -1)
+                    ops.linear_into(x2, sa.key_linear.weight, sa.key_linear.bias, kc[li][t])
+                    ops.linear_into(x2, sa.value_linear.weight, sa.value_linear.bias, vc[li][t])
+                    q = ops.LinearFn.apply(x2, sa.query_linear.weight, sa.query_linear.bias)
+                    x = post(sa, ops.beam_self_attn(q, kc[li], vc[li], idx, W, H, t, 1.0 / float(sa.attention.temperature)), x)
+                    q = ops.LinearFn.apply(x, ca.query_linear.weight, ca.query_linear.bias).view(B, W, H, dk).permute(0, 2, 1, 3)
+                    o = ops.SdpaFn.apply(q, cross[li][0], cross[li][1], None, None, False, 1.0 / float(ca.attention.temperature), 0.0)
+                    x = post(ca, o.permute(0, 2, 1, 3).reshape(R, H * dv), x)
+                    x = _ffn_core(layer.pos_ffn, x)
+                logits = ops.LinearFn.apply(x.view(R, -1), self.output_linear.weight, None)
+                ops.beam_step(buf, logits, tab, t, Te - 1, c_weight)
+                if (t + 1) % check_every == 0 and t + 1 < S and int(buf.n_live.item()) == 0:
+                    break
+            ids, lengths = ops.beam_backtrack(buf)
+    finally:
+        self.train(was_training)
+    return ids, lengths, buf.pool_score, buf.pool_final
+
+
+def beam_search(self, encoder_padded_outputs, beam_width=2, nbest=5, lm_rescoring=False, lm=None, lm_weight=0.1, c_weight=1,
+                prob_weight=1.0):
+    """Decoder.beam_search (models/asr/transformer.py:396-517): flat lists of the n-best yseqs (SOS ... EOS, as int lists) and
+    their strings ("".join of id2label over yseq[1:]), nbest entries per utterance in batch order, fewer where an utterance
+    ends fewer hypotheses (none when it ends none, so Transformer.evaluate falls back to greedy_search).  Decoded by
+    beam_decode with 300 steps; the ids come back in one device-to-host copy.  prob_weight is ignored, as by the reference.
+    lm_rescoring=True runs the reference's own method (kept by install()); the mirror has none."""
+    if lm_rescoring:
+        from .install import original
+        ref = original(type(self), "beam_search")
+        if ref is None:
+            raise NotImplementedError("beam_search with lm_rescoring=True runs the reference's own method; "
+                                      "call b200asr.install() on the reference's Decoder")
+        return ref(self, encoder_padded_outputs, beam_width=beam_width, nbest=nbest, lm_rescoring=lm_rescoring, lm=lm,
+                   lm_weight=lm_weight, c_weight=c_weight, prob_weight=prob_weight)
+    ids, lengths, _, _ = beam_decode(self, encoder_padded_outputs, beam_width, nbest=nbest, c_weight=c_weight, steps=300)
+    both = torch.cat([lengths.unsqueeze(-1), ids], dim=-1).cpu()
+    ys, strs = [], []
+    for b in range(both.shape[0]):
+        for i in range(both.shape[1]):
+            n = int(both[b, i, 0])
+            if n == 0:
+                continue
+            y = both[b, i, 1:1 + n].tolist()
+            ys.append(y)
+            strs.append("".join(self.id2label[t] for t in y[1:]))
+    return ys, strs
+
+
 def _front_end(self, padded_input):
     """CNN front end + flatten of Transformer.forward (models/asr/transformer.py:70-76).
     Returns (feats [B,T',D], cf_order or None)."""
@@ -405,10 +538,13 @@ class Decoder(nn.Module):
     forward = decoder_forward
     greedy_decode_ids = greedy_decode_ids
     greedy_decode_cached = greedy_decode_cached
+    beam_decode = beam_decode
+    beam_search = beam_search
 
 
 class Transformer(nn.Module):
-    """models/asr/transformer.py:16-85 (forward only; evaluate/beam search are out of scope)."""
+    """models/asr/transformer.py:16-85 (forward only; evaluate is not mirrored -- on the installed reference it runs its own
+    body, whose beam_search is Decoder.beam_search above)."""
 
     def __init__(self, encoder, decoder, feat_extractor="vgg_cnn"):
         super().__init__()

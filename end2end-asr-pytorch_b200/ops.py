@@ -262,10 +262,10 @@ def split_weight(w2, prec, need_bwd=True):
     return None
 
 
-def linear_fwd(x2, w, b, relu, prec, w_split=None):
+def linear_fwd(x2, w, b, relu, prec, w_split=None, out=None):
     M, K = x2.shape
     N = w.shape[0]
-    y = torch.empty((M, N), device=x2.device, dtype=torch.float32)
+    y = torch.empty((M, N), device=x2.device, dtype=torch.float32) if out is None else out
     L.check(_lib().b200asr_linear_fwd(L.ptr(x2), L.ptr(w), L.ptr(b), L.ptr(y), M, N, K, int(relu), prec,
                                       L.ptr(w_split.fwd if w_split is not None else None), _stream()), "linear_fwd")
     return y
@@ -377,6 +377,19 @@ def _linear_prec(N, K):
     if prec in _BF16_PRECS and K % 8 != 0:
         prec = L.PREC_TF32X3 if prec == L.PREC_BF16X3 else L.PREC_TF32
     return prec
+
+
+def linear_into(x, w, b, out):
+    """y = x W^T + b written by the GEMM straight into `out`, a contiguous fp32 tensor of x.rows x N elements (one step of a
+    K/V cache); no autograd."""
+    _need_cuda(x, w, b, out)
+    w2 = _f32c(w.reshape(w.shape[0], -1))
+    x2 = _f32c(x).reshape(-1, w2.shape[1])
+    if not (out.is_contiguous() and out.dtype == torch.float32 and out.numel() == x2.shape[0] * w2.shape[0]):
+        raise RuntimeError("linear_into: out must be a contiguous fp32 tensor of rows x N elements")
+    prec = _linear_prec(w2.shape[0], w2.shape[1])
+    linear_fwd(x2, w2, b, False, prec, split_weight(w2, prec, need_bwd=False), out=out)
+    return out
 
 
 class LinearFn(torch.autograd.Function):
@@ -1214,6 +1227,68 @@ def greedy_step(logits: torch.Tensor, ys: torch.Tensor, finished: torch.Tensor, 
     L.check(_lib().b200asr_greedy_step(L.ptr(x), L.ptr(tok), L.ptr(ys), L.ptr(finished), finished.data_ptr() + 4 * B, B, V, int(t),
                                        ys.shape[1], _stream()), "greedy_step")
     return tok
+
+
+class BeamBuffers:
+    """Device state of one batched beam search over B utterances of W slots (include/b200asr.h b200asr_beam_step): slot 0 of
+    every utterance starts live with score 0 and the SOS token, the others dead; the n-best pools start empty."""
+
+    def __init__(self, B, W, nbest, steps, device):
+        R = B * W
+        self.B, self.W, self.nbest, self.steps = B, W, nbest, steps
+        first = torch.arange(R, device=device) % W == 0
+        self.score = torch.where(first, 0.0, float("-inf")).to(torch.float32)
+        self.state = torch.zeros((R, 4), device=device, dtype=torch.int32)      # live, words, tail, kept index
+        self.state[:, 0] = first.to(torch.int32)
+        self.state[:, 3] = -1
+        self.next_tok = torch.where(first, 1, 0).to(torch.long).view(R, 1)       # SOS; PAD in dead slots
+        self.idx = [torch.empty((R, steps + 1), device=device, dtype=torch.int32) for _ in range(2)]
+        self.idx[0][:, 0] = (torch.arange(R, device=device) % W).to(torch.int32)
+        self.hist_tok = torch.empty((steps, R), device=device, dtype=torch.int32)
+        self.hist_par = torch.empty((steps, R), device=device, dtype=torch.int32)
+        self.pool_score = torch.full((B, nbest), float("nan"), device=device, dtype=torch.float32)     # NaN: no entry
+        self.pool_final = torch.full((B, nbest), float("nan"), device=device, dtype=torch.float32)
+        self.pool_ref = torch.full((B, nbest), -1, device=device, dtype=torch.int32)
+        self.pool_n = torch.zeros(B, device=device, dtype=torch.int32)
+        self.n_live = torch.full((1,), B, device=device, dtype=torch.int32)
+
+
+def beam_step(buf: BeamBuffers, logits: torch.Tensor, word_tab: torch.Tensor, t: int, t_eos: int, c_weight: float):
+    """Step t of the beam search on the device: selection, EOS, word counts, n-best pools, compaction and the index table of
+    step t + 1 (written into buf.idx[(t + 1) % 2] from buf.idx[t % 2])."""
+    _need_cuda(logits, word_tab)
+    x = _f32c(logits.detach())
+    V = x.shape[1]
+    L.check(_lib().b200asr_beam_step(L.ptr(x), L.ptr(word_tab), buf.B, buf.W, V, int(t), int(t_eos), buf.steps, buf.nbest,
+                                     float(c_weight), L.ptr(buf.score), L.ptr(buf.state), L.ptr(buf.next_tok),
+                                     L.ptr(buf.idx[t % 2]), L.ptr(buf.idx[(t + 1) % 2]), buf.steps + 1, L.ptr(buf.hist_tok),
+                                     L.ptr(buf.hist_par), L.ptr(buf.pool_score), L.ptr(buf.pool_final), L.ptr(buf.pool_ref),
+                                     L.ptr(buf.pool_n), L.ptr(buf.n_live), _stream()), "beam_step")
+
+
+def beam_self_attn(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, idx: torch.Tensor, W: int, H: int, t: int,
+                   scale: float) -> torch.Tensor:
+    """Single-query attention of every beam row over its history 0..t: q [R, H*dk]; caches [steps, R, H*d]; idx [R, stride]."""
+    _need_cuda(q, k_cache, v_cache, idx)
+    R = q.shape[0]
+    dk, dv = k_cache.shape[2] // H, v_cache.shape[2] // H
+    q = _f32c(q)
+    if not (k_cache.is_contiguous() and v_cache.is_contiguous() and idx.is_contiguous() and idx.dtype == torch.int32):
+        raise RuntimeError("beam_self_attn: caches and the index table must be contiguous (index table int32)")
+    out = torch.empty((R, H * dv), device=q.device, dtype=torch.float32)
+    L.check(_lib().b200asr_beam_self_attn(L.ptr(q), L.ptr(k_cache), L.ptr(v_cache), L.ptr(idx), L.ptr(out), R, H, W, dk, dv,
+                                          int(t), idx.shape[1], float(scale), _stream()), "beam_self_attn")
+    return out
+
+
+def beam_backtrack(buf: BeamBuffers):
+    """(ids [B, nbest, steps + 2] int64, lengths [B, nbest] int64) of the pooled hypotheses; see b200asr_beam_backtrack."""
+    ids = torch.empty((buf.B, buf.nbest, buf.steps + 2), device=buf.score.device, dtype=torch.long)
+    lengths = torch.empty((buf.B, buf.nbest), device=buf.score.device, dtype=torch.long)
+    L.check(_lib().b200asr_beam_backtrack(L.ptr(buf.hist_tok), L.ptr(buf.hist_par), L.ptr(buf.pool_ref), L.ptr(buf.pool_n),
+                                          L.ptr(ids), L.ptr(lengths), buf.B, buf.W, buf.nbest, buf.steps, _stream()),
+            "beam_backtrack")
+    return ids, lengths
 
 
 class CrossEntropyFn(torch.autograd.Function):

@@ -330,6 +330,39 @@ int b200asr_argmax_rows(const float* logits, int64_t* out, int rows, int V, b200
  * loop can stop early (SURVEY.md 8f row 3: on-device EOS stop). */
 int b200asr_greedy_step(const float* logits, int64_t* next_tok, int64_t* ys, int* finished, int* n_finished, int B, int V,
                         int t, int steps, b200asr_stream_t stream);
+/* Beam search (Decoder.beam_search without LM rescoring, models/asr/transformer.py:396-517) for B utterances of W slots each;
+ * row r = b * W + s.  Replaces, per step t: the log_softmax + topk of every hypothesis (:454-455), the scoring and the
+ * stable sorted(...)[:W] pruning (:458-466), the forced EOS at t == T_e - 1 (:471-473), the EOS test, word count and
+ * final_score (:476-495) and the ended_hyps list with its final sort (:504-506).
+ *   logits [B*W, V] fp32.  word_tab [V]: w * 8 + head * 4 + tail * 2 + empty per token (w = words of the label with the
+ *   PAD/SOS/EOS characters removed, head/tail = it starts/ends with a non-space character, empty = nothing is left).
+ *   score [B*W] fp32 and state [B*W][4] int32 (live, words, tail, kept index of the slot at the previous step, -1 before
+ *   step 0) are read and rewritten: survivors are compacted into slots 0..n-1 in kept order, dead slots get live = 0,
+ *   score = -inf.  next_tok [B*W] int64: the next input token (PAD for dead slots).
+ *   idx_cur / idx_nxt [B*W][idx_stride] int32 (idx_stride >= t + 2): entry p of a row is the slot of the utterance whose
+ *   K/V cache row at step p holds position p of that hypothesis.  idx_nxt rows get the parent's entries 0..t and their own
+ *   slot at t + 1; dead rows point at themselves.
+ *   hist_tok / hist_par [steps][B*W] int32: row b*W + k of step t holds the k-th kept candidate's token and its parent's kept
+ *   index at step t - 1.  pool_score / pool_final [B][nbest] fp32, pool_ref [B][nbest] int32 ((t * W + k) * 2 + forced) and
+ *   pool_n [B] (zero-initialised): the top-nbest ended hypotheses by final_score, stable (a later entry never displaces an
+ *   equal one).  *n_live (initialised to B) counts the utterances that still have live hypotheses.
+ * Scores are fp32 like the reference's; final_score = score + (float)(sqrt(words) * c_weight).  Ties: topk to the lower
+ * token id, the merge to the earlier parent, then the better rank.  1 <= W <= 32, W <= V, 1 <= nbest <= 32; otherwise
+ * B200ASR_BAD_SHAPE and nothing is written. */
+int b200asr_beam_step(const float* logits, const int32_t* word_tab, int B, int W, int V, int t, int t_eos, int steps, int nbest,
+                      double c_weight, float* score, int32_t* state, int64_t* next_tok, const int32_t* idx_cur,
+                      int32_t* idx_nxt, int idx_stride, int32_t* hist_tok, int32_t* hist_par, float* pool_score,
+                      float* pool_final, int32_t* pool_ref, int32_t* pool_n, int32_t* n_live, b200asr_stream_t stream);
+/* Single-query self-attention of beam row r over positions 0..t (the reference re-decodes the whole prefix under a causal
+ * mask, :444-452; its last position sees every earlier one, so no mask).  q [R, H*dk], out [R, H*dv]; k_cache / v_cache
+ * [steps][R][H*dk | H*dv]: position p of row r is read from step p, row (r - r % W) + idx[r * idx_stride + p].  Exact fp32.
+ * dk, dv in {16, 32, 64, 128}; t < 8192. */
+int b200asr_beam_self_attn(const float* q, const float* k_cache, const float* v_cache, const int32_t* idx, float* out, int R,
+                           int H, int W, int dk, int dv, int t, int idx_stride, float scale, b200asr_stream_t stream);
+/* The n-best yseqs (:500-515): ids [B][nbest][steps + 2] int64 = SOS, the tokens along hist_par from each pool entry, EOS if
+ * it was forced, then -1; lengths [B][nbest] int64 (0: no hypothesis). */
+int b200asr_beam_backtrack(const int32_t* hist_tok, const int32_t* hist_par, const int32_t* pool_ref, const int32_t* pool_n,
+                           int64_t* ids, int64_t* lengths, int B, int W, int nbest, int steps, b200asr_stream_t stream);
 int b200asr_ce_fwd(const float* logits, const int64_t* gold, float* row_lse, float* stats, int rows, int V,
                    float smoothing, b200asr_stream_t stream);
 /* stats[3] = stats[0] / stats[1] (the reference's mean loss), stats[4] = 1 / stats[1];
