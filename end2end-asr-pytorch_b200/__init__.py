@@ -9,13 +9,13 @@ from .config import ASRConfig, BASELINE_CONFIGS
 from .features import spectrogram_batch
 from .install import install, uninstall
 from .metrics import calculate_loss, calculate_metrics, loss_and_stats
-from .modules import (Decoder, DecoderLayer, Encoder, EncoderLayer, MultiHeadAttention, PositionalEncoding,
-                      PositionwiseFeedForwardWithConv, ScaledDotProductAttention, Transformer, build_model)
+from .modules import (LM, Decoder, DecoderLayer, Encoder, EncoderLayer, MultiHeadAttention, PositionalEncoding,
+                      PositionwiseFeedForwardWithConv, RNNModel, ScaledDotProductAttention, Transformer, build_model)
 from .ops import config as precision, manual_seed
 from .optim import FlatParams, FusedAdam, NoamOpt
 from .parallel import DataParallelStep, HostBatchPrefetcher, shard_batch
 
 __all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "calculate_loss", "calculate_metrics",
            "loss_and_stats", "Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
-           "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model",
+           "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model", "RNNModel", "LM",
            "precision", "manual_seed", "spectrogram_batch", "FlatParams", "FusedAdam", "NoamOpt", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]

@@ -90,6 +90,13 @@ SIGNATURES = {
     "b200asr_beam_step": (_i, [_vp, _vp] + [_i] * 7 + [C.c_double, _vp, _vp, _vp, _vp, _vp, _i] + [_vp] * 7 + [_vp]),
     "b200asr_beam_self_attn": (_i, [_vp] * 5 + [_i] * 7 + [_f, _vp]),
     "b200asr_beam_backtrack": (_i, [_vp] * 6 + [_i] * 4 + [_vp]),
+    "b200asr_beam_step_log": (_i, [_vp, _vp] + [_i] * 7 + [C.c_double, _vp, _vp, _vp, _vp, _vp, _i] + [_vp] * 7 + [_vp] * 3 +
+                              [_i, _vp]),
+    "b200asr_beam_backtrack_packed": (_i, [_vp] * 4 + [_i, _vp, _vp, _i, _vp, _i, _i, _i, _vp]),
+    "b200asr_lstm_prepare": (_i, [_vp] * 4 + [_i, _i] + [_vp] * 3 + [_vp]),
+    "b200asr_lstm_layer_fwd": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "b200asr_lm_nll": (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp]),
+    "b200asr_lm_seq_sum": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
     "b200asr_ce_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "b200asr_ce_finalize": (_i, [_vp, _vp, _i, _vp]),
     "b200asr_ce_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _f, _vp, _vp, _vp]),

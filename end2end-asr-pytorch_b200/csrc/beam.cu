@@ -33,7 +33,8 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_step_kernel(
     double c_weight, float* __restrict__ score, int32_t* __restrict__ state, int64_t* __restrict__ next_tok,
     const int32_t* __restrict__ idx_cur, int32_t* __restrict__ idx_nxt, int idx_stride, int32_t* __restrict__ hist_tok,
     int32_t* __restrict__ hist_par, float* __restrict__ pool_score, float* __restrict__ pool_final,
-    int32_t* __restrict__ pool_ref, int32_t* __restrict__ pool_n, int32_t* __restrict__ n_live, int BW) {
+    int32_t* __restrict__ pool_ref, int32_t* __restrict__ pool_n, int32_t* __restrict__ n_live, int BW,
+    int32_t* __restrict__ end_ref, float* __restrict__ end_score, int32_t* __restrict__ end_n, int end_cap) {
   __shared__ float c_val[BEAM_MAX * BEAM_MAX];     // candidate scores, index parent * W + rank
   __shared__ int c_tok[BEAM_MAX * BEAM_MAX];
   __shared__ float p_score[BEAM_MAX];
@@ -119,13 +120,20 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_step_kernel(
       hist_tok[(size_t)t * BW + row0 + k] = tok;
       hist_par[(size_t)t * BW + row0 + k] = p_state[j][3];
       if (forced || tok == TOK_EOS_ID) {
+        const int ref = ((t * W + k) << 1) | (forced ? 1 : 0);
+        if (end_ref) {                         // end log: every ended hypothesis, in insertion order
+          const int e = end_n[b];
+          end_ref[(size_t)b * end_cap + e] = ref;
+          end_score[(size_t)b * end_cap + e] = sc;
+          end_n[b] = e + 1;
+        }
         const float fs = sc + (float)(sqrt((double)words) * c_weight);
         int pos = 0;                           // stable: after every entry with an equal or larger final score
         while (pos < pn && !(fs > pf[pos])) pos++;
         if (pos < nbest) {
           const int last = pn < nbest ? pn : nbest - 1;
           for (int q = last; q > pos; q--) { ps[q] = ps[q - 1]; pf[q] = pf[q - 1]; pr[q] = pr[q - 1]; }
-          ps[pos] = sc; pf[pos] = fs; pr[pos] = ((t * W + k) << 1) | (forced ? 1 : 0);
+          ps[pos] = sc; pf[pos] = fs; pr[pos] = ref;
           if (pn < nbest) pn++;
         }
       } else {
@@ -221,19 +229,23 @@ __global__ void __launch_bounds__(128) beam_self_attn_kernel(const float* __rest
     if (a * 32 + lane < DV) o[a * 32 + lane] = acc[a] * inv;
 }
 
-// One thread per (utterance, pool entry): SOS, the tokens along the back-pointers, the forced EOS if any, then -1.
+// One thread per ended hypothesis: SOS, the tokens along the back-pointers, the forced EOS if any.  Entry i of utterance b's
+// list is refs[b * cap + i] ((t * W + k) * 2 + forced; valid for i < counts[b]).  Fixed-stride output (entries == nullptr):
+// thread e = b * cap + i writes row e of ids [B * cap][steps + 2], -1 after the hypothesis, and lengths[e] (0: no entry).
+// Packed output: thread j writes the t + 2 (+ 1 if forced) ids of entry entries[j] from ids + off[j].
 __global__ void beam_backtrack_kernel(const int32_t* __restrict__ hist_tok, const int32_t* __restrict__ hist_par,
-                                      const int32_t* __restrict__ pool_ref, const int32_t* __restrict__ pool_n,
-                                      int64_t* __restrict__ ids, int64_t* __restrict__ lengths, int B, int W, int nbest,
-                                      int steps) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= B * nbest) return;
-  const int b = e / nbest, i = e - b * nbest;
+                                      const int32_t* __restrict__ refs, const int32_t* __restrict__ counts, int cap,
+                                      const int64_t* __restrict__ entries, const int64_t* __restrict__ off, int n,
+                                      int64_t* __restrict__ ids, int64_t* __restrict__ lengths, int B, int W, int steps) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int e = entries ? (int)entries[j] : j;
+  const int b = e / cap, i = e - b * cap;
   const int L = steps + 2;
-  int64_t* y = ids + (size_t)e * L;
+  int64_t* y = entries ? ids + off[j] : ids + (size_t)e * L;
   int len = 0;
-  if (i < pool_n[b]) {
-    const int ref = pool_ref[e], forced = ref & 1;
+  if (i < counts[b]) {
+    const int ref = refs[e], forced = ref & 1;
     const int t = (ref >> 1) / W;
     int k = (ref >> 1) - t * W;
     len = t + 2 + forced;
@@ -245,6 +257,7 @@ __global__ void beam_backtrack_kernel(const int32_t* __restrict__ hist_tok, cons
     }
     if (forced) y[t + 2] = TOK_EOS_ID;
   }
+  if (entries) return;
   for (int p = len; p < L; p++) y[p] = -1;
   lengths[e] = len;
 }
@@ -278,12 +291,11 @@ static int launch_self_attn_dv(int dv, const float* q, const float* kc, const fl
 
 using namespace b200asr;
 
-extern "C" {
-
-int b200asr_beam_step(const float* logits, const int32_t* word_tab, int B, int W, int V, int t, int t_eos, int steps, int nbest,
-                      double c_weight, float* score, int32_t* state, int64_t* next_tok, const int32_t* idx_cur,
-                      int32_t* idx_nxt, int idx_stride, int32_t* hist_tok, int32_t* hist_par, float* pool_score,
-                      float* pool_final, int32_t* pool_ref, int32_t* pool_n, int32_t* n_live, b200asr_stream_t stream) {
+static int beam_step_impl(const float* logits, const int32_t* word_tab, int B, int W, int V, int t, int t_eos, int steps,
+                          int nbest, double c_weight, float* score, int32_t* state, int64_t* next_tok, const int32_t* idx_cur,
+                          int32_t* idx_nxt, int idx_stride, int32_t* hist_tok, int32_t* hist_par, float* pool_score,
+                          float* pool_final, int32_t* pool_ref, int32_t* pool_n, int32_t* n_live, int32_t* end_ref,
+                          float* end_score, int32_t* end_n, int end_cap, b200asr_stream_t stream) {
   B200_REQUIRE(logits && word_tab && score && state && next_tok && idx_cur && idx_nxt && hist_tok && hist_par && pool_score &&
                pool_final && pool_ref && pool_n && n_live, B200ASR_BAD_ARG, "beam_step: null pointer");
   B200_REQUIRE(idx_cur != idx_nxt, B200ASR_BAD_ARG, "beam_step: idx_cur and idx_nxt must be different buffers");
@@ -295,8 +307,33 @@ int b200asr_beam_step(const float* logits, const int32_t* word_tab, int B, int W
                idx_stride);
   beam_step_kernel<<<B, BEAM_THREADS, 0, (cudaStream_t)stream>>>(logits, word_tab, W, V, t, t_eos, nbest, c_weight, score, state,
                                                                  next_tok, idx_cur, idx_nxt, idx_stride, hist_tok, hist_par,
-                                                                 pool_score, pool_final, pool_ref, pool_n, n_live, B * W);
+                                                                 pool_score, pool_final, pool_ref, pool_n, n_live, B * W, end_ref,
+                                                                 end_score, end_n, end_cap);
   return check_launch("beam_step");
+}
+
+extern "C" {
+
+int b200asr_beam_step(const float* logits, const int32_t* word_tab, int B, int W, int V, int t, int t_eos, int steps, int nbest,
+                      double c_weight, float* score, int32_t* state, int64_t* next_tok, const int32_t* idx_cur,
+                      int32_t* idx_nxt, int idx_stride, int32_t* hist_tok, int32_t* hist_par, float* pool_score,
+                      float* pool_final, int32_t* pool_ref, int32_t* pool_n, int32_t* n_live, b200asr_stream_t stream) {
+  return beam_step_impl(logits, word_tab, B, W, V, t, t_eos, steps, nbest, c_weight, score, state, next_tok, idx_cur, idx_nxt,
+                        idx_stride, hist_tok, hist_par, pool_score, pool_final, pool_ref, pool_n, n_live, nullptr, nullptr,
+                        nullptr, 0, stream);
+}
+
+int b200asr_beam_step_log(const float* logits, const int32_t* word_tab, int B, int W, int V, int t, int t_eos, int steps,
+                          int nbest, double c_weight, float* score, int32_t* state, int64_t* next_tok, const int32_t* idx_cur,
+                          int32_t* idx_nxt, int idx_stride, int32_t* hist_tok, int32_t* hist_par, float* pool_score,
+                          float* pool_final, int32_t* pool_ref, int32_t* pool_n, int32_t* n_live, int32_t* end_ref,
+                          float* end_score, int32_t* end_n, int end_cap, b200asr_stream_t stream) {
+  B200_REQUIRE(end_ref && end_score && end_n, B200ASR_BAD_ARG, "beam_step_log: null pointer");
+  B200_REQUIRE(end_cap >= W * steps && W >= 1, B200ASR_BAD_SHAPE, "beam_step_log: end_cap=%d must be >= W * steps = %d", end_cap,
+               W * steps);
+  return beam_step_impl(logits, word_tab, B, W, V, t, t_eos, steps, nbest, c_weight, score, state, next_tok, idx_cur, idx_nxt,
+                        idx_stride, hist_tok, hist_par, pool_score, pool_final, pool_ref, pool_n, n_live, end_ref, end_score,
+                        end_n, end_cap, stream);
 }
 
 int b200asr_beam_self_attn(const float* q, const float* k_cache, const float* v_cache, const int32_t* idx, float* out, int R,
@@ -322,9 +359,22 @@ int b200asr_beam_backtrack(const int32_t* hist_tok, const int32_t* hist_par, con
   B200_REQUIRE(hist_tok && hist_par && pool_ref && pool_n && ids && lengths, B200ASR_BAD_ARG, "beam_backtrack: null pointer");
   B200_REQUIRE(B >= 1 && W >= 1 && W <= BEAM_MAX && nbest >= 1 && nbest <= BEAM_MAX && steps >= 1, B200ASR_BAD_SHAPE,
                "beam_backtrack: B=%d W=%d nbest=%d steps=%d", B, W, nbest, steps);
-  beam_backtrack_kernel<<<ceil_div(B * nbest, 128), 128, 0, (cudaStream_t)stream>>>(hist_tok, hist_par, pool_ref, pool_n, ids,
-                                                                                    lengths, B, W, nbest, steps);
+  beam_backtrack_kernel<<<ceil_div(B * nbest, 128), 128, 0, (cudaStream_t)stream>>>(
+      hist_tok, hist_par, pool_ref, pool_n, nbest, nullptr, nullptr, B * nbest, ids, lengths, B, W, steps);
   return check_launch("beam_backtrack");
+}
+
+int b200asr_beam_backtrack_packed(const int32_t* hist_tok, const int32_t* hist_par, const int32_t* end_ref, const int32_t* end_n,
+                                  int end_cap, const int64_t* entries, const int64_t* offsets, int n, int64_t* ids, int B, int W,
+                                  int steps, b200asr_stream_t stream) {
+  B200_REQUIRE(hist_tok && hist_par && end_ref && end_n && entries && offsets && ids, B200ASR_BAD_ARG,
+               "beam_backtrack_packed: null pointer");
+  B200_REQUIRE(B >= 1 && W >= 1 && W <= BEAM_MAX && steps >= 1 && end_cap >= 1 && n >= 0, B200ASR_BAD_SHAPE,
+               "beam_backtrack_packed: B=%d W=%d steps=%d end_cap=%d n=%d", B, W, steps, end_cap, n);
+  if (n == 0) return B200ASR_OK;
+  beam_backtrack_kernel<<<ceil_div(n, 128), 128, 0, (cudaStream_t)stream>>>(hist_tok, hist_par, end_ref, end_n, end_cap, entries,
+                                                                            offsets, n, ids, nullptr, B, W, steps);
+  return check_launch("beam_backtrack_packed");
 }
 
 }  // extern "C"

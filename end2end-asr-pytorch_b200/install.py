@@ -5,7 +5,7 @@
 After this, the reference's own `Transformer` (models/asr/transformer.py), `Trainer` loop
 (trainer/asr/trainer.py) and `test.py` run on libb200asr kernels: module tree, parameter names and checkpoints are
 untouched; only `forward` attributes, `Decoder.beam_search` and the two loss functions are rebound (SURVEY.md §8b).
-The replaced beam_search stays reachable through original(): LM rescoring still runs it.
+The replaced beam_search stays reachable through original(): LM rescoring with an LM other than an LSTM LM still runs it.
 """
 from __future__ import annotations
 

@@ -6,13 +6,17 @@ a composition of libb200asr kernels (ops.py).  The forward bodies are written ag
 exist in BOTH this mirror and the reference classes, so ``install()`` can bind the very same functions onto
 the reference's classes (class-level patch, SURVEY.md §8b).
 
-Decoder.beam_search is mirrored without LM rescoring (beam_decode: batched, KV-cached, selection on the device); with
-lm_rescoring=True it runs the reference's own method.  Not mirrored (out of scope, SURVEY.md §2): LM rescoring, the
-Linear-variant FFN (dead code).
+Decoder.beam_search is mirrored (beam_decode: batched, KV-cached, selection on the device), including lm_rescoring=True
+with an LSTM language model (RNNModel / LM below, or the reference's utils/lstm_utils.LM); with any other LM object it runs
+the reference's own method.  Not mirrored (out of scope, SURVEY.md §2): the Linear-variant FFN (dead code).
 """
 from __future__ import annotations
 
 import math
+import time
+import unicodedata
+
+import numpy as np
 
 import torch
 import torch.nn as nn
@@ -293,8 +297,8 @@ def _check_beam_positions(self, Te, steps):
                          f"covers trg_max_length={self.trg_max_length}: build the model with tgt_max_len >= {n}")
 
 
-def beam_decode(self, enc, beam_width, nbest=1, c_weight=1.0, steps=300, check_every=8):
-    """Batched, KV-cached Decoder.beam_search (models/asr/transformer.py:396-517, no LM rescoring) on the device.
+def beam_decode(self, enc, beam_width, nbest=1, c_weight=1.0, steps=300, check_every=8, lm=None, lm_weight=0.1):
+    """Batched, KV-cached Decoder.beam_search (models/asr/transformer.py:396-517) on the device.
 
     All B utterances decode together as B * beam_width rows.  Per step only the new position is projected: its self-attention
     K/V rows are written by the GEMM into step t of per-layer caches [steps, B*W, H*d], and each row attends over its own
@@ -302,11 +306,20 @@ def beam_decode(self, enc, beam_width, nbest=1, c_weight=1.0, steps=300, check_e
     K/V projected once per call (the W queries of an utterance share them).  Selection, the forced EOS at T_e - 1, word counts,
     final scores and the n-best pools stay on the device; the host reads the live-utterance counter every `check_every` steps.
 
+    lm: an LSTM language model (b200asr.LM, or the reference's utils/lstm_utils.LM) rescores every ended hypothesis as
+    lm_rescoring=True does (transformer.py:473-481): the selection is unchanged, the device keeps a log of every ended
+    hypothesis, and the n-best are ranked by score + lm_weight * lm_score + sqrt(num_words) * c_weight (see lm_rescore).
+
     Returns device tensors (ids [B, nbest, S + 2] int64: SOS, tokens, EOS, then -1, with S = min(steps, T_e); lengths [B, nbest]
     int64, 0 where an utterance has fewer than nbest ended hypotheses; score and final_score [B, nbest] fp32, NaN there),
     ordered by final_score as the reference's stable sort orders them."""
     B, Te, _ = enc.shape
     _check_beam_positions(self, Te, steps)
+    lm_parts = None
+    if lm is not None:
+        lm_parts = lstm_lm_parts(lm)
+        if lm_parts is None:
+            raise TypeError("beam_decode: lm must be an LSTM language model (b200asr.LM or utils/lstm_utils.LM)")
     dev = enc.device
     S = min(int(steps), int(Te))
     W = int(beam_width)
@@ -327,6 +340,7 @@ def beam_decode(self, enc, beam_width, nbest=1, c_weight=1.0, steps=300, check_e
                 kc.append(torch.empty((S, R, H * dk), device=dev, dtype=torch.float32))
                 vc.append(torch.empty((S, R, H * dv), device=dev, dtype=torch.float32))
             buf = ops.BeamBuffers(B, W, int(nbest), S, dev)
+            log = ops.EndLog(B, W, S, dev) if lm_parts is not None else None
 
             def post(mod, o, x):
                 o = ops.LinearFn.apply(o, mod.output_linear.weight, mod.output_linear.bias).view(R, 1, -1)
@@ -348,9 +362,14 @@ def beam_decode(self, enc, beam_width, nbest=1, c_weight=1.0, steps=300, check_e
                     x = post(ca, o.permute(0, 2, 1, 3).reshape(R, H * dv), x)
                     x = _ffn_core(layer.pos_ffn, x)
                 logits = ops.LinearFn.apply(x.view(R, -1), self.output_linear.weight, None)
-                ops.beam_step(buf, logits, tab, t, Te - 1, c_weight)
+                if log is None:
+                    ops.beam_step(buf, logits, tab, t, Te - 1, c_weight)
+                else:
+                    ops.beam_step_log(buf, log, logits, tab, t, Te - 1, c_weight)
                 if (t + 1) % check_every == 0 and t + 1 < S and int(buf.n_live.item()) == 0:
                     break
+            if log is not None:
+                return lm_rescore(self, buf, log, lm_parts, lm_weight, c_weight)
             ids, lengths = ops.beam_backtrack(buf)
     finally:
         self.train(was_training)
@@ -363,16 +382,18 @@ def beam_search(self, encoder_padded_outputs, beam_width=2, nbest=5, lm_rescorin
     their strings ("".join of id2label over yseq[1:]), nbest entries per utterance in batch order, fewer where an utterance
     ends fewer hypotheses (none when it ends none, so Transformer.evaluate falls back to greedy_search).  Decoded by
     beam_decode with 300 steps; the ids come back in one device-to-host copy.  prob_weight is ignored, as by the reference.
-    lm_rescoring=True runs the reference's own method (kept by install()); the mirror has none."""
-    if lm_rescoring:
+    lm_rescoring=True with an LSTM LM (b200asr.LM or utils/lstm_utils.LM) rescores on the device; with any other `lm` it runs
+    the reference's own method (kept by install())."""
+    if lm_rescoring and lstm_lm_parts(lm) is None:
         from .install import original
         ref = original(type(self), "beam_search")
         if ref is None:
-            raise NotImplementedError("beam_search with lm_rescoring=True runs the reference's own method; "
-                                      "call b200asr.install() on the reference's Decoder")
+            raise NotImplementedError("beam_search with lm_rescoring=True and a language model other than an LSTM LM runs the "
+                                      "reference's own method; call b200asr.install() on the reference's Decoder")
         return ref(self, encoder_padded_outputs, beam_width=beam_width, nbest=nbest, lm_rescoring=lm_rescoring, lm=lm,
                    lm_weight=lm_weight, c_weight=c_weight, prob_weight=prob_weight)
-    ids, lengths, _, _ = beam_decode(self, encoder_padded_outputs, beam_width, nbest=nbest, c_weight=c_weight, steps=300)
+    ids, lengths, _, _ = beam_decode(self, encoder_padded_outputs, beam_width, nbest=nbest, c_weight=c_weight, steps=300,
+                                     lm=lm if lm_rescoring else None, lm_weight=lm_weight)
     both = torch.cat([lengths.unsqueeze(-1), ids], dim=-1).cpu()
     ys, strs = [], []
     for b in range(both.shape[0]):
@@ -384,6 +405,144 @@ def beam_search(self, encoder_padded_outputs, beam_width=2, nbest=5, lm_rescorin
             ys.append(y)
             strs.append("".join(self.id2label[t] for t in y[1:]))
     return ys, strs
+
+
+# ------------------------------------------------------------------------------------------------ LM rescoring
+def _has_letter_lo(word):
+    """data/helper.py:33-54: a word is "Chinese" when one of its characters has Unicode category Lo."""
+    return any(unicodedata.category(ch) == "Lo" for ch in word)
+
+
+def lm_string(yseq, id2label) -> str:
+    """The string calculate_lm_score (utils/lstm_utils.py:9-44) scores for a hypothesis: the joined labels without the
+    PAD/SOS/EOS characters, "  " -> " " once; the " "-separated pieces grouped into runs of one kind ("Chinese" or not,
+    data/helper.py:56-99; the pieces of a run rejoined with " ", empty pieces only after a non-empty one); then every
+    character of a Chinese run -- spaces included -- is its own word, a non-Chinese run is one item, items are joined with
+    " " (an empty item adds nothing while the result is still empty), and "  " -> " " is applied twice."""
+    s = "".join(id2label[t] for t in yseq).replace(PAD_CHAR, "").replace(SOS_CHAR, "").replace(EOS_CHAR, "").replace("  ", " ")
+    runs = []                                   # [chinese, text]
+    for piece in s.split(" "):
+        kind = _has_letter_lo(piece)
+        if runs and runs[-1][0] == kind:
+            runs[-1][1] = runs[-1][1] + " " + piece if runs[-1][1] else piece
+        else:
+            runs.append([kind, piece])
+    out = ""
+    for kind, text in runs:
+        for item in (text if kind else (text,)):
+            out = out + " " + item if out else item
+    return out.replace("  ", " ").replace("  ", " ")
+
+
+def lm_word_ids(string, word2idx):
+    """LM.seq_to_tensor (utils/lstm_utils.py:82-97): ids of string.split() + ['<eos>'] and the number of words mapped to
+    '<oov>' (a KeyError if one is needed and the vocabulary has none, as in the reference)."""
+    ids, oov = [], 0
+    for w in string.split() + ["<eos>"]:
+        i = word2idx.get(w)
+        if i is None:
+            i = word2idx["<oov>"]
+            oov += 1
+        ids.append(int(i))
+    return ids, oov
+
+
+def lm_final_score(score, nll_sum, n, oov, lm_weight, c_weight):
+    """(lm_score, num_words, final_score) of one ended hypothesis in the reference's fp32 operations (transformer.py:478-481,
+    lstm_utils.py:36-44, 124-127): total = n * (nll_sum / n); lm_score = -total / n + 1 - 2 * oov; final = score +
+    lm_weight * lm_score + sqrt(n + 1) * c_weight.  n is None for an empty string: lm_score -999, num_words 0; n == 0 (a
+    string of spaces only) gives NaN, as the reference's mean over no targets does."""
+    f = np.float32
+    if n is None:
+        return -999.0, 0, f(f(score) + f(lm_weight * -999.0)) + f(0.0)
+    if n == 0:
+        return float("nan"), 1, f("nan")
+    total = f(n) * f(f(nll_sum) / f(n))
+    lm = f(f(f(-total) / f(n)) + f(1.0)) - f(2 * oov)
+    return float(lm), n + 1, f(f(score) + f(lm_weight) * lm) + f(math.sqrt(n + 1) * c_weight)
+
+
+def lstm_lm_parts(lm):
+    """(RNNModel, word2idx) of an LSTM language model object (b200asr.LM or utils/lstm_utils.LM), else None."""
+    model, w2i = getattr(lm, "model", None), getattr(lm, "word2idx", None)
+    rnn = getattr(model, "rnn", None)
+    if not (isinstance(w2i, dict) and isinstance(rnn, nn.LSTM) and isinstance(getattr(model, "encoder", None), nn.Embedding)
+            and isinstance(getattr(model, "decoder", None), nn.Linear)):
+        return None
+    if rnn.bidirectional or rnn.batch_first or getattr(rnn, "proj_size", 0) or rnn.input_size != model.encoder.embedding_dim:
+        return None
+    return model, w2i
+
+
+def rank_nbest(finals, nbest):
+    """Indices of the nbest largest final scores; equal scores keep insertion order (transformer.py:499: sorted(...,
+    reverse=True) is stable)."""
+    return sorted(range(len(finals)), key=lambda j: finals[j], reverse=True)[:nbest]
+
+
+lm_rescore_stats = {}      # timings and counts of the last lm_rescore call (tools/decode_bench.py --lm reports them)
+
+
+def lm_rescore(self, buf, log, lm_parts, lm_weight, c_weight):
+    """n-best of a finished beam search under LM rescoring.  The end log comes to the host in one copy; the yseqs of its
+    entries are walked on the device into a packed buffer sized by their lengths and read once; the host builds each LM
+    string and its word ids (identical strings are scored once); the word ids go up in one copy and the LSTM LM scores
+    every sequence on the device; final scores follow in the reference's fp32 order and each utterance's entries are
+    ranked by a stable sort, so equal final scores keep insertion order (transformer.py:499-500)."""
+    model, w2i = lm_parts
+    dev = buf.score.device
+    B, W, nbest, S = buf.B, buf.W, buf.nbest, buf.steps
+    t0 = time.perf_counter()
+    host = log.buf.cpu().numpy()
+    cap = log.cap
+    counts = host[:B].astype(np.int64)
+    refs = host[B:B + B * cap].astype(np.int64)
+    scores = host[B + B * cap:].view(np.float32)
+    entries = np.concatenate([b * cap + np.arange(counts[b], dtype=np.int64) for b in range(B)])
+    r = refs[entries]
+    lens = (r >> 1) // W + 2 + (r & 1)
+    offsets = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int64)
+    packed = ops.beam_backtrack_packed(buf, log, entries, offsets, int(lens.sum())).cpu().numpy()
+    seq_of, seqs, item = {}, [], []          # LM string -> index into seqs; per entry (seq index | None, n, oov)
+    for j in range(len(entries)):
+        st = lm_string(packed[offsets[j]:offsets[j] + lens[j]], self.id2label)
+        if st == "":
+            item.append((None, None, 0))
+            continue
+        ids, oov = lm_word_ids(st, w2i)
+        n = len(ids) - 1
+        if n == 0:
+            item.append((None, 0, oov))
+            continue
+        k = seq_of.setdefault(st, len(seqs))
+        if k == len(seqs):
+            seqs.append(ids)
+        item.append((k, n, oov))
+    t1 = time.perf_counter()
+    sums = ops.lstm_lm_nll_sums(model, seqs, dev)
+    t2 = time.perf_counter()
+    ids_out = np.full((B, nbest, S + 2), -1, dtype=np.int64)
+    len_out = np.zeros((B, nbest), dtype=np.int64)
+    sc_out = np.full((B, nbest), np.nan, dtype=np.float32)
+    fin_out = np.full((B, nbest), np.nan, dtype=np.float32)
+    j0 = 0
+    for b in range(B):
+        rows = range(j0, j0 + int(counts[b]))
+        j0 += int(counts[b])
+        finals = []
+        for j in rows:
+            k, n, oov = item[j]
+            finals.append(lm_final_score(scores[entries[j]], sums[k] if k is not None else 0.0, n, oov, lm_weight, c_weight)[2])
+        for i, r in enumerate(rank_nbest(finals, nbest)):
+            fs, j = finals[r], rows[r]
+            ids_out[b, i, :lens[j]] = packed[offsets[j]:offsets[j] + lens[j]]
+            len_out[b, i] = lens[j]
+            sc_out[b, i] = scores[entries[j]]
+            fin_out[b, i] = fs
+    lm_rescore_stats.update(ended=len(entries), sequences=len(seqs), positions=int(sum(len(q) - 1 for q in seqs)),
+                            host_s=t1 - t0, lm_s=t2 - t1)
+    to = lambda a: torch.from_numpy(a).to(dev)
+    return to(ids_out), to(len_out), to(sc_out), to(fin_out)
 
 
 def _front_end(self, padded_input):
@@ -568,6 +727,44 @@ class Transformer(nn.Module):
                 nn.init.xavier_uniform_(p)
 
     forward = transformer_forward
+
+
+class RNNModel(nn.Module):
+    """utils/lstm_utils.py:138-201 with rnn_type "LSTM" (the only recurrent LM the reference's rescoring loads): the same
+    submodules and state_dict names (encoder, rnn, decoder), so the reference's checkpoints load.  It holds the parameters
+    of beam-search rescoring, which runs on the device (ops.lstm_lm_nll_sums); it has no forward of its own."""
+
+    def __init__(self, rnn_type, ntoken, ninp, nhid, nlayers, dropout=0.5, tie_weights=False):
+        super().__init__()
+        if rnn_type != "LSTM":
+            raise ValueError(f"RNNModel: only rnn_type 'LSTM' is supported, got {rnn_type!r}")
+        self.drop = nn.Dropout(dropout)
+        self.encoder = nn.Embedding(ntoken, ninp)
+        self.rnn = nn.LSTM(ninp, nhid, nlayers, dropout=dropout if nlayers > 1 else 0.0)
+        self.decoder = nn.Linear(nhid, ntoken)
+        if tie_weights:
+            if nhid != ninp:
+                raise ValueError("When using the tied flag, nhid must be equal to emsize")
+            self.decoder.weight = self.encoder.weight
+        self.rnn_type, self.nhid, self.nlayers = rnn_type, nhid, nlayers
+        with torch.no_grad():
+            self.encoder.weight.uniform_(-0.1, 0.1)
+            self.decoder.bias.zero_()
+            self.decoder.weight.uniform_(-0.1, 0.1)
+
+
+class LM:
+    """utils/lstm_utils.LM: loads the reference's LM checkpoint {word2idx, idx2word, ntoken, ninp, nhid, nlayers, dropout,
+    tie_weights, model_state_dict} into an RNNModel.  Pass it as beam_search(..., lm_rescoring=True, lm=LM(path))."""
+
+    def __init__(self, model_path):
+        self.model_path = model_path
+        ck = torch.load(model_path, map_location="cpu", weights_only=False)
+        self.word2idx, self.idx2word = ck["word2idx"], ck["idx2word"]
+        self.model = RNNModel("LSTM", ntoken=ck["ntoken"], ninp=ck["ninp"], nhid=ck["nhid"], nlayers=ck["nlayers"],
+                              dropout=ck["dropout"], tie_weights=ck["tie_weights"])
+        self.model.load_state_dict(ck["model_state_dict"])
+        self.model.eval()
 
 
 def build_model(cfg, id2label=None) -> Transformer:

@@ -8,6 +8,7 @@ from __future__ import annotations
 import os
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -1289,6 +1290,190 @@ def beam_backtrack(buf: BeamBuffers):
                                           L.ptr(ids), L.ptr(lengths), buf.B, buf.W, buf.nbest, buf.steps, _stream()),
             "beam_backtrack")
     return ids, lengths
+
+
+class EndLog:
+    """Every ended hypothesis of a beam search, per utterance in insertion order (include/b200asr.h b200asr_beam_step_log):
+    one int32 buffer [B counts | B * cap refs | B * cap fp32 scores], so that the host reads the whole log in one copy."""
+
+    def __init__(self, B, W, steps, device):
+        self.B, self.cap = B, W * steps
+        self.buf = torch.zeros(B * (1 + 2 * self.cap), device=device, dtype=torch.int32)
+        self.n = self.buf[:B]
+        self.ref = self.buf[B:B + B * self.cap]
+        self.score = self.buf[B + B * self.cap:].view(torch.float32)
+
+
+def beam_step_log(buf: BeamBuffers, log: EndLog, logits: torch.Tensor, word_tab: torch.Tensor, t: int, t_eos: int, c_weight: float):
+    """beam_step that also appends every hypothesis ending at step t to `log`."""
+    _need_cuda(logits, word_tab)
+    x = _f32c(logits.detach())
+    V = x.shape[1]
+    L.check(_lib().b200asr_beam_step_log(L.ptr(x), L.ptr(word_tab), buf.B, buf.W, V, int(t), int(t_eos), buf.steps, buf.nbest,
+                                         float(c_weight), L.ptr(buf.score), L.ptr(buf.state), L.ptr(buf.next_tok),
+                                         L.ptr(buf.idx[t % 2]), L.ptr(buf.idx[(t + 1) % 2]), buf.steps + 1, L.ptr(buf.hist_tok),
+                                         L.ptr(buf.hist_par), L.ptr(buf.pool_score), L.ptr(buf.pool_final), L.ptr(buf.pool_ref),
+                                         L.ptr(buf.pool_n), L.ptr(buf.n_live), L.ptr(log.ref), L.ptr(log.score), L.ptr(log.n),
+                                         log.cap, _stream()), "beam_step_log")
+
+
+def beam_backtrack_packed(buf: BeamBuffers, log: EndLog, entries, offsets, total: int) -> torch.Tensor:
+    """yseqs of the end-log entries `entries` (host int64, b * cap + e), packed from `offsets` (host int64): one copy up, the
+    ids stay on the device (int64 [total])."""
+    n = len(entries)
+    dev = buf.score.device
+    ids = torch.empty(max(total, 1), device=dev, dtype=torch.long)
+    if n:
+        up = torch.from_numpy(np.concatenate([entries, offsets]).astype(np.int64)).to(dev)
+        L.check(_lib().b200asr_beam_backtrack_packed(L.ptr(buf.hist_tok), L.ptr(buf.hist_par), L.ptr(log.ref), L.ptr(log.n), log.cap,
+                                                     L.ptr(up), up.data_ptr() + 8 * n, n, L.ptr(ids), buf.B, buf.W, buf.steps,
+                                                     _stream()), "beam_backtrack_packed")
+    return ids[:total]
+
+
+# ----------------------------------------------------------------------------------------------- LSTM language model
+LM_LOGIT_SCRATCH_BYTES = 256 << 20      # logits of at most this many bytes exist at once (chunks of packed positions)
+
+
+def _pad8(n):
+    return (n + 7) // 8 * 8
+
+
+class LstmLmOperands:
+    """Device operands of an LSTM LM (RNNModel("LSTM"): encoder nn.Embedding, rnn nn.LSTM, decoder nn.Linear), built on the
+    GPU by b200asr_lstm_prepare / b200asr_split_bf16: the embedding and decoder weights zero-padded to I / H columns, per layer
+    the gate-interleaved bf16x3 W_ih and W_hh operands and the folded bias.  `fresh()` is False once any parameter's version
+    counter (or storage) moved since the operands were built."""
+
+    def __init__(self, model, device):
+        rnn = model.rnn
+        self.ntoken, self.ninp = model.encoder.weight.shape
+        self.nhid, self.nlayers = rnn.hidden_size, rnn.num_layers
+        self.I, self.H = _pad8(self.ninp), _pad8(self.nhid)
+        self.device = device
+        self.params = list(model.parameters())
+        self.stamp = self._stamp()
+        f32 = dict(device=device, dtype=torch.float32)
+        with torch.no_grad():
+            dv = lambda t: None if t is None else t.detach().to(**f32).contiguous()
+            self.emb = torch.zeros((self.ntoken, self.I), **f32)
+            self.emb[:, :self.ninp] = dv(model.encoder.weight)
+            dec = torch.zeros((self.ntoken, self.H), **f32)
+            dec[:, :self.nhid] = dv(model.decoder.weight)
+            self.dec_b = dv(model.decoder.bias) if model.decoder.bias is not None else torch.zeros(self.ntoken, **f32)
+            self.dec_split = self._split(dec)
+            self.dec = dec
+            self.zero_pe = torch.zeros((1, self.I), **f32)
+            self.layers = []
+            for l in range(self.nlayers):
+                K = self.I if l == 0 else self.H
+                kin = self.ninp if l == 0 else self.nhid
+                w_ih_p = torch.empty((4 * self.H, K), **f32)
+                w_hh_p = torch.empty((4 * self.H, self.H), **f32)
+                bias_p = torch.empty(4 * self.H, **f32)
+                g = lambda n: dv(getattr(rnn, f"{n}_l{l}", None))
+                w_ih, w_hh, b_ih, b_hh = g("weight_ih"), g("weight_hh"), g("bias_ih"), g("bias_hh")
+                L.check(_lib().b200asr_lstm_prepare(L.ptr(w_ih), L.ptr(w_hh), L.ptr(b_ih), L.ptr(b_hh), kin, self.nhid, L.ptr(w_ih_p),
+                                                    L.ptr(w_hh_p), L.ptr(bias_p), _stream()), "lstm_prepare")
+                self.layers.append((w_ih_p, self._split(w_ih_p), self._split(w_hh_p), bias_p))
+
+    def _stamp(self):
+        return [(p.data_ptr(), p._version) for p in self.params]
+
+    def fresh(self):
+        return self._stamp() == self.stamp
+
+    @staticmethod
+    def _split(w):
+        N, K = w.shape
+        out = torch.empty((2, N, K), device=w.device, dtype=torch.bfloat16)
+        L.check(_lib().b200asr_split_bf16(L.ptr(w), L.ptr(out), None, N, K, 2, _stream()), "split_bf16")
+        return out
+
+
+def lstm_lm_operands(model, device) -> LstmLmOperands:
+    """The LM's prepared operands, cached on the module and rebuilt when a parameter changed in place."""
+    device = torch.device(device)
+    if device.index is None:
+        device = torch.device(device.type, torch.cuda.current_device())
+    ops_ = model.__dict__.get("_b200_lm_operands")
+    if ops_ is None or ops_.device != device or not ops_.fresh():
+        ops_ = LstmLmOperands(model, device)
+        model.__dict__["_b200_lm_operands"] = ops_
+    return ops_
+
+
+def lstm_layer_fwd(xproj, w_hh_split, batch_sizes, H):
+    """One LSTM layer over packed sequences (b200asr_lstm_layer_fwd): xproj [P, 4H] -> h [P, H]; batch_sizes host int32 [T]."""
+    bs = np.ascontiguousarray(batch_sizes, dtype=np.int32)
+    P = xproj.shape[0]
+    h = torch.empty((P, H), device=xproj.device, dtype=torch.float32)
+    c = torch.empty((int(bs[0]), H), device=xproj.device, dtype=torch.float32)
+    L.check(_lib().b200asr_lstm_layer_fwd(L.ptr(xproj), L.ptr(w_hh_split), bs.ctypes.data, len(bs), H, L.ptr(c), L.ptr(h),
+                                          _stream()), "lstm_layer_fwd")
+    return h
+
+
+def lstm_lm_layers(op: LstmLmOperands, inp, batch_sizes):
+    """Outputs [P, H] of every LSTM layer over packed word ids `inp` (device int64 [P], t-major, M_t = batch_sizes[t] live
+    sequences at step t): layer 0 reads the embedding rows (b200asr_embed_fwd: scale 1, a zero one-row positional table, no
+    dropout), each layer's input projection is one linear GEMM over all packed positions, then the recurrence."""
+    P = inp.shape[0]
+    x = torch.empty((P, op.I), device=inp.device, dtype=torch.float32)
+    L.check(_lib().b200asr_embed_fwd(L.ptr(inp), L.ptr(op.emb), L.ptr(op.zero_pe), L.ptr(x), P, 1, op.I, op.ntoken, 1.0, 0.0, 0, 0,
+                                     _stream()), "embed_fwd")
+    outs = []
+    for w_ih_p, ih_split, hh_split, bias_p in op.layers:
+        xproj = linear_fwd(x, w_ih_p, bias_p, False, L.PREC_BF16X3, WSplit(ih_split, None))
+        x = lstm_layer_fwd(xproj, hh_split, np.asarray(batch_sizes, dtype=np.int32), op.H)
+        outs.append(x)
+    return outs
+
+
+def lm_nll(logits, targets, out=None):
+    """Exact-fp32 logsumexp(row) - row[target] of every row of logits [rows, V] (row pitch logits.stride(0))."""
+    rows, V = logits.shape
+    out = torch.empty(rows, device=logits.device, dtype=torch.float32) if out is None else out
+    L.check(_lib().b200asr_lm_nll(L.ptr(logits), logits.stride(0), L.ptr(targets), L.ptr(out), rows, V, _stream()), "lm_nll")
+    return out
+
+
+def lstm_lm_nll_sums(model, seqs, device):
+    """Summed token NLL of every word-id sequence in `seqs` under the LSTM LM (LM.evaluate, utils/lstm_utils.py:105-127): the
+    LSTM runs from a zero state over ids[0 .. n-2] and scores targets ids[1 .. n-1].  Each sequence has n >= 2 ids.  Sequences
+    are packed t-major, longest first (stable); the ids go up in one copy.  Returns the fp32 sums in `seqs` order (host)."""
+    op = lstm_lm_operands(model, device)
+    n = len(seqs)
+    if n == 0:
+        return np.zeros(0, dtype=np.float32)
+    lens = np.array([len(s) - 1 for s in seqs], dtype=np.int64)
+    order = np.argsort(-lens, kind="stable")
+    T = int(lens[order[0]])
+    M = np.array([(lens > t).sum() for t in range(T)], dtype=np.int64)
+    off = np.concatenate([[0], np.cumsum(M)[:-1]]).astype(np.int64)
+    P = int(M.sum())
+    inp, tgt = np.empty(P, dtype=np.int64), np.empty(P, dtype=np.int64)
+    for j, s in enumerate(order):
+        ids = seqs[s]
+        pos = off[:lens[s]] + j
+        inp[pos] = ids[:-1]
+        tgt[pos] = ids[1:]
+    up = torch.from_numpy(np.concatenate([inp, tgt, off, lens[order]])).to(device)
+    inp_d, tgt_d, off_d, len_d = up[:P], up[P:2 * P], up[2 * P:2 * P + T], up[2 * P + T:]
+    x = lstm_lm_layers(op, inp_d, M)[-1]
+    nll = torch.empty(P, device=device, dtype=torch.float32)
+    chunk = max(1, min(P, LM_LOGIT_SCRATCH_BYTES // (4 * op.ntoken)))
+    scratch = torch.empty((chunk, op.ntoken), device=device, dtype=torch.float32)
+    for r0 in range(0, P, chunk):
+        r1 = min(P, r0 + chunk)
+        lg = scratch[:r1 - r0]
+        linear_fwd(x[r0:r1], op.dec, op.dec_b, False, L.PREC_BF16X3, WSplit(op.dec_split, None), out=lg)
+        lm_nll(lg, tgt_d[r0:r1], out=nll[r0:r1])
+    sums = torch.empty(n, device=device, dtype=torch.float32)
+    L.check(_lib().b200asr_lm_seq_sum(L.ptr(nll), L.ptr(off_d), L.ptr(len_d), n, L.ptr(sums), _stream()), "lm_seq_sum")
+    out = np.empty(n, dtype=np.float32)
+    out[order] = sums.cpu().numpy()
+    return out
 
 
 class CrossEntropyFn(torch.autograd.Function):

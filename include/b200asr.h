@@ -363,6 +363,42 @@ int b200asr_beam_self_attn(const float* q, const float* k_cache, const float* v_
  * it was forced, then -1; lengths [B][nbest] int64 (0: no hypothesis). */
 int b200asr_beam_backtrack(const int32_t* hist_tok, const int32_t* hist_par, const int32_t* pool_ref, const int32_t* pool_n,
                            int64_t* ids, int64_t* lengths, int B, int W, int nbest, int steps, b200asr_stream_t stream);
+/* Beam search with LM rescoring (lm_rescoring=True, :473-481): b200asr_beam_step plus an end log of EVERY ended hypothesis,
+ * since the LM may promote one that the non-LM n-best pool drops.  Per utterance b, in insertion order (step, then kept rank):
+ * end_ref[b * end_cap + e] = (t * W + k) * 2 + forced, end_score[...] = its fp32 score; end_n [B] (zero-initialised) counts
+ * them.  end_cap >= W * steps.  Everything else is exactly b200asr_beam_step (which is this call without the log). */
+int b200asr_beam_step_log(const float* logits, const int32_t* word_tab, int B, int W, int V, int t, int t_eos, int steps,
+                          int nbest, double c_weight, float* score, int32_t* state, int64_t* next_tok, const int32_t* idx_cur,
+                          int32_t* idx_nxt, int idx_stride, int32_t* hist_tok, int32_t* hist_par, float* pool_score,
+                          float* pool_final, int32_t* pool_ref, int32_t* pool_n, int32_t* n_live, int32_t* end_ref,
+                          float* end_score, int32_t* end_n, int end_cap, b200asr_stream_t stream);
+/* The yseqs of n end-log entries, packed: entry j = entries[j] (= b * end_cap + e) gets its t + 2 ids (SOS, tokens), plus the
+ * EOS if forced, at ids + offsets[j]; the length follows from the entry's ref alone, so the caller sizes ids exactly. */
+int b200asr_beam_backtrack_packed(const int32_t* hist_tok, const int32_t* hist_par, const int32_t* end_ref, const int32_t* end_n,
+                                  int end_cap, const int64_t* entries, const int64_t* offsets, int n, int64_t* ids, int B, int W,
+                                  int steps, b200asr_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * LSTM language model of the LM rescoring (utils/lstm_utils.py: LM.evaluate :105-127 -> RNNModel.forward :185-193 ->
+ * nn.LSTM(ninp, nhid, nlayers) + nn.Linear(nhid, ntoken) + CrossEntropyLoss).  H = nhid and I = ninp rounded up to multiples
+ * of 8; prepared matrices are gate-interleaved (row 4u + g = gate g of unit u, gate order i, f, g, o) with zero padding.
+ *   lstm_prepare: w_ih [4*nhid][ninp], w_hh [4*nhid][nhid], b_ih / b_hh [4*nhid] (NULL = 0) of one layer (nn.LSTM's
+ *     weight_ih_l{k} ...) -> w_ih_p [4H][I], w_hh_p [4H][H], bias_p [4H] = b_ih + b_hh.  The bf16x3 operands are then
+ *     b200asr_split_bf16(w_*_p, dst, NULL, 4H, K, 2).
+ *   lstm_layer_fwd: sequences packed t-major, longest first: batch_sizes (HOST array [T]) = M_t sequences live at step t,
+ *     non-increasing, >= 1; position off[t] + s, off[t] = M_0 + .. + M_{t-1}.  xproj [P][4H] = layer input x w_ih_p^T +
+ *     bias_p (b200asr_linear_fwd); h [P][H] gets the layer output, c [M_0][H] is workspace.  Step 0 is the zero-state cell;
+ *     each later step is one tensor-core launch (bf16x3 h_{t-1} W_hh^T, w_hh_split = its bf16 [2][4H][H] operand) whose
+ *     epilogue adds xproj and applies the fp32 cell (1/(1+expf(-x)), tanhf).  H % 8 == 0.
+ *   lm_nll: nll[r] = logsumexp(logits[r, :V]) - logits[r, targets[r]] in exact fp32 (row pitch ld); NaN for a target outside
+ *     [0, V).  lm_seq_sum: sums[s] = sum over t < lengths[s] of nll[offsets[t] + s], in t order (reproducible). */
+int b200asr_lstm_prepare(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, int ninp, int nhid,
+                         float* w_ih_p, float* w_hh_p, float* bias_p, b200asr_stream_t stream);
+int b200asr_lstm_layer_fwd(const float* xproj, const void* w_hh_split, const int32_t* batch_sizes, int T, int H, float* c, float* h,
+                           b200asr_stream_t stream);
+int b200asr_lm_nll(const float* logits, long long ld, const int64_t* targets, float* nll, int rows, int V, b200asr_stream_t stream);
+int b200asr_lm_seq_sum(const float* nll, const int64_t* offsets, const int64_t* lengths, int nseq, float* sums,
+                       b200asr_stream_t stream);
 int b200asr_ce_fwd(const float* logits, const int64_t* gold, float* row_lse, float* stats, int rows, int V,
                    float smoothing, b200asr_stream_t stream);
 /* stats[3] = stats[0] / stats[1] (the reference's mean loss), stats[4] = 1 / stats[1];
