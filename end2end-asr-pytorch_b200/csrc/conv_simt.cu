@@ -561,15 +561,6 @@ __global__ void maxpool2x2_bwd_tail_kernel(float* __restrict__ dx, uint16_t* __r
   }
 }
 
-__global__ void relu_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dx, long long n4) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n4) return;
-  float4 g = reinterpret_cast<const float4*>(dy)[i];
-  float4 v = reinterpret_cast<const float4*>(y)[i];
-  g.x = v.x > 0.f ? g.x : 0.f; g.y = v.y > 0.f ? g.y : 0.f; g.z = v.z > 0.f ? g.z : 0.f; g.w = v.w > 0.f ? g.w : 0.f;
-  reinterpret_cast<float4*>(dx)[i] = g;
-}
-
 // host-side launchers used by the API and (for precision 0) nothing else
 int conv3x3_simt(const float* in, const float* wr, const float* bias, const float* mask, float* out, int B, int T, int F,
                  int Cin, int Cout, int relu, cudaStream_t st) {
@@ -691,6 +682,7 @@ int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float
     return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st);
   }
   conv_repack_k_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (float*)ws, Ci, Co, 0, precision == B200ASR_PREC_TF32X3);
+  if (precision == B200ASR_PREC_TF32X3) return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st);
   return conv3x3_tc(x, (const float*)ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st);
 }
 
@@ -733,6 +725,7 @@ int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_
   }
   B200_REQUIRE(!dx16, B200ASR_BAD_ARG, "conv3x3_bwd_data: the bf16 pair output exists in the bf16 modes only");
   conv_repack_k_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (float*)ws, Ci, Co, 1, precision == B200ASR_PREC_TF32X3);
+  if (precision == B200ASR_PREC_TF32X3) return conv3x3_tc_halo(dy, ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st);
   return conv3x3_tc(dy, (const float*)ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st);
 }
 

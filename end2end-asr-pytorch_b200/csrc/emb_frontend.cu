@@ -1,8 +1,8 @@
 // emb_cnn front end (models/asr/transformer.py:33-40): generic strided NCHW convolution (direct form),
 // BatchNorm2d with batch statistics fused with the Hardtanh clamp, and the (B,C,F,T)->(B,T,C*F) flatten.
-// This path only serves the emb_cnn configuration (BASELINE cfg3).  Two formulations: direct kernels coalesced along W
-// (precision 0, exact fp32), and -- the default -- im2col / col2im around the tensor-core GEMM of the linear layers
-// (b200asr_linear_*): the 41x11 and 21x11 kernels make K = Ci*KH*KW = 451 / 7392, i.e. GEMM-shaped work.
+// This path only serves the emb_cnn configuration (BASELINE cfg3).  The convolutions here are the direct kernels coalesced
+// along W (precision 0, exact fp32); the tensor-core modes run them as implicit GEMMs (tc_emb.cu).  The BatchNorm / clamp
+// and flatten kernels serve both.
 #include "../../include/b200asr.h"
 #include "common.cuh"
 
@@ -302,66 +302,6 @@ __global__ void flatten_bcft_kernel(const float* __restrict__ src, float* __rest
   }
 }
 
-// ---- GEMM formulation of the same convolutions (tensor-core path): im2col, its adjoint, and the layout change between the
-// GEMM's pixel-major [B*OH*OW, C] results and the NCHW tensors of the BatchNorm / clamp kernels.
-// col[m][k], m = (b, oh, ow), k = (ci, kh, kw) -- the weight tensor [Co][Ci][KH][KW] is then the K-major B operand as is;
-// columns k >= K (row pitch padded to a multiple of 4 floats for TMA) are zero.
-// One thread per (m, ci, kh): its KW taps are contiguous both in the input row and in the column matrix, so the index
-// decomposition is paid once per KW elements.
-__global__ void im2col_kernel(const float* __restrict__ x, float* __restrict__ col, ConvG g, int K, int Kp, long long total) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int R = g.Ci * g.KH;
-  const int r = (int)(i % R);
-  const long long m = i / R;
-  const int kh = r % g.KH, ci = r / g.KH;
-  const int ow = (int)(m % g.OW), oh = (int)((m / g.OW) % g.OH), b = (int)(m / ((long long)g.OW * g.OH));
-  const int ih = oh * g.SH + kh - g.PH, iw0 = ow * g.SW - g.PW;
-  float* dst = col + m * Kp + (long long)r * g.KW;
-  const bool row_ok = ih >= 0 && ih < g.H;
-  const float* src = x + (((size_t)b * g.Ci + ci) * g.H + (row_ok ? ih : 0)) * g.W;
-  for (int kw = 0; kw < g.KW; kw++) {
-    const int iw = iw0 + kw;
-    dst[kw] = (row_ok && iw >= 0 && iw < g.W) ? src[iw] : 0.f;
-  }
-  if (r == R - 1)
-    for (int k = K; k < Kp; k++) col[m * Kp + k] = 0.f;
-}
-// adjoint: dx[b][ci][ih][iw] += dcol[m][k] (dx zeroed by the caller)
-__global__ void col2im_kernel(const float* __restrict__ dcol, float* __restrict__ dx, ConvG g, int K, int Kp, long long total) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int R = g.Ci * g.KH;
-  const int r = (int)(i % R);
-  const long long m = i / R;
-  const int kh = r % g.KH, ci = r / g.KH;
-  const int ow = (int)(m % g.OW), oh = (int)((m / g.OW) % g.OH), b = (int)(m / ((long long)g.OW * g.OH));
-  const int ih = oh * g.SH + kh - g.PH, iw0 = ow * g.SW - g.PW;
-  if (ih < 0 || ih >= g.H) return;
-  const float* src = dcol + m * Kp + (long long)r * g.KW;
-  float* dst = dx + (((size_t)b * g.Ci + ci) * g.H + ih) * g.W;
-  for (int kw = 0; kw < g.KW; kw++) {
-    const int iw = iw0 + kw;
-    if (iw >= 0 && iw < g.W) atomicAdd(dst + iw, src[kw]);
-  }
-}
-// [B][C][P] <-> [B][P][C] (32 x 32 tiles through shared memory)
-__global__ void transpose_cp_kernel(const float* __restrict__ src, float* __restrict__ dst, int C, int P, int to_pc) {
-  __shared__ float tile[32][33];
-  const int b = blockIdx.z, p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  const float* s = src + (size_t)b * C * P;
-  float* d = dst + (size_t)b * C * P;
-  if (to_pc) {          // src [C][P] -> dst [P][C]
-    for (int i = threadIdx.y; i < 32; i += 8) { const int c = c0 + i, pp = p0 + threadIdx.x; tile[i][threadIdx.x] = (c < C && pp < P) ? s[(size_t)c * P + pp] : 0.f; }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += 8) { const int pp = p0 + i, c = c0 + threadIdx.x; if (pp < P && c < C) d[(size_t)pp * C + c] = tile[threadIdx.x][i]; }
-  } else {              // src [P][C] -> dst [C][P]
-    for (int i = threadIdx.y; i < 32; i += 8) { const int pp = p0 + i, c = c0 + threadIdx.x; tile[i][threadIdx.x] = (pp < P && c < C) ? s[(size_t)pp * C + c] : 0.f; }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += 8) { const int c = c0 + i, pp = p0 + threadIdx.x; if (c < C && pp < P) d[(size_t)c * P + pp] = tile[threadIdx.x][i]; }
-  }
-}
-
 static int make_geom(ConvG& g, int B, int Ci, int H, int W, int Co, int KH, int KW, int SH, int SW, int PH, int PW) {
   B200_REQUIRE(B > 0 && Ci > 0 && Co > 0 && KH > 0 && KW > 0 && SH > 0 && SW > 0 && PH >= 0 && PW >= 0, B200ASR_BAD_SHAPE, "conv2d: bad geometry");
   g = ConvG{B, Ci, H, W, Co, KH, KW, SH, SW, PH, PW, (H + 2 * PH - KH) / SH + 1, (W + 2 * PW - KW) / SW + 1};
@@ -403,37 +343,6 @@ int b200asr_conv2d_bwd_weight(const float* dy, const float* x, float* dw, float*
   rc = check_launch("conv2d_bwd_weight"); if (rc) return rc;
   if (dbias) { conv2d_bias_grad_kernel<<<Co, 256, 0, st>>>(dy, dbias, B, Co, g.OH * g.OW); return check_launch("conv2d_bias_grad"); }
   return B200ASR_OK;
-}
-
-int b200asr_im2col(const float* x, float* col, int B, int Ci, int H, int W, int KH, int KW, int SH, int SW, int PH, int PW,
-                   int Kp, b200asr_stream_t stream) {
-  B200_REQUIRE(x && col, B200ASR_BAD_ARG, "im2col: null pointer");
-  ConvG g; int rc = make_geom(g, B, Ci, H, W, 1, KH, KW, SH, SW, PH, PW); if (rc) return rc;
-  const int K = Ci * KH * KW;
-  B200_REQUIRE(Kp >= K, B200ASR_BAD_SHAPE, "im2col: row pitch %d < %d", Kp, K);
-  const long long total = (long long)B * g.OH * g.OW * Ci * KH;
-  im2col_kernel<<<(unsigned)ceil_div_ll(total, 256), 256, 0, (cudaStream_t)stream>>>(x, col, g, K, Kp, total);
-  return check_launch("im2col");
-}
-
-int b200asr_col2im(const float* dcol, float* dx, int B, int Ci, int H, int W, int KH, int KW, int SH, int SW, int PH, int PW,
-                   int Kp, b200asr_stream_t stream) {
-  B200_REQUIRE(dcol && dx, B200ASR_BAD_ARG, "col2im: null pointer");
-  ConvG g; int rc = make_geom(g, B, Ci, H, W, 1, KH, KW, SH, SW, PH, PW); if (rc) return rc;
-  const int K = Ci * KH * KW;
-  B200_REQUIRE(Kp >= K, B200ASR_BAD_SHAPE, "col2im: row pitch %d < %d", Kp, K);
-  cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(dx, 0, sizeof(float) * (size_t)B * Ci * H * W, st);
-  const long long total = (long long)B * g.OH * g.OW * Ci * KH;
-  col2im_kernel<<<(unsigned)ceil_div_ll(total, 256), 256, 0, st>>>(dcol, dx, g, K, Kp, total);
-  return check_launch("col2im");
-}
-
-int b200asr_transpose_cp(const float* src, float* dst, int B, int C, int P, int to_pc, b200asr_stream_t stream) {
-  B200_REQUIRE(src && dst && B > 0 && C > 0 && P > 0 && B <= 65535, B200ASR_BAD_ARG, "transpose_cp: bad arguments");
-  dim3 grid(ceil_div(P, 32), ceil_div(C, 32), B);
-  transpose_cp_kernel<<<grid, dim3(32, 8), 0, (cudaStream_t)stream>>>(src, dst, C, P, to_pc);
-  return check_launch("transpose_cp");
 }
 
 size_t b200asr_bn_ws_bytes(int C) { return C > 0 ? sizeof(float) * 4 * BN_SPLITS * (size_t)C : 0; }

@@ -31,12 +31,12 @@ int bgemm_tc(const BOperand& A, bool a_kmaj, const BOperand& B, bool b_kmaj, flo
              int M, int N, int K, int Bsz, int H, float alpha, int nsplit, cudaStream_t st);
 
 // Tensor-core implicit-GEMM convolution (tc_conv.cu); takes K-major repacked weights wk[9][Cout][Cin]
-// (conv_repack_k_kernel); the weight-gradient variant takes/produces dwr[9][Ci][Co].
+// (conv_repack_k_kernel); the weight-gradient variant takes/produces dwr[9][Ci][Co].  conv3x3_tc is the TF32 forward /
+// data gradient (precision 1 only).
 int conv3x3_tc(const float* in, const float* wr, const float* bias, const float* mask, float* out, int B, int T, int F,
                int Cin, int Cout, int relu, int precision, cudaStream_t st);
-// 3xTF32 forward / data gradient with the input patch (incl. halo) fetched once per 32-channel slice (tc_conv_halo.cu);
-// conv3x3_tc dispatches to it for precision 3 (B200ASR_CONV_HALO=0 selects the tap-shifted engine policy instead).
-// mode 3 = 3xTF32 (fp32 hi | lo weights), 6 = bf16x3 / 2 = bf16 (bf16 weights from conv_repack_k_bf16)
+// Forward / data gradient of the 3xTF32 and bf16 modes, with the input patch (incl. halo) fetched once per 32-channel slice
+// (tc_conv_halo.cu).  mode 3 = 3xTF32 (fp32 hi | lo weights), 6 = bf16x3 / 2 = bf16 (bf16 weights from conv_repack_k_bf16)
 int conv3x3_tc_halo(const float* in, const void* wk, const float* bias, const float* mask, float* out, int B, int T, int F,
                     int Cin, int Cout, int relu, int mode, cudaStream_t st, void* out16 = nullptr, float* pool = nullptr);
 // out16: optional bf16 hi | lo pairs [2][B,T,F,Cout] of the output, written by the epilogue next to `out`

@@ -1,13 +1,14 @@
 // Tensor-core implicit-GEMM 3x3 convolution on channels-last [B,T,F,C] activations: forward / data gradient and weight
 // gradient, as policies of the persistent tile engine (tc_engine.cuh).
 //
+// Forward / data gradient (TF32; the 3xTF32 and bf16 modes run on the halo kernel, tc_conv_halo.cu):
 //   out[p][n] = act( sum_{tap} sum_c in[p + off(tap)][c] * wk[tap][n][c] + bias[n] ) (.* mask > 0)
 //
 // One tile = an 8 (time) x 16 (freq) patch = 128 output pixels x BN output channels.  The A operand of k-block
 // (tap, 32-channel slice) is ONE 4-D TMA box {32 ch, 16 freq, 8 time, 1 utt} fetched at the tap-shifted coordinate:
 // the zero padding of the convolution is TMA's out-of-bounds fill, so there is no im2col buffer and no halo logic.
 // The box lands in shared memory as 128 rows x 128 B (K-major, 128B swizzle).
-// The B operand is the repacked weight wk[tap][n][c] (K-major, one 2-D box), pre-split into hi | lo for 3xTF32.
+// The B operand is the repacked weight wk[tap][n][c] (K-major, one 2-D box).
 //
 // Weight gradient (bf16 modes; tf32 / 3xTF32 run on the halo weight-gradient kernel, tc_conv_wgrad.cu):
 //   dwr[tap][ci][co] += sum_p x[p + off(tap)][ci] * dy[p][co]
@@ -19,8 +20,6 @@
 // pixel blocks (its split) and writes its 128 x Co partial to the split's slot; reduce_parts sums the splits in order.  The
 // bias gradient (column sums of dy over all pixels) is taken by the tap-group-0 tiles while the dy tile is in shared memory,
 // instead of a separate pass that re-reads dy from HBM, and summed over the splits the same way.
-#include <stdlib.h>
-
 #include "../../include/b200asr.h"
 #include "common.cuh"
 #include "kernels.h"
@@ -47,10 +46,10 @@ struct WgP {
   int B, T, F, Ci, Co, nft, ntt, blocks_per_cta, total_blocks;
 };
 
-template <int BN_, int NSPLIT>
+template <int BN_>
 struct ConvPolicy {
   static constexpr int BN = BN_, kABytes = A_TILE, kBBytes = BN_ * 128;
-  static constexpr bool kSplitA = true, kSplitB = false, kAMN = false, kBMN = false;     // weights arrive pre-split
+  static constexpr bool kSplitA = true, kSplitB = false, kAMN = false, kBMN = false;     // weights arrive K-major
   static constexpr bool kSumA = false, kSumB = false;
   struct Params { ConvEpi e; int nft, ntt, cch; };
   static __device__ __forceinline__ int num_tiles(const Params& p) { return p.nft * p.ntt * p.e.B; }
@@ -67,12 +66,11 @@ struct ConvPolicy {
   }
   // k order: tap-major (tap = 3 * (df + 1) + (dt + 1)), 32-channel blocks inside a tap
   static __device__ __forceinline__ void load(const Params& p, Tile& t, const CUtensorMap* mapA, const CUtensorMap* mapB,
-                                              uint32_t sa, uint32_t sb, uint32_t sb_lo, uint32_t bar, bool leader) {
+                                              uint32_t sa, uint32_t sb, uint32_t, uint32_t bar, bool leader) {
     const int c0 = t.cb * 32;
     if (leader) {
       tma_load_4d(sa, mapA, bar, c0, t.f0 + t.df, t.t0 + t.dt, t.b);
       tma_load_2d(sb, mapB, bar, c0, t.tap * BN);
-      if (NSPLIT == 3) tma_load_2d(sb_lo, mapB, bar, c0, (9 + t.tap) * BN);
     }
     if (++t.cb == p.cch) {
       t.cb = 0; t.tap++;
@@ -196,12 +194,12 @@ struct WgradPairPolicy : WgradPolicy<CI, BN_> {
   }
 };
 
-template <int BN, int NSPLIT>
+template <int BN>
 static int launch_conv_persistent(const CUtensorMap& ma, const CUtensorMap& mb, const ConvEpi& e, cudaStream_t st) {
-  typename ConvPolicy<BN, NSPLIT>::Params p{e, ceil_div(e.F, CT_F), ceil_div(e.T, CT_T), e.Cin / 32};
+  typename ConvPolicy<BN>::Params p{e, ceil_div(e.F, CT_F), ceil_div(e.T, CT_T), e.Cin / 32};
   const long long tiles = (long long)p.nft * p.ntt * e.B;
   if (tiles >= (1LL << 31)) { set_error("conv3x3_tc: too many tiles"); return B200ASR_BAD_SHAPE; }
-  return launch_engine<ConvPolicy<BN, NSPLIT>, NSPLIT>(ma, mb, p, (int)tiles, st, "tc_conv3x3");
+  return launch_engine<ConvPolicy<BN>, 1>(ma, mb, p, (int)tiles, st, "tc_conv3x3");
 }
 
 // pixel blocks per split and number of splits: about two tiles per SM over the tap groups, at least 64 blocks per tile
@@ -220,38 +218,32 @@ static int launch_wgrad(const CUtensorMap& mx, const CUtensorMap& mdy, const WgP
 
 }  // namespace tc
 
-// wk: [9][Cout][Cin] K-major weights (conv_repack_k_kernel); for precision 3 the buffer holds [2][9][Cout][Cin]:
-// hi = rn_tf32(w) followed by lo = w - hi, so the kernel only has to split the activation tiles.
+// wk: [9][Cout][Cin] K-major weights (conv_repack_k_kernel).
 int conv3x3_tc(const float* in, const float* wk, const float* bias, const float* mask, float* out, int B, int T, int F,
                int Cin, int Cout, int relu, int precision, cudaStream_t st) {
   using namespace tc;
-  B200_REQUIRE(precision == 1 || precision == 3, B200ASR_BAD_ARG, "conv3x3_tc: precision must be 1 or 3");
+  B200_REQUIRE(precision == 1, B200ASR_BAD_ARG, "conv3x3_tc: precision must be 1");
   B200_REQUIRE(Cin % 32 == 0 && (Cout == 64 || Cout == 128), B200ASR_BAD_SHAPE,
                "conv3x3_tc: needs Cin %% 32 == 0 and Cout in {64,128} (Cin=%d Cout=%d)", Cin, Cout);
   B200_REQUIRE(aligned16(in) && aligned16(wk) && aligned16(out) && (!bias || aligned16(bias)) && (!mask || aligned16(mask)),
                B200ASR_BAD_ALIGN, "conv3x3_tc: pointers must be 16-byte aligned");
-  if (precision == 3) {
-    static const int halo = [] { const char* v = getenv("B200ASR_CONV_HALO"); return v ? atoi(v) : 1; }();
-    if (halo) return conv3x3_tc_halo(in, wk, bias, mask, out, B, T, F, Cin, Cout, relu, 3, st);
-  }
   CUtensorMap ma, mb;
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)F, (uint64_t)T, (uint64_t)B};
     uint64_t strides[3] = {(uint64_t)Cin, (uint64_t)F * Cin, (uint64_t)T * F * Cin};
     uint32_t box[4] = {32, CT_F, CT_T, 1};
-    int rc = make_tensor_map_f32(&ma, in, 4, dims, strides, box, precision == 1);
+    int rc = make_tensor_map_f32(&ma, in, 4, dims, strides, box, true);
     if (rc) return rc;
   }
   {
-    uint64_t dims[2] = {(uint64_t)Cin, (uint64_t)(precision == 3 ? 18 : 9) * Cout};     // [hi | lo] halves for 3xTF32
+    uint64_t dims[2] = {(uint64_t)Cin, (uint64_t)9 * Cout};
     uint64_t strides[1] = {(uint64_t)Cin};
     uint32_t box[2] = {32, (uint32_t)Cout};
-    int rc = make_tensor_map_f32(&mb, wk, 2, dims, strides, box, precision == 1);
+    int rc = make_tensor_map_f32(&mb, wk, 2, dims, strides, box, true);
     if (rc) return rc;
   }
   ConvEpi e{out, bias, mask, relu, B, T, F, Cin, Cout};
-  if (Cout == 64) return precision == 1 ? launch_conv_persistent<64, 1>(ma, mb, e, st) : launch_conv_persistent<64, 3>(ma, mb, e, st);
-  return precision == 1 ? launch_conv_persistent<128, 1>(ma, mb, e, st) : launch_conv_persistent<128, 3>(ma, mb, e, st);
+  return Cout == 64 ? launch_conv_persistent<64>(ma, mb, e, st) : launch_conv_persistent<128>(ma, mb, e, st);
 }
 
 // dbias (optional, not at precision 1): [Co], produced by the kernel; returns with *dbias_done = 1 when the

@@ -40,8 +40,6 @@ class _Config:
         self.conv_wgrad = _PREC_NAMES[os.environ.get("B200ASR_CONV_WGRAD", "tf32x3")]
         self.attn = _PREC_NAMES[os.environ.get("B200ASR_ATTN", "tf32x3")]          # "bf16x3" = the fused single-kernel path (opt-in)
         self.attn_bwd = _PREC_NAMES[os.environ.get("B200ASR_ATTN_BWD", "fp32")]
-        # emb_cnn's second convolution as implicit GEMMs (tc_emb.cu) instead of im2col + GEMM
-        self.emb_implicit = os.environ.get("B200ASR_EMB_IMPLICIT", "1") != "0"
 
     def set(self, linear=None, conv=None, attn=None, conv_wgrad=None, attn_bwd=None):
         if attn_bwd is not None:
@@ -315,33 +313,6 @@ def _grad_sink(param):
     return g
 
 
-class _WgradStream:
-    """Weight-gradient GEMMs of the dense layers are off the critical path of the backward pass (nothing downstream reads
-    them before the optimizer).  When `enabled` (parallel.DataParallelStep turns it on around loss.backward()) the ones that
-    accumulate straight into the flat gradient buffer are queued on a second stream: their CTAs fill the SMs that the
-    data-gradient GEMMs of the main stream leave idle in their last, partial wave and run under the small LayerNorm /
-    softmax kernels.  sync() makes the current stream wait for all of them.  Not the default: the engine kernels are
-    persistent (one CTA per SM for the whole tile list, most of the shared memory each), so a weight-gradient kernel that
-    got the SMs first holds them until its last tile and the critical-path data-gradient kernel queues behind it.  Kept
-    behind B200ASR_ASYNC_WGRAD=1."""
-
-    def __init__(self):
-        self.enabled, self.stream, self.used = False, None, False
-
-    def get(self, device):
-        if self.stream is None or self.stream.device != device:
-            self.stream = torch.cuda.Stream(device=device)
-        return self.stream
-
-    def sync(self):
-        if self.used and self.stream is not None:
-            torch.cuda.current_stream().wait_stream(self.stream)
-        self.used = False
-
-
-wgrad_stream = _WgradStream()
-
-
 def linear_bwd_weight(dy2, x2, want_bias, prec, w_sink=None, b_sink=None):
     """dW = dy^T x (+ column sums).  With sinks the kernels ACCUMULATE into the given .grad tensors and (None, None) is
     returned for them, so autograd has nothing left to add."""
@@ -349,15 +320,6 @@ def linear_bwd_weight(dy2, x2, want_bias, prec, w_sink=None, b_sink=None):
     K = x2.shape[1]
     direct = w_sink is not None and (not want_bias or b_sink is not None)
     if direct:
-        if wgrad_stream.enabled:
-            side, cur = wgrad_stream.get(dy2.device), torch.cuda.current_stream()
-            side.wait_stream(cur)                        # dy2 / x2 were produced on the main stream
-            dy2.record_stream(side); x2.record_stream(side)      # the caching allocator must not recycle them under the kernel
-            with torch.cuda.stream(side):
-                L.check(_lib().b200asr_linear_bwd_weight(L.ptr(dy2), L.ptr(x2), L.ptr(w_sink), L.ptr(b_sink) if want_bias else None,
-                                                         M, N, K, 1, prec, _stream()), "linear_bwd_weight")
-            wgrad_stream.used = True
-            return None, None
         L.check(_lib().b200asr_linear_bwd_weight(L.ptr(dy2), L.ptr(x2), L.ptr(w_sink), L.ptr(b_sink) if want_bias else None, M, N, K,
                                                  1, prec, _stream()), "linear_bwd_weight")
         return None, None
@@ -909,79 +871,29 @@ class PermuteColsFn(torch.autograd.Function):
 
 
 # ----------------------------------------------------------------------------------------------- emb_cnn front end
-def _conv_geom(x, w, geom):
-    B, Ci, H, W = x.shape
-    KH, KW, SH, SW, PH, PW = geom
-    OH, OW = (H + 2 * PH - KH) // SH + 1, (W + 2 * PW - KW) // SW + 1
-    K = Ci * KH * KW
-    return B, Ci, H, W, w.shape[0], OH, OW, K, (K + 7) // 8 * 8      # K padded to 8: legal row pitch for fp32 and bf16 operands
-
-
-def _im2col(x, geom, Kp):
-    B, Ci, H, W = x.shape
-    KH, KW, SH, SW, PH, PW = geom
-    OH, OW = (H + 2 * PH - KH) // SH + 1, (W + 2 * PW - KW) // SW + 1
-    col = torch.empty((B * OH * OW, Kp), device=x.device, dtype=torch.float32)
-    L.check(_lib().b200asr_im2col(L.ptr(x), L.ptr(col), B, Ci, H, W, KH, KW, SH, SW, PH, PW, Kp, _stream()), "im2col")
-    return col
-
-
-def _padded_weight(w, K, Kp):
-    w2 = _f32c(w).reshape(w.shape[0], K)
-    if Kp == K:
-        return w2
-    wp = torch.zeros((w.shape[0], Kp), device=w.device, dtype=torch.float32)
-    wp[:, :K] = w2
-    return wp
-
-
-def _conv_gemm_fwd(x, w, b, geom, prec):
-    """NCHW convolution as im2col + the tensor-core GEMM of the linear layers (+ bias in its epilogue); returns NCHW."""
-    B, Ci, H, W, Co, OH, OW, K, Kp = _conv_geom(x, w, geom)
-    col = _im2col(x, geom, Kp)
-    wp = _padded_weight(w, K, Kp)
-    y_pc = linear_fwd(col, wp, b, False, prec, split_weight(wp, prec))           # [B*OH*OW, Co]
-    y = torch.empty((B, Co, OH, OW), device=x.device, dtype=torch.float32)
-    L.check(_lib().b200asr_transpose_cp(L.ptr(y_pc), L.ptr(y), B, Co, OH * OW, 0, _stream()), "transpose_cp")
-    return y, col          # the column matrix is kept for the weight gradient (9 GB at cfg3 -- small change on 180 GB)
-
-
-def _conv_gemm_bwd(dy, x, w, col, geom, prec, prec_w, need_dx):
-    """(dx or None, dw, db) of _conv_gemm_fwd: weight gradient = GEMM over the saved im2col matrix (bias gradient fused),
-    data gradient = GEMM into the column space followed by col2im."""
-    B, Ci, H, W, Co, OH, OW, K, Kp = _conv_geom(x, w, geom)
-    lib, st = _lib(), _stream()
-    dy_pc = torch.empty((B * OH * OW, Co), device=x.device, dtype=torch.float32)
-    L.check(lib.b200asr_transpose_cp(L.ptr(_f32c(dy)), L.ptr(dy_pc), B, Co, OH * OW, 1, st), "transpose_cp")
-    dwp, db = linear_bwd_weight(dy_pc, col, True, prec_w)
-    dw = dwp[:, :K].reshape(w.shape).contiguous() if Kp != K else dwp.view(w.shape)
-    dx = None
-    if need_dx:
-        wp = _padded_weight(w, K, Kp)
-        dcol = linear_bwd_data(dy_pc, wp, None, prec, split_weight(wp, prec))
-        dx = torch.empty((B, Ci, H, W), device=x.device, dtype=torch.float32)
-        KH, KW, SH, SW, PH, PW = geom
-        L.check(lib.b200asr_col2im(L.ptr(dcol), L.ptr(dx), B, Ci, H, W, KH, KW, SH, SW, PH, PW, Kp, st), "col2im")
-    return dx, dw, db
-
-
 class EmbFrontendFn(torch.autograd.Function):
     """models/asr/transformer.py:33-40 (+ flatten :74-76): conv(41x11,s2x2,p0x10)+BN+clamp, conv(21x11,s2x1)+BN+clamp.
     BatchNorm2d semantics of torch: `training` -> batch statistics, and the module's running_mean / running_var /
     num_batches_tracked buffers (bn1, bn2 = (running_mean, running_var, num_batches_tracked, momentum) or None) are
     updated in the kernel; eval -> the running statistics normalise (the reference validates with model.eval(),
     trainer.py:123, and Transformer.evaluate reads the same buffers through the stock nn.BatchNorm2d).
-    Tensor-core modes: the first convolution (C_in = 1, K = 451) runs as im2col + the GEMM of the linear layers; the second
-    (32 -> 32 channels, 21 x 11 taps, 88% of the front end's FLOPs) as IMPLICIT GEMMs for forward, data gradient and weight
-    gradient (tc_emb.cu) on row-pitched NCHW tensors -- no column matrix.  Precision "fp32": direct CUDA-core kernels."""
+    Tensor-core modes: both convolutions run as IMPLICIT GEMMs (tc_emb.cu) for forward and weight gradient, the second
+    (32 -> 32 channels, 21 x 11 taps, 88% of the front end's FLOPs) also for its data gradient, on row-pitched NCHW tensors
+    -- no column matrix.  These kernels take the reference's two weight shapes only; any other shape is an error.
+    Precision "fp32": direct CUDA-core kernels."""
 
-    G1, G2 = (41, 11, 2, 2, 0, 10), (21, 11, 2, 1, 0, 0)
+    W0, W3 = (32, 1, 41, 11), (32, 32, 21, 11)
 
     @staticmethod
     def forward(ctx, x, w0, b0, g1, be1, w3, b3, g4, be4, eps, training=True, bn1=None, bn2=None):
         _need_cuda(x, w0)
         if not training and (bn1 is None or bn2 is None):
             raise RuntimeError("emb_cnn front end in eval mode needs the BatchNorm running statistics")
+        tc = config.conv != L.PREC_FP32
+        if tc and (tuple(w0.shape) != EmbFrontendFn.W0 or tuple(w3.shape) != EmbFrontendFn.W3):
+            # the kernels are given the reference's geometry: another weight shape would be read out of bounds
+            raise RuntimeError(f"emb_cnn front end: the tensor-core kernels support conv weights {EmbFrontendFn.W0} and "
+                               f"{EmbFrontendFn.W3} only, got {tuple(w0.shape)} and {tuple(w3.shape)}")
 
         def bn_args(bn):
             if bn is None:
@@ -996,37 +908,27 @@ class EmbFrontendFn(torch.autograd.Function):
         dev = x.device
         new = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)
         C = w0.shape[0]
-        gemm = config.conv != L.PREC_FP32 and C % 4 == 0
-        implicit = (gemm and config.emb_implicit and C == 32 and w3.shape[1] == 32          # tc_emb.cu: 1 -> 32 and 32 -> 32 channels
-                    and tuple(w0.shape) == (32, 1, 41, 11) and tuple(w3.shape[2:]) == (21, 11))
         H1, W1 = (H - 41) // 2 + 1, (W + 20 - 11) // 2 + 1
         H2, W2 = (H1 - 21) // 2 + 1, (W1 - 11) // 1 + 1
-        P1, P2 = ((W1 + 3) // 4 * 4, (W2 + 3) // 4 * 4) if implicit else (W1, W2)      # TMA: 16-byte row pitches
-        col1 = None
+        P1, P2 = ((W1 + 3) // 4 * 4, (W2 + 3) // 4 * 4) if tc else (W1, W2)      # TMA: 16-byte row pitches
         prec2 = config.conv if config.conv in (L.PREC_TF32X3, L.PREC_BF16X3, L.PREC_BF16) else L.PREC_TF32X3
-        if implicit:
-            c1 = new(B, C, H1, W1)
+        c1 = new(B, C, H1, W1)
+        if tc:
             ws1 = torch.empty(lib.b200asr_conv2d_c1_tc_ws_bytes(B, H, W, 41, 11) // 4, device=dev, dtype=torch.float32)
             L.check(lib.b200asr_conv2d_c1_tc_fwd(L.ptr(x), L.ptr(_f32c(w0)), L.ptr(b0), L.ptr(c1), L.ptr(ws1), B, H, W, C, 41, 11, 10, W1, prec2, st),
                     "emb_conv1_tc")
-        elif gemm:
-            c1, col1 = _conv_gemm_fwd(x, w0, b0, EmbFrontendFn.G1, config.conv)
         else:
-            c1 = new(B, C, H1, W1)
             L.check(lib.b200asr_conv2d_fwd(L.ptr(x), L.ptr(_f32c(w0)), L.ptr(b0), L.ptr(c1), B, 1, H, W, C, 41, 11, 2, 2, 0, 10, st), "emb_conv1")
         a1, m1, s1 = new(B, C, H1, P1), new(C), new(C)
         bws = new(lib.b200asr_bn_ws_bytes(C) // 4)
         rm, rv, nbt, mom = bn_args(bn1)
         L.check(lib.b200asr_bn_clamp_fwd(L.ptr(c1), L.ptr(g1), L.ptr(be1), L.ptr(a1), L.ptr(m1), L.ptr(s1), L.ptr(rm), L.ptr(rv),
                                          L.ptr(nbt), L.ptr(bws), B, C, H1, W1, W1, P1, eps, mom, int(training), 0.0, 20.0, st), "emb_bn1")
-        col2 = None
         c2 = new(B, C, H2, P2)
-        if implicit:
+        if tc:
             ws = torch.empty(lib.b200asr_conv2d_tc_ws_bytes(B, H1, W1, 21, 11) // 4, device=dev, dtype=torch.float32)
             L.check(lib.b200asr_conv2d_tc_fwd(L.ptr(a1), L.ptr(_f32c(w3)), L.ptr(b3), L.ptr(c2), L.ptr(ws), B, C, H1, W1, C, 21, 11, 2,
                                               P1, P2, prec2, st), "emb_conv2_tc")
-        elif gemm:
-            c2, col2 = _conv_gemm_fwd(a1, w3, b3, EmbFrontendFn.G2, config.conv)
         else:
             L.check(lib.b200asr_conv2d_fwd(L.ptr(a1), L.ptr(_f32c(w3)), L.ptr(b3), L.ptr(c2), B, C, H1, W1, C, 21, 11, 2, 1, 0, 0, st), "emb_conv2")
         a2, m2, s2 = new(B, C, H2, W2), new(C), new(C)
@@ -1038,10 +940,9 @@ class EmbFrontendFn(torch.autograd.Function):
         ctx.save_for_backward(x, c1, a1, m1, s1, c2, a2, m2, s2, w0, g1, w3, g4)
         if decision_capture is not None:
             decision_capture.extend([("hardtanh", a1[..., :W1]), ("hardtanh", a2)])
-        ctx.gemm = (gemm, implicit, config.conv, config.conv_wgrad)
+        ctx.prec2 = prec2 if tc else None          # None: the direct fp32 kernels
         ctx.geom = (H1, W1, P1, H2, W2, P2)
         ctx.training = bool(training)
-        ctx.cols = (col1, col2)
         return out
 
     @staticmethod
@@ -1049,7 +950,7 @@ class EmbFrontendFn(torch.autograd.Function):
         if frontend_backward_hook is not None:
             frontend_backward_hook()
         x, c1, a1, m1, s1, c2, a2, m2, s2, w0, g1, w3, g4 = ctx.saved_tensors
-        gemm, implicit, prec, prec_w = ctx.gemm
+        prec2 = ctx.prec2
         H1, W1, P1, H2, W2, P2 = ctx.geom
         lib, st = _lib(), _stream()
         B, _, H, W = x.shape
@@ -1065,33 +966,25 @@ class EmbFrontendFn(torch.autograd.Function):
         L.check(lib.b200asr_bn_clamp_bwd(L.ptr(da2), L.ptr(c2), L.ptr(a2), L.ptr(g4), L.ptr(m2), L.ptr(s2), L.ptr(dc2), L.ptr(dg4), L.ptr(dbe4),
                                          L.ptr(bws), B, C, H2, W2, W2, P2, W2, P2, tr, 0.0, 20.0, st), "emb_bn2_bwd")
         da1 = new(B, C, H1, P1)
-        if implicit:
-            dw3, db3 = torch.empty_like(w3), new(C)
+        dw3, db3 = torch.empty_like(w3), new(C)
+        if prec2 is not None:
             ws = torch.empty(lib.b200asr_conv2d_tc_ws_bytes(B, H1, W1, 21, 11) // 4, device=dev, dtype=torch.float32)
             L.check(lib.b200asr_conv2d_tc_bwd_weight(L.ptr(dc2), L.ptr(a1), L.ptr(dw3), L.ptr(db3), L.ptr(ws), B, C, H1, W1, C, 21, 11, 2, P1, P2, st),
                     "emb_conv2_tc_wgrad")
-            prec2 = prec if prec in (L.PREC_TF32X3, L.PREC_BF16X3, L.PREC_BF16) else L.PREC_TF32X3
             L.check(lib.b200asr_conv2d_tc_bwd_data(L.ptr(dc2), L.ptr(_f32c(w3)), L.ptr(da1), L.ptr(ws), B, C, H1, W1, C, 21, 11, 2, P1, P2,
                                                    prec2, st), "emb_conv2_tc_dgrad")
-        elif gemm:
-            da1, dw3, db3 = _conv_gemm_bwd(dc2, a1, w3, ctx.cols[1], EmbFrontendFn.G2, prec, prec_w, True)
         else:
-            dw3, db3 = torch.empty_like(w3), new(C)
             L.check(lib.b200asr_conv2d_bwd_weight(L.ptr(dc2), L.ptr(a1), L.ptr(dw3), L.ptr(db3), B, C, H1, W1, C, 21, 11, 2, 1, 0, 0, st), "emb_conv2_wgrad")
             L.check(lib.b200asr_conv2d_bwd_data(L.ptr(dc2), L.ptr(_f32c(w3)), L.ptr(da1), B, C, H1, W1, C, 21, 11, 2, 1, 0, 0, st), "emb_conv2_dgrad")
         dc1, dg1, dbe1 = new(B, C, H1, P1), new(C), new(C)          # P1 = W1 unless the implicit-GEMM weight gradient reads it by TMA
         L.check(lib.b200asr_bn_clamp_bwd(L.ptr(da1), L.ptr(c1), L.ptr(a1), L.ptr(g1), L.ptr(m1), L.ptr(s1), L.ptr(dc1), L.ptr(dg1), L.ptr(dbe1),
                                          L.ptr(bws), B, C, H1, W1, P1, W1, P1, P1, tr, 0.0, 20.0, st), "emb_bn1_bwd")
-        if implicit:
-            dw0, db0 = torch.empty_like(w0), new(C)
+        dw0, db0 = torch.empty_like(w0), new(C)
+        if prec2 is not None:
             ws1 = torch.empty(lib.b200asr_conv2d_c1_tc_ws_bytes(B, H, W, 41, 11) // 4, device=dev, dtype=torch.float32)
             L.check(lib.b200asr_conv2d_c1_tc_bwd_weight(L.ptr(dc1), L.ptr(x), L.ptr(dw0), L.ptr(db0), L.ptr(ws1), B, H, W, C, 41, 11, 10, P1, st),
                     "emb_conv1_tc_wgrad")
-        elif gemm:
-            _, dw0, db0 = _conv_gemm_bwd(dc1, x, w0, ctx.cols[0], EmbFrontendFn.G1, prec, prec_w, False)
-            ctx.cols = None
         else:
-            dw0, db0 = torch.empty_like(w0), new(C)
             L.check(lib.b200asr_conv2d_bwd_weight(L.ptr(dc1), L.ptr(x), L.ptr(dw0), L.ptr(db0), B, 1, H, W, C, 41, 11, 2, 2, 0, 10, st), "emb_conv1_wgrad")
         return None, dw0, db0, dg1, dbe1, dw3, db3, dg4, dbe4, None, None, None, None
 

@@ -8,8 +8,6 @@ gathered global batch (trainer.py:84 + metrics.py:127-130).
 """
 from __future__ import annotations
 
-import os
-
 import torch
 import torch.distributed as dist
 
@@ -80,11 +78,7 @@ class DataParallelStep:
         self.pg = process_group
         self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
         self.clip = clip_max_norm
-        # all-reduce the transformer's gradients under the CNN front end's backward / dense-layer weight gradients on a second
-        # stream (ops._WgradStream); the environment switches exist for A/B measurements
-        self.overlap = os.environ.get("B200ASR_DP_OVERLAP", "1") != "0"
-        self.async_wgrad = os.environ.get("B200ASR_ASYNC_WGRAD", "0") != "0"    # measured and rejected, see ops._WgradStream
-        self._early = None
+        self._early = None          # the all-reduce of the gradients before flat.tail_offset, issued by _reduce_head_early
         self._scale = torch.zeros(4, device=self.flat.flat.device, dtype=torch.float32)    # [scale, grad norm, scratch, -]
         self._host_tail = loss_fn is not None or adam_factory is not None                  # CPU stand-ins (gloo tests)
         if self.world > 1:
@@ -99,7 +93,6 @@ class DataParallelStep:
         """Runs at the start of the CNN front end's backward (ops.frontend_backward_hook): every gradient before
         flat.tail_offset is final, so their all-reduce is issued now, on NCCL's own stream, under the convolution backward."""
         if self.world > 1 and self._early is None and 0 < self.flat.tail_offset < self.flat.numel:
-            ops.wgrad_stream.sync()          # the dense layers' weight gradients queued on the side stream
             self._early = dist.all_reduce(self.flat.flat_grad[:self.flat.tail_offset], op=dist.ReduceOp.SUM, group=self.pg, async_op=True)
 
     def forward_backward(self, src, lengths, tgt):
@@ -108,14 +101,11 @@ class DataParallelStep:
         pred, gold, hyp, _ = self.model(src, lengths, tgt)
         loss_sum, stats = self.loss_fn(pred, gold, self.smoothing, reduction="sum")
         self._early = None
-        prev, ops.frontend_backward_hook = ops.frontend_backward_hook, (self._reduce_head_early if self.overlap else None)
-        ops.wgrad_stream.enabled = self.async_wgrad and not self._host_tail
+        prev, ops.frontend_backward_hook = ops.frontend_backward_hook, self._reduce_head_early
         try:
             loss_sum.backward()
         finally:
             ops.frontend_backward_hook = prev
-            ops.wgrad_stream.enabled = False
-            ops.wgrad_stream.sync()
         self.flat.ensure_grad_views()
         self.flat.extras.copy_(stats[0:2])            # [sum-loss, n_tokens] ride with the gradients
         return pred, hyp, stats

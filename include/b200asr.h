@@ -10,8 +10,8 @@
  *     int64 token ids (torch.long), uint8 masks (1 = masked / padded).
  *   - the caller owns all memory it passes (including workspaces); the library keeps one scratch buffer per
  *     (device, stream) of its own, for the partial results of reductions summed in a fixed order, so that the same
- *     inputs give the same bits every run (the fp32 CUDA-core GEMM / convolution / attention backward variants and
- *     the im2col convolution path still accumulate with atomics).
+ *     inputs give the same bits every run (the fp32 CUDA-core GEMM / convolution / attention backward variants still
+ *     accumulate with atomics).
  *   - every function enqueues work on `stream` (a cudaStream_t passed as void*) and returns without
  *     synchronising.  Return value: 0 on success, <0 on error (B200ASR_* below);
  *     b200asr_last_error() gives a thread-local message.  No C++ exception crosses the ABI.
@@ -409,16 +409,6 @@ int b200asr_ce_finalize(float* stats, float* loss_out, int mean, b200asr_stream_
 int b200asr_ce_bwd(const float* logits, const int64_t* gold, const float* row_lse, float* dlogits, int rows,
                    int V, float smoothing, float gscale, const float* gscale_dev, const float* gscale_dev2,
                    b200asr_stream_t stream);
-
-/* GEMM formulation of the emb_cnn convolutions (default for precision != 0): col[(b,oh,ow)][(ci,kh,kw)] with row pitch Kp
- * (>= Ci*KH*KW, zero padded; multiple of 4 for the tensor-core GEMM), so that conv = b200asr_linear_fwd(col, w[Co][K]),
- * weight gradient = b200asr_linear_bwd_weight, data gradient = b200asr_linear_bwd_data followed by col2im (the adjoint
- * scatter; dx is zeroed inside).  transpose_cp converts [B][C][P] <-> [B][P][C] (to_pc != 0: C-major -> pixel-major). */
-int b200asr_im2col(const float* x, float* col, int B, int Ci, int H, int W, int KH, int KW, int SH, int SW, int PH,
-                   int PW, int Kp, b200asr_stream_t stream);
-int b200asr_col2im(const float* dcol, float* dx, int B, int Ci, int H, int W, int KH, int KW, int SH, int SW, int PH,
-                   int PW, int Kp, b200asr_stream_t stream);
-int b200asr_transpose_cp(const float* src, float* dst, int B, int C, int P, int to_pc, b200asr_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Step tail ("next" row of SURVEY.md §8f): Adam(betas, eps) with the learning rate supplied by the host

@@ -316,6 +316,22 @@ def test_emb_frontend_fwd_bwd(b200):
     assert max(errs.values()) < 1e-3, errs
 
 
+def test_emb_frontend_rejects_other_weight_shapes(b200_mod):
+    """At the default (tensor-core) precision the front end's kernels are given the reference's geometry, so any other
+    weight shape is refused before a kernel is launched: it would be read out of bounds."""
+    ops = _ops(b200_mod)
+    assert ops.config.conv != b200_mod._lib.PREC_FP32
+    lib = b200_mod._lib.load()
+    r = lambda *s: torch.randn(s, device="cuda")
+    x, w0, w3 = r(2, 1, 161, 38), r(32, 1, 41, 11), r(32, 32, 21, 11)
+    for a, b in ((r(32, 1, 21, 11), w3), (w0, r(32, 32, 11, 11)), (r(16, 1, 41, 11), r(16, 16, 21, 11))):
+        v = [r(a.shape[0]) for _ in range(6)]
+        n0 = lib.b200asr_launch_count()
+        with pytest.raises(RuntimeError, match=r"\(32, 1, 41, 11\) and \(32, 32, 21, 11\)"):
+            ops.EmbFrontendFn.apply(x, a, v[0], v[1], v[2], b, v[3], v[4], v[5], 1e-5)
+        assert lib.b200asr_launch_count() == n0
+
+
 def test_emb_frontend_batchnorm_state_and_eval_mode(b200):
     """nn.BatchNorm2d state of the emb_cnn front end (models/asr/transformer.py:34,38): three training steps update
     running_mean / running_var / num_batches_tracked exactly as torch does, and model.eval() normalises with them."""

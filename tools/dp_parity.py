@@ -53,6 +53,6 @@ if rank == 0:
     # parameters: the first Adam step is lr * g / (|g| + 1e-9), i.e. sign-like; entries whose gradient is rounding noise
     # (mathematically zero, e.g. key biases) may step in either direction, so the bound is a few learning rates, not 1e-4
     assert rel_err(g_dp, g_ref) < 1e-3 and rel_err(p_dp, ref.flat.flat) < 1e-2
-    print("DP PARITY OK (gradient all-reduce overlapped with the front-end backward: %s)" % (dp.overlap and dp.flat.tail_offset < dp.flat.numel))
+    print("DP PARITY OK (gradient all-reduce overlapped with the front-end backward: %s)" % (dp.flat.tail_offset < dp.flat.numel))
 dist.barrier()
 dist.destroy_process_group()
