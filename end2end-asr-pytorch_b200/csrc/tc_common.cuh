@@ -6,7 +6,6 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace b200asr {
 namespace tc {
@@ -39,21 +38,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug becomes a trap (CUDA error reported to the caller) instead of a hung GPU.
+// Bounded wait: a protocol bug becomes a trap (CUDA error reported to the caller) instead of a hung GPU.  It prints no
+// message on purpose: printf is a function call, and ptxas serializes every wgmma of a kernel that contains a call ANYWHERE
+// (C7510, "wgmma pipeline crossing function boundary") -- a message on the producer warp's path alone, where no wgmma is
+// ever in flight, is enough to make each MMA of the consumers wait for the previous one.  Every kernel that issues wgmma
+// must therefore stay call-free, including its policies' load / store code.  (A call-free record of block, thread and
+// barrier, stored into host-mapped memory before the trap, was tried: with it the cfg2 linear weight gradient took 4.93
+// instead of 4.52 ms per step on an H100, so the wait stays this small.)
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("b200asr: mbarrier wait timed out (block %d,%d,%d thread %d bar 0x%x parity %u)\n", blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, bar, parity);
-      __trap();
-    }
-  }
-}
-// The same bound without the message, for code that waits while its own wgmma are in flight: the printf is a function
-// call, and ptxas serializes every wgmma of a kernel whose MMA pipeline crosses a call.
-__device__ __forceinline__ void mbar_wait_inflight(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity))

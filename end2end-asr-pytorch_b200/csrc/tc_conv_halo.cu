@@ -6,7 +6,7 @@
 // traffic (weights are unchanged).
 //
 // This is possible because the A operand never reaches the tensor core from shared memory: the consumer threads read the
-// fp32 patch, round / split it in registers and issue register-A wgmma (tc_engine.cuh, mma_kblock).  So the patch needs no
+// fp32 patch, round / split it in registers and issue register-A wgmma (tc_engine.cuh, build_afrag / mma_pipeline).  So the patch needs no
 // MMA-legal layout -- a thread simply reads patch row (tt + dt) * 10 + (ff + df) for its output pixel (tt, ff) and tap (dt, df).
 //
 // Roles (384 threads, 1 CTA / SM, persistent over tiles): warp 0 TMA (patch ring of 3, one slice ahead; weight ring of S),
@@ -89,7 +89,9 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
     b = r / p.ntt;
   };
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<kProducerRegs>();   // the whole producer warpgroup (tc_engine.cuh)
+    if (warp != 0) return;
     // ------------------------------------------------------------------ TMA producer
     // Patches run ONE SLICE AHEAD of the weights: a patch is first-touch data from HBM while the consumers want it as soon
     // as its slice starts, so it is requested a whole slice (9 k-blocks) early into a ring of three.
@@ -127,7 +129,7 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
     }
     return;
   }
-  if (warp < 4) return;
+  setmaxnreg_inc<kConsumerRegs>();
 
   // -------------------------------------------------------------------- consumers
   const int ctid = threadIdx.x - 128;
@@ -137,35 +139,49 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
   const int prow0 = (r0 >> 3) * HPF + (r0 & 7), prow1 = (r1 >> 3) * HPF + (r1 & 7);   // their patch rows for tap (0, 0)
   float* epi = reinterpret_cast<float*>(gen_base + Cfg::kOffEpi);
   float dummy0 = 0.f, dummy1 = 0.f;
-  uint32_t s = 0, ph = 0, ps = 0, pph = 0;
+  uint32_t s = 0, ph = 0, rs = 0;                  // weight ring: next k-block, its phase, next release
+  uint32_t ps = 0, pph = 0, rps = 0;               // patch ring: the same
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
-    for (int sl = 0; sl < p.cch; sl++) {
-      const uint8_t* patch = gen_base + ps * HPATCH_STAGE;
-      mbar_wait(pfull_bar(ps), pph);
-      for (int tap = 0; tap < 9; tap++) {
-        mbar_wait(full_bar(s), ph);
-        const int shift = (tap % 3) * HPF + tap / 3;                // tap = 3 * (df + 1) + (dt + 1)
-        const int pr0 = prow0 + shift, pr1 = prow1 + shift;
-        const uint32_t sb = smem_base + Cfg::kRingOff + s * Cfg::kStageBytes;
-        // A element (pixel row r, channel k): patch row pr, 128B swizzle of the TMA box
-        mma_kblock<MODE, BN, true, false>(
-            acc,
-            [&](int r, int k) {
-              const int pr = r == r0 ? pr0 : pr1;
-              return reinterpret_cast<const float*>(patch + pr * 128 + (((k >> 2) ^ (pr & 7)) << 4) + (k & 3) * 4);
-            },
-            r0, r1, q, sb, sb + Cfg::kBBytes, dummy0, dummy1);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(s));
-        if (++s == S) { s = 0; ph ^= 1; }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pempty_bar(ps));      // this warp has read the patch for the last time
-      if (++ps == HPATCH_SLOTS) { ps = 0; pph ^= 1; }
-    }
+    // k-block = (slice, tap), taps fastest
+    int tap = 0, rtap = 0;
+    mma_pipeline<MODE, BN>(
+        acc, p.cch * 9,
+        [&](int, AFrag<MODE>& fr, uint32_t& bhi, uint32_t& blo) {
+          if (tap == 0) mbar_wait(pfull_bar(ps), pph);
+          mbar_wait(full_bar(s), ph);
+          const uint8_t* patch = gen_base + ps * HPATCH_STAGE;
+          const int shift = (tap % 3) * HPF + tap / 3;                // tap = 3 * (df + 1) + (dt + 1)
+          const int pr0 = prow0 + shift, pr1 = prow1 + shift;
+          const uint32_t sb = smem_base + Cfg::kRingOff + s * Cfg::kStageBytes;
+          // A element (pixel row r, channel k): patch row pr, 128B swizzle of the TMA box
+          build_afrag<MODE, true, false>(
+              fr,
+              [&](int r, int k) {
+                const int pr = r == r0 ? pr0 : pr1;
+                return reinterpret_cast<const float*>(patch + pr * 128 + (((k >> 2) ^ (pr & 7)) << 4) + (k & 3) * 4);
+              },
+              r0, r1, q, dummy0, dummy1);
+          bhi = sb;
+          blo = sb + Cfg::kBBytes;
+          if (++s == S) { s = 0; ph ^= 1; }
+          if (++tap == 9) {
+            tap = 0;
+            if (++ps == HPATCH_SLOTS) { ps = 0; pph ^= 1; }
+          }
+        },
+        [&](int) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(rs));
+          if (++rs == S) rs = 0;
+          if (++rtap == 9) {                           // this warp has read the slice's patch for the last time
+            rtap = 0;
+            if (lane == 0) mbar_arrive(pempty_bar(rps));
+            if (++rps == HPATCH_SLOTS) rps = 0;
+          }
+        });
 
     // ---- epilogue: bias, ReLU, mask, optional bf16 pairs and fused 2 x 2 max-pool; a warp covers 4 time rows x 8 freq bins
     int f0, t0, b;

@@ -111,7 +111,7 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
     uint32_t ls = 0, lph = 0;                          // ring position / phase of the next load
     int loaded = 0;
     auto load_next = [&]() {
-      mbar_wait_inflight(empty_bar(ls), lph ^ 1);
+      mbar_wait(empty_bar(ls), lph ^ 1);
       if (leader) {
         const uint32_t sa = smem_base + ls * Cfg::kStageBytes;
         const int f0 = ft * WH_F, t0 = tt * WH_T;
@@ -134,7 +134,7 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
     float bs[WH_N / 32][4] = {};
     uint32_t s = 0, ph = 0;
     for (int kb = 0; kb < nkb; kb++) {
-      mbar_wait_inflight(full_bar(s), ph);
+      mbar_wait(full_bar(s), ph);
       uint8_t* stage = gen_base + s * Cfg::kStageBytes;
 #pragma unroll
       for (int c = 0; c < WH_N / 32; c++) {
@@ -191,8 +191,8 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   uint32_t ah[2][4] = {}, al[2][4] = {};
   uint32_t s = 0, ph = 0;
   for (int kb = 0; kb < nkb; kb++) {
-    mbar_wait_inflight(full_bar(s), ph);
-    mbar_wait_inflight(ready_bar(s), ph);
+    mbar_wait(full_bar(s), ph);
+    mbar_wait(ready_bar(s), ph);
     const uint8_t* patch = gen_base + s * Cfg::kStageBytes + aoff;
     const uint32_t bhi = smem_base + s * Cfg::kStageBytes + Cfg::kOffHi, blo = bhi + (Cfg::kOffLo - Cfg::kOffHi);
     asm volatile("" : "+r"(sw[0]), "+r"(sw[1]));     // keeps the extracts below in the loop (see sw)

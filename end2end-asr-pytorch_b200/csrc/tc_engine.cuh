@@ -2,15 +2,22 @@
 //
 // One CTA per SM loops over 128 x BN output tiles (static round-robin).  Roles (384 threads):
 //   warp 0               TMA producer -- runs ahead across tiles through a ring of shared-memory stages
-//   warps 1-3            idle (they complete the producer warpgroup, so that the consumers are whole warpgroups)
+//   warps 1-3            B converters for B_T16_FROM32 without column sums (EngineCfg::kBByProducer): per stage they
+//                        transpose the fp32 B tile into bf16 hi | lo and arrive on the stage's "ready" mbarrier; otherwise
+//                        idle (they complete the producer warpgroup, so that the consumers are whole warpgroups)
 //   warpgroups 1 and 2   consumers, rows 0-63 and 64-127 of the tile.  Per k-block (32 deep) they
 //                          * read their rows of the raw fp32 A tile from the stage and round / split them into wgmma
 //                            register fragments (A never needs a tensor-core layout, so either major works);
 //                          * make B the K-major operand wgmma reads from shared memory when it did not arrive that way
-//                            (MN-major tiles are transposed, fp32 operands split into hi | lo or converted to bf16);
-//                          * issue the MMAs and release the stage;
+//                            and warps 1-3 do not convert it (MN-major tiles are transposed, fp32 operands split into
+//                            hi | lo or converted to bf16);
+//                          * issue the MMAs;
+//                        pipelined (mma_pipeline): k-block kb + 1 is prepared -- B made ready, A fragments built into a
+//                        second register buffer -- while kb's MMAs run, and kb's stage is released one k-block late;
 //                        after the last k-block they stage the accumulators through shared memory and hand 32-column row
 //                        pieces to Policy::store, a warp covering 32 consecutive rows.
+// The producer warpgroup gives registers to the consumers (setmaxnreg: 40 / 232 per thread).  The kernel must contain no
+// function call anywhere (no printf, no 64-bit division helper in a Policy): ptxas then serializes every wgmma (C7510).
 //
 // A Policy supplies the problem-specific parts:
 //   static constexpr int  BN, kABytes, kBBytes;  static constexpr bool kSplitA, kSplitB (operand needs the in-kernel split);
@@ -74,6 +81,9 @@ template <class Policy, int NSPLIT> struct EngineCfg {
   static constexpr int kBMode = kBf16 ? (Policy::kSplitB ? B_T16_FROM32 : (Policy::kBMN ? B_T16 : B_READY))
                                       : (Policy::kBMN ? B_T32 : ((NSPLIT == 3 && Policy::kSplitB) ? B_SPLIT_K : B_READY));
   static constexpr bool kBSplit = NSPLIT == 3 && Policy::kSplitB;     // B_T32: fp32 B split into hi | lo while transposed
+  // B_T16_FROM32 without column sums: warps 1-3 convert B (engine_convert_b16) and signal the consumers per stage.
+  // (B_T32 transposes in place, which needs the whole tile in registers first; B_SPLIT_K on warps 1-3 measured no faster.)
+  static constexpr bool kBByProducer = kBMode == B_T16_FROM32 && !Policy::kSumB;
   static constexpr int kTxBytes = kBf16 ? Policy::kABytes + (Policy::kSplitB ? Policy::kBBytes : kBHalves * kBTile)
                                         : Policy::kABytes + Policy::kBBytes +
                                           (NSPLIT == 3 && !Policy::kSplitB ? Policy::kBBytes : 0);   // pre-split B arrives as hi+lo
@@ -89,6 +99,7 @@ template <class Policy, int NSPLIT> struct EngineCfg {
   static_assert(!Policy::kSumB || Policy::kBMN, "column sums need an MN-major B tile");
   static_assert(BN == 32 || BN == 64 || BN == 128, "BN");
   static_assert(kStages >= 2, "stage too large");
+  static_assert(3 * 8 * kStages <= 256, "barriers (full, empty, ready per stage)");
   static_assert(kSmemBytes <= ENG_SMEM_CAP, "shared memory");
 };
 
@@ -101,15 +112,34 @@ template <bool MN> __device__ __forceinline__ uint32_t a_off(int r, int k) {
 __device__ __forceinline__ uint32_t kmaj32_off(int n, int k) { return n * 128 + (((k >> 2) ^ (n & 7)) << 4) + (k & 3) * 4; }
 __device__ __forceinline__ uint32_t kmaj16_off(int n, int k) { return n * 64 + (((k >> 3) ^ ((n >> 1) & 3)) << 4) + (k & 7) * 2; }
 
-// One 32-deep k-block of a 128 x BN tile: this thread's A rows r0 / r1 (fp32 in shared memory at a_ptr(r, k)) rounded or
-// split into wgmma register fragments per NSPLIT, times the K-major B tile(s) at bhi (| blo); returns once the MMAs have
-// completed, so the caller may release the stage.  KPAIR: elements (r, k) and (r, k + 1) are adjacent (8-byte loads).
-// SUMS: asum0 / asum1 += the fp32 A values of rows r0 / r1 this thread read (a quarter of each row; the caller reduces).
-template <int NSPLIT, int BN, bool KPAIR, bool SUMS, class APtr>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], APtr a_ptr, int r0, int r1, int q, uint32_t bhi, uint32_t blo,
-                                           float& asum0, float& asum1) {
+// Register split of the 384 threads (setmaxnreg): the producer warpgroup drops to kProducerRegs, the two consumer warpgroups
+// rise to kConsumerRegs -- 128 * 40 + 256 * 232 = 64,512, the 168 per thread that __launch_bounds__(384, 1) allots.  The
+// consumers need the room for a second set of A fragments (the pipelined k-loop below) next to the accumulators.
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 384 * 168, "register split");
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// wgmma register-A fragments of one 32-deep k-block of this thread's rows r0 / r1: hi (and, for the split modes, lo) per
+// k-step -- four tf32 k8 steps or two bf16 k16 steps
+template <int NSPLIT> struct AFrag {
+  static constexpr int KS = eng_is_bf16(NSPLIT) ? 2 : 4;
+  uint32_t h[KS][4], l[KS][4];
+};
+template <int NSPLIT> __device__ __forceinline__ void keep_live(const AFrag<NSPLIT>& f) {
+#pragma unroll
+  for (int ks = 0; ks < AFrag<NSPLIT>::KS; ks++) {
+    keep_live(f.h[ks]);
+    if constexpr (NSPLIT == 3 || NSPLIT == 6) keep_live(f.l[ks]);
+  }
+}
+
+// The A fragments of one k-block: this thread's A rows r0 / r1 (fp32 in shared memory at a_ptr(r, k)) rounded or split per
+// NSPLIT.  KPAIR: elements (r, k) and (r, k + 1) are adjacent (8-byte loads).  SUMS: asum0 / asum1 += the fp32 A values of
+// rows r0 / r1 this thread read (a quarter of each row; the caller reduces).
+template <int NSPLIT, bool KPAIR, bool SUMS, class APtr>
+__device__ __forceinline__ void build_afrag(AFrag<NSPLIT>& f, APtr a_ptr, int r0, int r1, int q, float& asum0, float& asum1) {
   if constexpr (!eng_is_bf16(NSPLIT)) {
-    uint32_t ah[4][4], al[4][4];
 #pragma unroll
     for (int ks = 0; ks < 4; ks++) {
       const int k0 = ks * 8 + q, k1 = k0 + 4;
@@ -118,21 +148,11 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], APtr a_ptr, int
 #pragma unroll
       for (int i = 0; i < 4; i++) {
         const float h = tf32_rn(x[i]);
-        ah[ks][i] = __float_as_uint(h);
-        al[ks][i] = __float_as_uint(x[i] - h);
+        f.h[ks][i] = __float_as_uint(h);
+        f.l[ks][i] = __float_as_uint(x[i] - h);
       }
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ks++) {
-      if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
-        wgmma_tf32<BN>(acc, al[ks], kmajor_desc_tf32(bhi + ks * 32));
-        wgmma_tf32<BN>(acc, ah[ks], kmajor_desc_tf32(blo + ks * 32));
-      }
-      wgmma_tf32<BN>(acc, ah[ks], kmajor_desc_tf32(bhi + ks * 32));
     }
   } else {
-    uint32_t ah[2][4], al[2][4];
 #pragma unroll
     for (int ks = 0; ks < 2; ks++) {
 #pragma unroll
@@ -147,23 +167,68 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], APtr a_ptr, int
           x1 = *a_ptr(r, k + 1);
         }
         if constexpr (SUMS) { if (i & 1) asum1 += x0 + x1; else asum0 += x0 + x1; }
-        if constexpr (NSPLIT == 6) split_bf16_pair(x0, x1, ah[ks][i], al[ks][i]);
-        else ah[ks][i] = pack_bf16_pair(x0, x1);
+        if constexpr (NSPLIT == 6) split_bf16_pair(x0, x1, f.h[ks][i], f.l[ks][i]);
+        else f.h[ks][i] = pack_bf16_pair(x0, x1);
       }
     }
-    wgmma_fence();
+  }
+}
+
+// The MMAs of one k-block, committed as one group: acc += A (fragments f) * B (K-major tile(s) at bhi | blo).
+template <int NSPLIT, int BN>
+__device__ __forceinline__ void issue_kblock(float (&acc)[BN / 2], const AFrag<NSPLIT>& f, uint32_t bhi, uint32_t blo) {
+  wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < 2; ks++) {
-      if constexpr (NSPLIT == 6) {
-        wgmma_bf16<BN>(acc, al[ks], kmajor_desc_bf16(bhi + ks * 32));
-        wgmma_bf16<BN>(acc, ah[ks], kmajor_desc_bf16(blo + ks * 32));
+  for (int ks = 0; ks < AFrag<NSPLIT>::KS; ks++) {
+    if constexpr (!eng_is_bf16(NSPLIT)) {
+      if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
+        wgmma_tf32<BN>(acc, f.l[ks], kmajor_desc_tf32(bhi + ks * 32));
+        wgmma_tf32<BN>(acc, f.h[ks], kmajor_desc_tf32(blo + ks * 32));
       }
-      wgmma_bf16<BN>(acc, ah[ks], kmajor_desc_bf16(bhi + ks * 32));
+      wgmma_tf32<BN>(acc, f.h[ks], kmajor_desc_tf32(bhi + ks * 32));
+    } else {
+      if constexpr (NSPLIT == 6) {
+        wgmma_bf16<BN>(acc, f.l[ks], kmajor_desc_bf16(bhi + ks * 32));
+        wgmma_bf16<BN>(acc, f.h[ks], kmajor_desc_bf16(blo + ks * 32));
+      }
+      wgmma_bf16<BN>(acc, f.h[ks], kmajor_desc_bf16(bhi + ks * 32));
     }
   }
   wgmma_commit();
+}
+
+// Pipelined k-loop over the nkb k-blocks of one tile: the MMAs of k-block kb run while the fragments of kb + 1 are built
+// into the other of two fragment buffers, and k-block kb's stage is released one k-block late, once the wait that leaves
+// only kb + 1's group in flight has retired its MMAs.  Each accumulator still receives the same MMAs in the same order.
+//   prep(kb, f, bhi, blo): wait for k-block kb's data, make its B operand ready, build its fragments into f and return the
+//                          shared-memory addresses of its B tile(s) -- called once per k-block, in order;
+//   release(kb):           k-block kb's MMAs have completed (its stage may be refilled) -- called once per k-block, in order.
+// Returns with every MMA complete.  The loop runs two k-blocks per trip so that the buffer index is a compile-time constant.
+template <int NSPLIT, int BN, class Prep, class Release>
+__device__ __forceinline__ void mma_pipeline(float (&acc)[BN / 2], int nkb, Prep&& prep, Release&& release) {
+  if (nkb <= 0) return;
+  AFrag<NSPLIT> f[2];
+  uint32_t bhi[2], blo[2];
+  prep(0, f[0], bhi[0], blo[0]);
+  auto step = [&](auto u_, int kb) {
+    constexpr int U = decltype(u_)::value;
+    issue_kblock<NSPLIT, BN>(acc, f[U], bhi[U], blo[U]);
+    if (kb > 0) {
+      wgmma_wait<1>();                     // k-block kb - 1 is done: its fragment buffer and its stage are free
+      keep_live(f[U ^ 1]);                 // (until here the compiler must not reuse those registers)
+      release(kb - 1);
+    }
+    if (kb + 1 < nkb) prep(kb + 1, f[U ^ 1], bhi[U ^ 1], blo[U ^ 1]);
+  };
+  for (int kb = 0; kb < nkb; kb += 2) {
+    step(std::integral_constant<int, 0>(), kb);
+    if (kb + 1 < nkb) step(std::integral_constant<int, 1>(), kb + 1);
+  }
   wgmma_wait<0>();
+  keep_live(f[0]);
+  keep_live(f[1]);
   acc_fence(acc);
+  release(nkb - 1);
 }
 
 // Accumulators of a 128 x BN tile (this thread: rows r0 / r1) staged through shared memory `epi` (128 rows of EC + 4 floats)
@@ -195,6 +260,33 @@ __device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], float*
   }
 }
 
+constexpr int ENG_CONVERTERS = 3;          // warps 1-3 (Cfg::kBByProducer)
+
+// fp32 MN-major B tile (BN columns x 32 k, at src) -> K-major bf16 hi (| lo) tiles at dh / dl, by one of the ENG_CONVERTERS
+// warps (cw): a work item is 32 consecutive columns (lane = column) x 8 consecutive k, read down 8 k-lines and stored as one
+// 16-byte row piece per half.  The same split_bf16_pair / pack_bf16_pair of the same (k, k + 1) pairs as the consumers' path.
+template <int NSPLIT, int BN>
+__device__ __forceinline__ void engine_convert_b16(const uint8_t* src, uint8_t* dh, uint8_t* dl, int cw, int lane) {
+  for (int it = cw; it < (BN / 32) * 4; it += ENG_CONVERTERS) {
+    const int n = (it >> 2) * 32 + lane, kg = it & 3;
+    const uint8_t* col = src + (it >> 2) * 4096 + (lane & 3) * 4;
+    float x[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+      const int k = kg * 8 + j;
+      x[j] = *reinterpret_cast<const float*>(col + k * 128 + ((((lane & 31) >> 2) ^ (k & 7)) << 4));
+    }
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      if constexpr (NSPLIT == 6) split_bf16_pair(x[2 * j], x[2 * j + 1], hi[j], lo[j]);
+      else hi[j] = pack_bf16_pair(x[2 * j], x[2 * j + 1]);
+    }
+    *reinterpret_cast<uint4*>(dh + kmaj16_off(n, kg * 8)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    if constexpr (NSPLIT == 6) *reinterpret_cast<uint4*>(dl + kmaj16_off(n, kg * 8)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  }
+}
+
 template <class Policy, int NSPLIT>
 __global__ void __launch_bounds__(ENG_THREADS, 1)
 tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
@@ -208,12 +300,15 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
   const uint32_t bar_base = smem_base + Cfg::kBarOff;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
+  auto ready_bar = [&](int s) { return bar_base + 8u * (2 * S + s); };   // Cfg::kBByProducer: B of stage s converted
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = Policy::num_tiles(p);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), ENG_CONSUMERS / 32); }
+    if constexpr (Cfg::kBByProducer)
+      for (int s = 0; s < S; s++) mbar_init(ready_bar(s), ENG_CONVERTERS);
     fence_barrier_init();
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
@@ -222,7 +317,27 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
   griddep_launch();      // the next kernel in the stream may start its own prologue as our CTAs retire ...
   griddep_wait();        // ... and ours ran under the predecessor's tail: from here on its results are visible (common.cuh)
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<kProducerRegs>();   // the whole producer warpgroup, so that the consumers can take the registers
+    if (warp != 0) {
+      if constexpr (Cfg::kBByProducer) {
+        // ---------------------------------------------------------------- B conversion (warps 1-3), in k-block order
+        uint32_t s = 0, ph = 0;
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+          const int nkb = Policy::num_kb(p, tile);
+          for (int kb = 0; kb < nkb; kb++) {
+            mbar_wait(full_bar(s), ph);
+            uint8_t* stage = gen_base + s * Cfg::kStageBytes;
+            engine_convert_b16<NSPLIT, BN>(stage + Cfg::kOffBraw, stage + Cfg::kOffBhi, stage + Cfg::kOffBlo, warp - 1, lane);
+            fence_proxy_async_smem();        // the consumers' wgmma read these tiles through the async proxy
+            __syncwarp();
+            if (lane == 0) mbar_arrive(ready_bar(s));
+            if (++s == S) { s = 0; ph ^= 1; }
+          }
+        }
+      }
+      return;
+    }
     // ------------------------------------------------------------------ TMA producer (whole warp loops, one lane issues)
     const bool leader = elect_one();
     uint32_t kbg = 0;
@@ -242,7 +357,7 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     }
     return;
   }
-  if (warp < 4) return;
+  setmaxnreg_inc<kConsumerRegs>();
 
   // -------------------------------------------------------------------- consumers
   const int ctid = threadIdx.x - 128;                 // 0 .. 255
@@ -254,7 +369,7 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
   const int n0 = (ctid % NG) * 4, kk0 = (ctid / NG) * KR;
   float* epi = reinterpret_cast<float*>(gen_base + Cfg::kOffEpi);
 
-  uint32_t s = 0, ph = 0;
+  uint32_t s = 0, ph = 0, rs = 0;                     // ring position / phase of the next k-block, ring position of the next release
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int nkb = Policy::num_kb(p, tile);
     const typename Policy::Tile tc = Policy::tile(p, tile);
@@ -267,8 +382,9 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
 #pragma unroll
     for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
 
-    for (int kb = 0; kb < nkb; kb++) {
+    auto prep = [&](int, AFrag<NSPLIT>& f, uint32_t& bhi, uint32_t& blo) {
       mbar_wait(full_bar(s), ph);
+      if constexpr (Cfg::kBByProducer) mbar_wait(ready_bar(s), ph);
       uint8_t* stage = gen_base + s * Cfg::kStageBytes;
       const uint32_t stage_s = smem_base + s * Cfg::kStageBytes;
 
@@ -290,7 +406,7 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         }
         fence_proxy_async_smem();
         named_bar_sync(ENG_BAR, ENG_CONSUMERS);
-      } else if constexpr (Cfg::kBMode == B_T32 || Cfg::kBMode == B_T16_FROM32) {
+      } else if constexpr (Cfg::kBMode == B_T32 || (Cfg::kBMode == B_T16_FROM32 && !Cfg::kBByProducer)) {
         // fp32 MN-major tile -> K-major (tf32: as is, or hi | lo; bf16: hi (| lo)); thread: 4 columns x KR k-lines
         const uint8_t* src = stage + (Cfg::kBMode == B_T32 ? Cfg::kOffBhi : Cfg::kOffBraw);
         constexpr int NH = (Cfg::kBMode == B_T32 && !Cfg::kBSplit) ? Cfg::kBHalves : 1;    // pre-split halves transposed as they are
@@ -382,15 +498,19 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         named_bar_sync(ENG_BAR, ENG_CONSUMERS);
       }
 
-      // ---- A fragments + MMAs
+      // ---- A fragments
       const uint8_t* araw = stage;
-      mma_kblock<NSPLIT, BN, !Policy::kAMN, Policy::kSumA>(
-          acc, [&](int r, int k) { return reinterpret_cast<const float*>(araw + a_off<Policy::kAMN>(r, k)); }, r0, r1, q,
-          stage_s + Cfg::kOffBhi, stage_s + Cfg::kOffBlo, asum0, asum1);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(s));
+      build_afrag<NSPLIT, !Policy::kAMN, Policy::kSumA>(
+          f, [&](int r, int k) { return reinterpret_cast<const float*>(araw + a_off<Policy::kAMN>(r, k)); }, r0, r1, q, asum0, asum1);
+      bhi = stage_s + Cfg::kOffBhi;
+      blo = stage_s + Cfg::kOffBlo;
       if (++s == S) { s = 0; ph ^= 1; }
-    }
+    };
+    mma_pipeline<NSPLIT, BN>(acc, nkb, prep, [&](int) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(rs));
+      if (++rs == S) rs = 0;
+    });
 
     // ---- fused reductions
     if constexpr (kSums) {

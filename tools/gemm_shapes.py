@@ -1,10 +1,12 @@
 #!/usr/bin/env python
 """Per-shape timing of the three linear kernels (fwd, dgrad, wgrad) at the cfg2 shapes, through the C ABI.
 
-  python tools/gemm_shapes.py [prec]        # prec: 0 fp32, 1 tf32, 3 3xTF32 (default)
+  python tools/gemm_shapes.py [prec] [--overheads]   # prec: 0 fp32, 1 tf32, 3 3xTF32, 2 bf16, 6 bf16x3 (default)
 
-Prints us per call, fp32-equivalent TFLOP/s (2MNK / t) and, for 3xTF32, the fraction of the tensor-pipe roofline
-(3 tf32 MMAs per product; peak = MEASURED_PEAKS bf16 dense / 2 if present, else 1100 TF/s).
+Prints us per call, algorithmic TFLOP/s (2MNK / t) and the fraction of the tensor-pipe ceiling: the MMAs per product (3 for
+3xTF32 and bf16x3, else 1) times the algorithmic rate, over the dense rate of the MMA type -- bf16 for precisions 2 / 6,
+tf32 (half the bf16 rate) for 1 / 3.  The bf16 rate is MEASURED_PEAKS.json's bf16_tflops if present, else the H100 SXM data
+sheet's 989 TFLOP/s (a figure no kernel reaches).  B200ASR_LIB selects an A/B build of the library.
 """
 import json
 import os
@@ -51,16 +53,19 @@ def overheads(prec):
 
 
 def main():
-    prec = int(sys.argv[1]) if len(sys.argv) > 1 else 3
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    prec = int(args[0]) if args else 6
     if "--overheads" in sys.argv:
         return overheads(prec)
-    peak = 1100.0
+    bf16 = 989.0
     try:
-        peak = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["bf16_tflops"] / 2   # burst figure: each kernel is timed alone
+        bf16 = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["bf16_tflops"]   # burst figure: each kernel is timed alone
     except Exception:
         pass
+    peak = bf16 if prec in (2, 6) else bf16 / 2
+    mult = 3 if prec in (3, 6) else 1
     dev = torch.device("cuda:0")
-    print("prec", prec, "tf32 peak", peak)
+    print("prec", prec, "MMA-type peak", peak, "TF/s, MMAs per product", mult)
     for name, M, N, K in SHAPES:
         x = torch.randn(M, K, device=dev)
         w = torch.randn(N, K, device=dev) * 0.05
@@ -73,7 +78,6 @@ def main():
         t_d = timeit(lambda: ops.linear_bwd_data(dy, w, None, prec, ws))
         t_w = timeit(lambda: ops.linear_bwd_weight(dy, x, True, prec, dw, db))
         fl = 2.0 * M * N * K
-        mult = 3 if prec == 3 else 1
         print("%-10s M=%5d N=%5d K=%5d | fwd %7.1f us %6.1f TF (%.2f) | dgrad %7.1f us %6.1f TF (%.2f) | wgrad %7.1f us %6.1f TF (%.2f)" % (
             name, M, N, K, t_f, fl / t_f / 1e6, mult * fl / t_f / 1e6 / peak, t_d, fl / t_d / 1e6, mult * fl / t_d / 1e6 / peak,
             t_w, fl / t_w / 1e6, mult * fl / t_w / 1e6 / peak))
