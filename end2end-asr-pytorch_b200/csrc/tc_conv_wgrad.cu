@@ -5,25 +5,30 @@
 //
 // Why: the tap-shifted weight gradient (tc_conv.cu, WgradPolicy) covers 128 rows of (tap, ci) per tile, so a pixel block's
 // dy tile is fetched, transposed and split once per tap group (5 or 9 times) and its x data once per tap.  Here a tile is
-// 9 taps x 64 input channels (M = 576, nine m64 row blocks) x 32 output channels: per pixel block of 4 (time) x 8 (freq)
+// 9 taps x 64 input channels (M = 576, nine m64 row blocks) x 64 output channels: per pixel block of 4 (time) x 8 (freq)
 // the CTA loads the x patch including its one-pixel halo -- 6 x 10 pixels x 64 channels, TMA zero fill = padding -- and
 // the dy tile once, converts dy once for all nine taps, and the taps are nine shifted row mappings of the patch, exactly
 // as in the halo forward convolution (tc_conv_halo.cu).
 //
-// Roles (416 threads, 1 CTA / SM, one tile per CTA):
-//   warpgroups 0, 1, 2     consumers: warpgroup w owns taps 3w .. 3w + 2 (df = w - 1, dt = -1 .. 1), i.e. three m64n32
-//                          accumulator blocks.  Per (tap, 8-pixel k-step) a thread reads its four patch elements, splits
-//                          them into tf32 hi | lo fragments and issues the MMAs asynchronously; fragments are double
-//                          buffered, so the next k-step is built while the previous one's MMAs run (wgmma.wait_group 1).
-//   warp 12                producer: TMA of the x patch + dy tile of each pixel block into a ring of stages, and the dy
-//                          conversion -- raw MN-major tile -> K-major hi | lo in the same stage, once for all nine taps,
-//                          with the bias-gradient column sums on the way; it signals the consumers through an mbarrier.
+// Roles (512 threads, 1 CTA / SM, one tile per CTA):
+//   warpgroup 0            producer: warp 0 issues the TMA of the x patch + dy tile of each pixel block into a ring of
+//                          stages; warps 0-3 convert dy -- raw MN-major tile -> K-major hi | lo in the same stage, once for
+//                          all nine taps, with the bias-gradient column sums on the way -- and signal the consumers through
+//                          an mbarrier.
+//   warpgroups 1, 2, 3     consumers: warpgroup w owns taps 3 (w - 1) .. 3 (w - 1) + 2 (df = w - 2, dt = -1 .. 1), i.e. three
+//                          m64n64 accumulator blocks.  Per (tap, 8-pixel k-step) a thread reads its four patch elements
+//                          while the previous k-step's MMAs run, waits for them (wgmma.wait_group 0), splits the elements
+//                          into tf32 hi | lo fragments and issues the MMAs asynchronously.  One fragment buffer: the three
+//                          warpgroups keep the tensor cores fed between each other's waits.
+// The producer warpgroup gives registers to the consumers (setmaxnreg), which need 96 for the accumulators alone.  Even so
+// ptxas (CUDA 12.9) allocates the consumers barely past 128 registers at 512 threads: it spills a few registers once per
+// pixel block and reports C7512 (serialized wgmma) for this kernel.  A second fragment buffer spills more.
 //
 // Contraction order inside a k-step: MMA k position j of step ks is pixel (time ks, freq 2j) for j < 4 and (ks, 2j - 7)
 // for j >= 4, so the four lanes q of a quad read patch columns 2q (+1): distinct 128-byte swizzle phases, no bank conflicts.
 // The dy conversion writes B in the same order.
 //
-// Each tile reduces one contiguous range of pixel blocks (its split) and writes its 576 x 32 partial to the split's slot of
+// Each tile reduces one contiguous range of pixel blocks (its split) and writes its 576 x 64 partial to the split's slot of
 // [splits][9][Ci][Co]; reduce_parts sums the splits in a fixed order (no floating-point atomics: bit-reproducible).
 #include "../../include/b200asr.h"
 #include "common.cuh"
@@ -38,12 +43,17 @@ constexpr int WH_T = 4, WH_F = 8;                        // pixel block = one 32
 constexpr int WH_PT = WH_T + 2, WH_PF = WH_F + 2;        // x patch incl. halo: 6 x 10 pixels
 constexpr int WH_PATCH_BOX = WH_PT * WH_PF * 128;        // 7,680 B per 32-channel box
 constexpr int WH_PATCH_CHUNK = 8192;                     // boxes on 1024-byte boundaries (128B swizzle phase = row & 7)
-constexpr int WH_N = 32;                                 // output channels per tile
-// three consumer warpgroups (warps 0-11) and one producer warp.  13 warps put 4 on one SM sub-partition, which caps a
-// thread at 128 registers: a consumer's three m64n32 accumulator blocks (48) and double-buffered fragments fit, three
-// m64n64 blocks (96) do not.
-constexpr int WH_CONSUMERS = 384;
-constexpr int WH_THREADS = WH_CONSUMERS + 32;
+constexpr int WH_N = 64;                                 // output channels per tile
+constexpr int WH_PRODUCER = 128;                         // warpgroup 0: TMA (warp 0) and dy conversion (warps 0-3)
+constexpr int WH_CONSUMERS = 384;                        // warpgroups 1-3
+constexpr int WH_THREADS = WH_PRODUCER + WH_CONSUMERS;
+constexpr int WH_CONVERTERS = WH_PRODUCER / 32;
+// Register split (setmaxnreg): __launch_bounds__(512, 1) allots 128 per thread.  One SM sub-partition holds one producer
+// and three consumer warps, 40 + 3 * 152 = 496 <= 512 registers per lane: room for a consumer's three m64n64 accumulator
+// blocks (96) next to its hi | lo fragments and the next k-step's patch elements.
+constexpr int WH_PRODUCER_REGS = 40, WH_CONSUMER_REGS = 152;
+static_assert(WH_PRODUCER * WH_PRODUCER_REGS + WH_CONSUMERS * WH_CONSUMER_REGS <= WH_THREADS * 128, "register split");
+constexpr int WH_BAR_CONV = 1;                           // named barrier of the producer warpgroup (bias partials)
 
 struct WgHaloP {
   float* part;         // [splits][9][Ci][Co] partial weight gradients
@@ -51,19 +61,21 @@ struct WgHaloP {
   int Ci, Co, ncs, ncn, nft, ntt, blocks_per_cta, total_blocks;
 };
 
-// stage: x patch (two 32-channel boxes) | raw dy tile (32-channel chunks, MN-major) | dy hi (| lo) K-major WH_N x 32
+// stage: x patch (two 32-channel boxes) | raw dy tile (two 32-channel chunks, MN-major) | dy hi (| lo) K-major 64 x 32
 template <int NSPLIT> struct WgHaloCfg {
   static constexpr int kOffRaw = 2 * WH_PATCH_CHUNK;
   static constexpr int kOffHi = kOffRaw + (WH_N / 32) * 4096;
   static constexpr int kOffLo = kOffHi + WH_N * 128;
   static constexpr int kStageBytes = kOffHi + (NSPLIT == 3 ? 2 : 1) * WH_N * 128;
   static constexpr int kTxBytes = 2 * WH_PATCH_BOX + (WH_N / 32) * 4096;
-  static constexpr int kBySmem = (ENG_SMEM_CAP - 1024 - 256) / kStageBytes;
+  static constexpr int kBySmem = (ENG_SMEM_CAP - 1024 - 512) / kStageBytes;
   static constexpr int kStages = kBySmem > 8 ? 8 : kBySmem;
   static constexpr int kBarOff = kStages * kStageBytes;
-  static constexpr int kSmemBytes = kBarOff + 256 + 1024;
+  static constexpr int kBiasOff = kBarOff + 256;          // bias partials of converter warps 2, 3 (WH_N floats)
+  static constexpr int kSmemBytes = kBiasOff + 256 + 1024;
   static_assert(kStages >= 3, "stage too large");
   static_assert(3 * 8 * kStages <= 256, "barriers");
+  static_assert(WH_N * 4 <= 256, "bias partials");
   static_assert(kSmemBytes <= ENG_SMEM_CAP, "shared memory");
 };
 
@@ -91,7 +103,7 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; s++) {
       mbar_init(full_bar(s), 1);
-      mbar_init(ready_bar(s), 1);
+      mbar_init(ready_bar(s), WH_CONVERTERS);
       mbar_init(empty_bar(s), WH_CONSUMERS / 32);
     }
     fence_barrier_init();
@@ -102,11 +114,12 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   griddep_launch();      // programmatic dependent launch, see common.cuh
   griddep_wait();
 
-  if (warp == WH_CONSUMERS / 32) {
-    // ------------------------------------------------------------------ producer: TMA + dy conversion
-    // The loads run S - 1 pixel blocks ahead of the conversion.  (Not S: the stage of block kb + S is free only once the
-    // consumers have moved on to block kb + 1, which waits for this warp's conversion of it.)
-    const bool leader = elect_one();
+  if (warp < WH_CONVERTERS) {
+    // ------------------------------------------------------------------ producer: TMA (warp 0) + dy conversion (warps 0-3)
+    setmaxnreg_dec<WH_PRODUCER_REGS>();
+    // The loads run S - 1 pixel blocks ahead of warp 0's conversion.  (Not S: the stage of block kb + S is free only once
+    // the consumers have moved on to block kb + 1, which waits for this warpgroup's conversion of it.)
+    const bool leader = elect_one() && warp == 0;
     int ft = blk0 % p.nft, tt = (blk0 / p.nft) % p.ntt, b = blk0 / (p.nft * p.ntt);   // pixel-block cursor, ft fastest
     uint32_t ls = 0, lph = 0;                          // ring position / phase of the next load
     int loaded = 0;
@@ -129,48 +142,54 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
       if (++ls == S) { ls = 0; lph ^= 1; }
       loaded++;
     };
-    while (loaded < nkb && loaded < S - 1) load_next();
-    // dy conversion: lane = output channels n = lane (+ 32 ...); bias-gradient column sums on the way
-    float bs[WH_N / 32][4] = {};
+    if (warp == 0)
+      while (loaded < nkb && loaded < S - 1) load_next();
+    // dy conversion: warp w converts output channel n = (w & 1) * 32 + lane at k = 16 (w >> 1) .. + 15 (time rows 2 (w >> 1)
+    // and + 1); bias-gradient column sums on the way
+    const int c = warp & 1, kg0 = (warp >> 1) * 4, n = c * 32 + lane;
+    float bs[4] = {0.f, 0.f, 0.f, 0.f};
     uint32_t s = 0, ph = 0;
     for (int kb = 0; kb < nkb; kb++) {
       mbar_wait(full_bar(s), ph);
       uint8_t* stage = gen_base + s * Cfg::kStageBytes;
+      const uint8_t* raw = stage + Cfg::kOffRaw + c * 4096 + (lane & 3) * 4;
 #pragma unroll
-      for (int c = 0; c < WH_N / 32; c++) {
-        const int n = c * 32 + lane;
-        const uint8_t* raw = stage + Cfg::kOffRaw + c * 4096 + (lane & 3) * 4;
+      for (int kk = 0; kk < 4; kk++) {            // K-major k = 4 kg .. 4 kg + 3 (see the contraction order above)
+        const int kg = kg0 + kk;
+        float x[4], h[4], l[4];
 #pragma unroll
-        for (int kg = 0; kg < 8; kg++) {          // K-major k = 4 kg .. 4 kg + 3 (see the contraction order above)
-          float x[4], h[4], l[4];
-#pragma unroll
-          for (int i = 0; i < 4; i++) {
-            const int pix = (kg >> 1) * WH_F + 2 * i + (kg & 1);
-            x[i] = *reinterpret_cast<const float*>(raw + pix * 128 + (((lane >> 2) ^ (pix & 7)) << 4));
-            bs[c][i] += x[i];
-            h[i] = NSPLIT == 3 ? tf32_rn(x[i]) : x[i];
-            l[i] = x[i] - h[i];
-          }
-          *reinterpret_cast<float4*>(stage + Cfg::kOffHi + kmaj32_off(n, 4 * kg)) = make_float4(h[0], h[1], h[2], h[3]);
-          if constexpr (NSPLIT == 3)
-            *reinterpret_cast<float4*>(stage + Cfg::kOffLo + kmaj32_off(n, 4 * kg)) = make_float4(l[0], l[1], l[2], l[3]);
+        for (int i = 0; i < 4; i++) {
+          const int pix = (kg >> 1) * WH_F + 2 * i + (kg & 1);
+          x[i] = *reinterpret_cast<const float*>(raw + pix * 128 + (((lane >> 2) ^ (pix & 7)) << 4));
+          bs[i] += x[i];
+          h[i] = NSPLIT == 3 ? tf32_rn(x[i]) : x[i];
+          l[i] = x[i] - h[i];
         }
+        *reinterpret_cast<float4*>(stage + Cfg::kOffHi + kmaj32_off(n, 4 * kg)) = make_float4(h[0], h[1], h[2], h[3]);
+        if constexpr (NSPLIT == 3)
+          *reinterpret_cast<float4*>(stage + Cfg::kOffLo + kmaj32_off(n, 4 * kg)) = make_float4(l[0], l[1], l[2], l[3]);
       }
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(ready_bar(s));
       if (++s == S) { s = 0; ph ^= 1; }
-      if (loaded < nkb) load_next();
+      if (warp == 0 && loaded < nkb) load_next();
     }
-    // every pixel block is visited once by the input-channel-slice-0 tiles (over all splits)
-    if (p.bpart && ci0 == 0)
-#pragma unroll
-      for (int c = 0; c < WH_N / 32; c++) p.bpart[(size_t)z * p.Co + co0 + c * 32 + lane] = (bs[c][0] + bs[c][1]) + (bs[c][2] + bs[c][3]);
+    // every pixel block is visited once by the input-channel-slice-0 tiles (over all splits); channel n's sum is warp
+    // (n / 32)'s time rows 0-1 plus warp (n / 32 + 2)'s rows 2-3, added in that order
+    if (p.bpart && ci0 == 0) {
+      float* bx = reinterpret_cast<float*>(gen_base + Cfg::kBiasOff);
+      const float v = (bs[0] + bs[1]) + (bs[2] + bs[3]);
+      if (warp >= 2) bx[n] = v;
+      named_bar_sync(WH_BAR_CONV, WH_PRODUCER);
+      if (warp < 2) p.bpart[(size_t)z * p.Co + co0 + n] = v + bx[n];
+    }
     return;
   }
+  setmaxnreg_inc<WH_CONSUMER_REGS>();
 
   // -------------------------------------------------------------------- consumers
-  const int wg = threadIdx.x >> 7, cw = warp & 3;
+  const int wg = (threadIdx.x - WH_PRODUCER) >> 7, cw = warp & 3;
   const int g = lane >> 2, q = lane & 3;
   // A rows of this thread in each tap block: input channels cw * 16 + g and + 8 (same 32-channel box, swizzle chunks cch
   // and cch + 2); tap 3 * wg + j reads patch row R + pcol, R = (t + j) * WH_PF + h, for pixel (t, 2q + h).  Its 128B
@@ -188,7 +207,7 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   for (int j = 0; j < 3; j++)
 #pragma unroll
     for (int i = 0; i < WH_N / 2; i++) acc[j][i] = 0.f;
-  uint32_t ah[2][4] = {}, al[2][4] = {};
+  uint32_t ah[4], al[4];
   uint32_t s = 0, ph = 0;
   for (int kb = 0; kb < nkb; kb++) {
     mbar_wait(full_bar(s), ph);
@@ -204,30 +223,30 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
     for (int j = 0; j < 3; j++) {
 #pragma unroll
       for (int ks = 0; ks < 4; ks++) {
-        const int u = (j * 4 + ks) & 1;
         const int r = (ks + j) * WH_PF;
-        // fragment: a0 = (row g, pixel 2q), a1 = (g + 8, 2q), a2 = (g, 2q + 1), a3 = (g + 8, 2q + 1) of time row ks
+        // fragment: a0 = (row g, pixel 2q), a1 = (g + 8, 2q), a2 = (g, 2q + 1), a3 = (g + 8, 2q + 1) of time row ks;
+        // loaded while the previous k-step's MMAs run
         const float x[4] = {ld(r, 0), ld(r, 1), ld(r + 1, 0), ld(r + 1, 1)};
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const float h = tf32_rn(x[i]);
-          ah[u][i] = __float_as_uint(h);
-          al[u][i] = __float_as_uint(x[i] - h);
-        }
-        wgmma_fence();
-        if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
-          wgmma_tf32<WH_N>(acc[j], al[u], kmajor_desc_tf32(bhi + ks * 32));
-          wgmma_tf32<WH_N>(acc[j], ah[u], kmajor_desc_tf32(blo + ks * 32));
-        }
-        wgmma_tf32<WH_N>(acc[j], ah[u], kmajor_desc_tf32(bhi + ks * 32));
-        wgmma_commit();
-        wgmma_wait<1>();                        // the previous k-step's MMAs are done: its fragment buffer is free
-        keep_live(ah[u ^ 1]);                   // (so far: the compiler must not reuse those registers while they run)
-        keep_live(al[u ^ 1]);
+        wgmma_wait<0>();                        // the previous k-step's MMAs are done: the fragment registers are free
+        keep_live(ah);                          // (so far: the compiler must not reuse those registers while they run)
+        if constexpr (NSPLIT == 3) keep_live(al);
         if (j == 0 && ks == 0 && kb > 0) {      // ... and they were the last ones to read the previous stage
           __syncwarp();
           if (lane == 0) mbar_arrive(empty_bar(s == 0 ? S - 1 : s - 1));
         }
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          const float h = tf32_rn(x[i]);
+          ah[i] = __float_as_uint(h);
+          if constexpr (NSPLIT == 3) al[i] = __float_as_uint(x[i] - h);
+        }
+        wgmma_fence();
+        if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
+          wgmma_tf32<WH_N>(acc[j], al, kmajor_desc_tf32(bhi + ks * 32));
+          wgmma_tf32<WH_N>(acc[j], ah, kmajor_desc_tf32(blo + ks * 32));
+        }
+        wgmma_tf32<WH_N>(acc[j], ah, kmajor_desc_tf32(bhi + ks * 32));
+        wgmma_commit();
       }
     }
     if (++s == S) { s = 0; ph ^= 1; }
@@ -289,7 +308,7 @@ int conv3x3_wgrad_tc_halo(const float* x, const float* dy, float* dwr, int B, in
   const long long total = (long long)B * p.nft * p.ntt;
   B200_REQUIRE(total < (1LL << 31), B200ASR_BAD_SHAPE, "conv3x3_wgrad_tc_halo: too many pixel blocks");
   p.total_blocks = (int)total;
-  // one wave: about one tile per SM over the channel groups, at least 32 pixel blocks per tile
+  // one wave: about one tile per SM over the (Ci / 64) x (Co / 64) channel groups, at least 32 pixel blocks per tile
   const int groups = p.ncs * p.ncn;
   p.blocks_per_cta = max(32, ceil_div(p.total_blocks, max(1, device_sm_count() / groups)));
   const int splits = ceil_div(p.total_blocks, p.blocks_per_cta);

@@ -106,7 +106,7 @@ def step(src, dst_md, dst_json=None):
 
 
 # C-ABI kernel group (bench.py's roofline.kernel) -> substrings of the kernel names that implement it
-GROUPS = {"conv3x3_bwd_weight": ["WgradPolicy"], "conv3x3_fwd": ["tc_conv3x3_halo"], "conv3x3_fwd_pool": ["tc_conv3x3_halo"], "conv3x3_bwd_data": ["tc_conv3x3_halo"],
+GROUPS = {"conv3x3_bwd_weight": ["tc_conv3x3_wgrad"], "conv3x3_fwd": ["tc_conv3x3_halo"], "conv3x3_fwd_pool": ["tc_conv3x3_halo"], "conv3x3_bwd_data": ["tc_conv3x3_halo"],
           "linear_fwd": ["GemmPolicy<0, 0", "GemmPolicy<false, false"], "linear_bwd_data": ["GemmPolicy<0, 0", "GemmPolicy<false, false", "GemmPolicy<false, true"],
           "linear_bwd_weight": ["GemmPolicy<1, 1", "GemmPolicy<true, true"],
           "sdpa_mat_fwd": ["BGemmPolicy", "softmax_fwd"], "sdpa_mat_bwd": ["BGemmPolicy", "softmax_bwd"],
