@@ -97,6 +97,9 @@ SIGNATURES = {
     "b200asr_ce_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "b200asr_ce_finalize": (_i, [_vp, _vp, _i, _vp]),
     "b200asr_ce_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _f, _vp, _vp, _vp]),
+    "b200asr_ctc_ws_bytes": (_sz, [_i, _i, _i]),
+    "b200asr_ctc_fwd": (_i, [_vp] * 7 + [_i] * 5 + [_vp]),
+    "b200asr_ctc_bwd": (_i, [_vp] * 8 + [_i] * 5 + [_vp]),
     "b200asr_adam_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _i, _f, _vp, _vp]),
     "b200asr_sumsq": (_i, [_vp, _ll, _vp, _vp]),
     "b200asr_grad_scale": (_i, [_vp, _ll, _vp, _f, _vp, _vp, _vp]),

@@ -115,4 +115,67 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// (value, index) max with first-index tie-break
+__device__ __forceinline__ void argmax_combine(float& v, int& i, float ov, int oi) {
+  if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
+}
+
+// Log-sum-exp statistics of one row x[0 .. V-1], reduced by one CTA of THREADS threads: the maximum mx, the first index of
+// it, sumexp = sum of exp(x - mx) and, with SUM_DIFF, sumdiff = sum of (x - mx).  lse = mx + logf(sumexp); a term x - lse is
+// best formed as (x - mx) - logf(sumexp), which stays exact when the whole row shares a large offset.  Every reduction runs
+// in a fixed order, so the bits do not depend on scheduling.  Every thread gets the results; the call ends with a barrier,
+// so it may be repeated in a loop.
+struct RowLse {
+  float mx, sumexp, sumdiff;
+  int amax;
+};
+#ifdef __CUDACC__
+template <int THREADS, bool SUM_DIFF>
+__device__ __forceinline__ RowLse block_row_lse(const float* __restrict__ x, int V) {
+  __shared__ float sv[THREADS / 32];
+  __shared__ int si[THREADS / 32];
+  __shared__ float ss[THREADS / 32];
+  __shared__ float bc[2];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float bv = -INFINITY; int bi = 0x7fffffff;
+  for (int c = tid; c < V; c += THREADS) {
+    float v = x[c];
+    if (v > bv) { bv = v; bi = c; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    argmax_combine(bv, bi, ov, oi);
+  }
+  if (lane == 0) { sv[warp] = bv; si[warp] = bi; }
+  __syncthreads();
+  if (tid == 0) {
+    float v = sv[0]; int i = si[0];
+    for (int w = 1; w < THREADS / 32; w++) argmax_combine(v, i, sv[w], si[w]);
+    bc[0] = v; bc[1] = __int_as_float(i);
+  }
+  __syncthreads();
+  RowLse r;
+  r.mx = bc[0];
+  r.amax = __float_as_int(bc[1]);
+  float e = 0.f, sd = 0.f;
+  for (int c = tid; c < V; c += THREADS) {
+    const float xs = x[c] - r.mx;
+    e += expf(xs);
+    if (SUM_DIFF) sd += xs;
+  }
+  e = warp_sum(e);
+  if (SUM_DIFF) sd = warp_sum(sd);
+  if (lane == 0) { ss[warp] = e; if (SUM_DIFF) sv[warp] = sd; }
+  __syncthreads();
+  float t = 0.f, sumd = 0.f;
+  for (int w = 0; w < THREADS / 32; w++) { t += ss[w]; if (SUM_DIFF) sumd += sv[w]; }
+  r.sumexp = t;
+  r.sumdiff = sumd;
+  __syncthreads();
+  return r;
+}
+#endif
+
 }  // namespace b200asr

@@ -107,11 +107,6 @@ __global__ void embed_bwd_kernel(const int64_t* __restrict__ tokens, const float
   }
 }
 
-// (value, index) max with first-index tie-break
-__device__ __forceinline__ void argmax_combine(float& v, int& i, float ov, int oi) {
-  if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
-}
-
 __global__ void argmax_rows_kernel(const float* __restrict__ x, int64_t* __restrict__ out, int rows, int V) {
   int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -159,49 +154,15 @@ constexpr int CE_THREADS = 256;
 __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restrict__ logits,
                                                             const int64_t* __restrict__ gold, float* __restrict__ row_lse,
                                                             float* __restrict__ part, int rows, int V, float eps) {
-  __shared__ float sv[CE_THREADS / 32];
-  __shared__ int si[CE_THREADS / 32];
-  __shared__ float ss[CE_THREADS / 32];
-  __shared__ float bc[3];
-  const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int row = blockIdx.x;
   const float* x = logits + (size_t)row * V;
-  float bv = -INFINITY; int bi = 0x7fffffff;
-  for (int c = tid; c < V; c += CE_THREADS) {
-    float v = x[c];
-    if (v > bv) { bv = v; bi = c; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-    int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    argmax_combine(bv, bi, ov, oi);
-  }
-  if (lane == 0) { sv[warp] = bv; si[warp] = bi; }
-  __syncthreads();
-  if (tid == 0) {
-    float v = sv[0]; int i = si[0];
-    for (int w = 1; w < CE_THREADS / 32; w++) argmax_combine(v, i, sv[w], si[w]);
-    bc[0] = v; bc[1] = __int_as_float(i);
-  }
-  __syncthreads();
-  const float mx = bc[0];
-  const int amax = __float_as_int(bc[1]);
   // sum of exp and the sum of the logits, both relative to the row maximum: the loss below is then a combination of
   // terms of the size of the loss itself, whatever offset the logits share (lse - x_g with both ~ 200 would lose 8 bits)
-  float e = 0.f, sd = 0.f;
-  for (int c = tid; c < V; c += CE_THREADS) {
-    const float xs = x[c] - mx;
-    e += expf(xs);
-    sd += xs;
-  }
-  e = warp_sum(e);
-  sd = warp_sum(sd);
-  if (lane == 0) { ss[warp] = e; sv[warp] = sd; }
-  __syncthreads();
-  if (tid == 0) {
-    float t = 0.f, sumd = 0.f;
-    for (int w = 0; w < CE_THREADS / 32; w++) { t += ss[w]; sumd += sv[w]; }
-    const float lt = logf(t);                      // lse - mx
+  const RowLse st = block_row_lse<CE_THREADS, true>(x, V);
+  const float mx = st.mx, sumd = st.sumdiff;
+  const int amax = st.amax;
+  if (threadIdx.x == 0) {
+    const float lt = logf(st.sumexp);              // lse - mx
     row_lse[row] = mx + lt;
     const int64_t g = gold[row];
     float* pr = part + (size_t)row * 3;            // (loss, 1, correct) of this row; zeros for PAD rows

@@ -127,28 +127,12 @@ __global__ void lstm_prepare_kernel(const float* __restrict__ w_ih, const float*
 constexpr int NLL_THREADS = 256;
 __global__ void __launch_bounds__(NLL_THREADS) lm_nll_kernel(const float* __restrict__ logits, long long ld,
                                                              const int64_t* __restrict__ targets, float* __restrict__ nll, int V) {
-  __shared__ float red[NLL_THREADS / 32];
-  const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int row = blockIdx.x;
   const float* x = logits + (size_t)row * ld;
-  float mx = -INFINITY;
-  for (int c = tid; c < V; c += NLL_THREADS) mx = fmaxf(mx, x[c]);
-  mx = warp_max(mx);
-  if (lane == 0) red[warp] = mx;
-  __syncthreads();
-  mx = red[0];
-#pragma unroll
-  for (int w = 1; w < NLL_THREADS / 32; w++) mx = fmaxf(mx, red[w]);
-  __syncthreads();
-  float s = 0.f;
-  for (int c = tid; c < V; c += NLL_THREADS) s += expf(x[c] - mx);
-  s = warp_sum(s);
-  if (lane == 0) red[warp] = s;
-  __syncthreads();
-  if (tid == 0) {
-    float tot = 0.f;
-    for (int w = 0; w < NLL_THREADS / 32; w++) tot += red[w];
+  const RowLse st = block_row_lse<NLL_THREADS, false>(x, V);
+  if (threadIdx.x == 0) {
     const int64_t tg = targets[row];
-    nll[row] = (tg >= 0 && tg < V) ? (mx + logf(tot)) - x[tg] : NAN;
+    nll[row] = (tg >= 0 && tg < V) ? (st.mx + logf(st.sumexp)) - x[tg] : NAN;
   }
 }
 

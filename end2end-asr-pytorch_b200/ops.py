@@ -1406,3 +1406,63 @@ class CrossEntropyFn(torch.autograd.Function):
         L.check(_lib().b200asr_ce_bwd(L.ptr(x), L.ptr(g), L.ptr(lse), L.ptr(dx), rows, V, smoothing, 1.0, L.ptr(gs),
                                       L.ptr(inv_n), _stream()), "ce_bwd")
         return dx.view(shape), None, None, None
+
+
+def _ctc_host_lengths(lengths, B, limit, what):
+    """The lengths of one ctc_loss argument as host ints, checked as torch's ctc_loss checks them: B values in [0, limit].
+    CPU tensors (the reference's `sizes` and loader `tgt_lengths`) need no device sync; device tensors are read back."""
+    if not torch.is_tensor(lengths):
+        lengths = torch.as_tensor(lengths)
+    vals = lengths.detach().reshape(-1).cpu().tolist()
+    if len(vals) != B:
+        raise RuntimeError(f"ctc_loss: expected {what} to have {B} entries, got {len(vals)}")
+    for v in vals:
+        if v < 0:
+            raise RuntimeError(f"ctc_loss: {what} must be non-negative, got {v}")
+        if v > limit:
+            raise RuntimeError(f"ctc_loss: expected {what} to have value at most {limit}, but got value {v}")
+    return vals
+
+
+class CtcLossFn(torch.autograd.Function):
+    """CTC loss of utils/metrics.py:133-154 -- F.ctc_loss(log_softmax(pred.transpose(0, 1), 2), gold, input_lengths,
+    target_lengths, blank=0, reduction="mean") -- from the [B, T, V] logits in place (b200asr_ctc_fwd / _bwd).
+
+    pred: CUDA fp32 [B, T, V]; targets: [B, S] (padded, row b read up to target_lengths[b]); the lengths: [B] integer
+    tensors, validated on the host (0 <= input_lengths <= T, 0 <= target_lengths <= S) and staged through pinned memory,
+    so with CPU lengths neither direction synchronises the host.  Returns the 0-dim mean loss (+inf if some utterance has
+    no alignment; its gradient rows are then NaN, as torch's)."""
+
+    @staticmethod
+    def forward(ctx, pred, targets, input_lengths, target_lengths):
+        _need_cuda(pred, targets)
+        if pred.dim() != 3 or targets.dim() != 2 or targets.shape[0] != pred.shape[0]:
+            raise RuntimeError(f"ctc_loss: expected pred [B, T, V] and targets [B, S], got {tuple(pred.shape)} and "
+                               f"{tuple(targets.shape)}")
+        B, T, V = pred.shape
+        S = targets.shape[1]
+        il = _ctc_host_lengths(input_lengths, B, T, "input_lengths")
+        tl = _ctc_host_lengths(target_lengths, B, S, "target_lengths")
+        lmax = max(tl)
+        dev = pred.device
+        x = _f32c(pred)
+        tg = targets.to(torch.long).contiguous()
+        lens = _pinned_stage.to_device(torch.tensor(il + tl, dtype=torch.int32), dev)
+        lib, st = _lib(), _stream()
+        ws = torch.empty(lib.b200asr_ctc_ws_bytes(B, T, lmax), device=dev, dtype=torch.uint8)
+        nll = torch.empty(B, device=dev, dtype=torch.float32)
+        loss = torch.empty((), device=dev, dtype=torch.float32)
+        L.check(lib.b200asr_ctc_fwd(L.ptr(x), L.ptr(tg), L.ptr(lens), L.ptr(lens[B:]), L.ptr(nll), L.ptr(loss), L.ptr(ws), B, T,
+                                    V, S, lmax, st), "ctc_fwd")
+        ctx.save_for_backward(x, tg, lens, nll, ws)
+        ctx.meta = (pred.shape, lmax)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        x, tg, lens, nll, ws = ctx.saved_tensors
+        (B, T, V), lmax = ctx.meta
+        dx = torch.empty_like(x)
+        L.check(_lib().b200asr_ctc_bwd(L.ptr(x), L.ptr(tg), L.ptr(lens), L.ptr(lens[B:]), L.ptr(nll), L.ptr(_f32c(dloss)),
+                                       L.ptr(dx), L.ptr(ws), B, T, V, tg.shape[1], lmax, _stream()), "ctc_bwd")
+        return dx, None, None, None

@@ -411,6 +411,29 @@ int b200asr_ce_bwd(const float* logits, const int64_t* gold, const float* row_ls
                    b200asr_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * CTC loss, the ctc branch of calculate_loss (utils/metrics.py:133-154, trainer/asr/trainer.py:81-85):
+ *   F.ctc_loss(log_softmax(logits.transpose(0, 1), dim=2), targets, input_lengths, target_lengths, blank=0,
+ *              reduction="mean", zero_infinity=False)
+ * computed from the logits in place, exact fp32, in log space.
+ *   logits [B][T][V] fp32 contiguous; targets [B][S] int64, row b read at 0 .. target_lengths[b] - 1 only, labels in [0, V)
+ *   (label 0 is the blank and allowed: the standard extended-label lattice); input_lengths / target_lengths [B] int32 (device).
+ *   max_target_len >= every target_lengths[b], <= S and <= 4095; lengths must satisfy 0 <= input_lengths[b] <= T and
+ *   0 <= target_lengths[b] <= max_target_len (the caller validates them; an utterance that breaks this gets NaN).
+ *   ws: b200asr_ctc_ws_bytes(B, T, max_target_len) bytes, caller-owned, written by ctc_fwd and read by ctc_bwd (row
+ *   log-sum-exps, the extended-label log-probabilities, the scaled alpha and beta lattices, label chains).
+ * ctc_fwd: nll [B] = -log P(target_b | logits_b) (+inf if no alignment fits in input_lengths[b] frames; 0 when both lengths
+ *   are 0); loss [1] = (sum over b in order of nll[b] / max(target_lengths[b], 1)) / B.
+ * ctc_bwd: dlogits [B][T][V] = d(*dloss * loss) / d logits, with nll from ctc_fwd: rows t >= input_lengths[b] get 0, every
+ *   row t < input_lengths[b] of an utterance with infinite nll gets NaN (as torch's backward).  No host synchronisation;
+ *   reductions in a fixed order, so repeated calls give identical bits. */
+size_t b200asr_ctc_ws_bytes(int B, int T, int max_target_len);
+int b200asr_ctc_fwd(const float* logits, const int64_t* targets, const int32_t* input_lengths, const int32_t* target_lengths,
+                    float* nll, float* loss, void* ws, int B, int T, int V, int S, int max_target_len, b200asr_stream_t stream);
+int b200asr_ctc_bwd(const float* logits, const int64_t* targets, const int32_t* input_lengths, const int32_t* target_lengths,
+                    const float* nll, const float* dloss, float* dlogits, void* ws, int B, int T, int V, int S, int max_target_len,
+                    b200asr_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Step tail ("next" row of SURVEY.md §8f): Adam(betas, eps) with the learning rate supplied by the host
  * (NoamOpt, utils/optimizer.py:15-32; torch.optim.Adam at utils/functions.py:107) over a flat buffer.
  * g is read as g * gscale * (*gscale_dev if non-NULL) -- e.g. 1/global num_word and the clip coefficient.
