@@ -92,6 +92,10 @@ SIGNATURES = {
     "b200asr_beam_backtrack_packed": (_i, [_vp] * 4 + [_i, _vp, _vp, _i, _vp, _i, _i, _i, _vp]),
     "b200asr_lstm_prepare": (_i, [_vp] * 4 + [_i, _i] + [_vp] * 3 + [_vp]),
     "b200asr_lstm_layer_fwd": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "b200asr_lstm_layer_train_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b200asr_lstm_layer_train_bwd": (_i, [_vp] * 7 + [_i, _i, _i] + [_vp] * 4),
+    "b200asr_lstm_dropout": (_i, [_vp, _vp, _ll, _f, _u64, _u64, _vp]),
+    "b200asr_lstm_grad_unprepare": (_i, [_vp] * 3 + [_i, _i] + [_vp] * 5),
     "b200asr_lm_nll": (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp]),
     "b200asr_lm_seq_sum": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
     "b200asr_ce_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),

@@ -3,9 +3,10 @@
     import b200asr; b200asr.install()      # after `utils.constant` has parsed its flags
 
 After this, the reference's own `Transformer` (models/asr/transformer.py), `Trainer` loop
-(trainer/asr/trainer.py) and `test.py` run on libb200asr kernels: module tree, parameter names and checkpoints are
-untouched; only `forward` attributes, `Decoder.beam_search` and the two loss functions are rebound (SURVEY.md §8b).
-The replaced beam_search stays reachable through original(): LM rescoring with an LM other than an LSTM LM still runs it.
+(trainer/asr/trainer.py), `test.py` and the LSTM LM's `RNNModel.forward` (utils/lstm_utils.py) run on libb200asr kernels:
+module tree, parameter names and checkpoints are untouched; only `forward` attributes, `Decoder.beam_search` and the two
+loss functions are rebound (SURVEY.md §8b).  The replaced methods stay reachable through original(): LM rescoring with an
+LM other than an LSTM LM still runs the reference's beam_search, and a GRU / RNN LM its own RNNModel.forward.
 """
 from __future__ import annotations
 
@@ -39,6 +40,12 @@ def install(reference_root: str = None):
         (um, "calculate_metrics", metrics.calculate_metrics),
         (tr, "calculate_metrics", metrics.calculate_metrics),
     ]
+    try:                                                # RNNModel.forward of the LSTM LM (training, LM.evaluate)
+        lu = importlib.import_module("utils.lstm_utils")
+    except ImportError:
+        lu = None
+    if lu is not None:
+        targets.append((lu.RNNModel, "forward", modules.rnn_model_forward))
     t_mod = sys.modules.get("trainer.asr.trainer")      # `from utils.metrics import calculate_metrics` binds by value
     if t_mod is not None:
         targets.append((t_mod, "calculate_metrics", metrics.calculate_metrics))

@@ -729,10 +729,30 @@ class Transformer(nn.Module):
     forward = transformer_forward
 
 
+def rnn_model_forward(self, input, hidden):
+    """RNNModel.forward (utils/lstm_utils.py:185-193) -> (decoded [T, B, ntoken], (h_n, c_n)) for rnn_type "LSTM": the
+    embedding, the LSTM stack and both dropouts on the device (ops.lstm_stack; dropout only in train mode), the decoder
+    through LinearFn.  Other recurrent types and a bidirectional, batch_first or projected LSTM run the reference's own
+    forward (install.original)."""
+    rnn = self.rnn
+    if (getattr(self, "rnn_type", None) != "LSTM" or not isinstance(rnn, nn.LSTM) or rnn.bidirectional or rnn.batch_first
+            or getattr(rnn, "proj_size", 0)):
+        from .install import original
+        ref = original(type(self), "forward")
+        if ref is None:
+            raise NotImplementedError(f"RNNModel.forward runs on the device for a unidirectional, sequence-first LSTM only "
+                                      f"(rnn_type {getattr(self, 'rnn_type', None)!r})")
+        return ref(self, input, hidden)
+    p_drop = float(self.drop.p) if self.training else 0.0
+    p_mid = float(rnn.dropout) if self.training and rnn.num_layers > 1 else 0.0
+    out, hidden = ops.lstm_stack(self, input, hidden, p_emb=p_drop, p_mid=p_mid, p_out=p_drop)
+    return ops.LinearFn.apply(out, self.decoder.weight, self.decoder.bias), hidden
+
+
 class RNNModel(nn.Module):
     """utils/lstm_utils.py:138-201 with rnn_type "LSTM" (the only recurrent LM the reference's rescoring loads): the same
-    submodules and state_dict names (encoder, rnn, decoder), so the reference's checkpoints load.  It holds the parameters
-    of beam-search rescoring, which runs on the device (ops.lstm_lm_nll_sums); it has no forward of its own."""
+    submodules and state_dict names (encoder, rnn, decoder), so the reference's checkpoints load.  Beam-search rescoring
+    runs on the device (ops.lstm_lm_nll_sums); forward (rnn_model_forward) trains it on the device."""
 
     def __init__(self, rnn_type, ntoken, ninp, nhid, nlayers, dropout=0.5, tie_weights=False):
         super().__init__()
@@ -751,6 +771,13 @@ class RNNModel(nn.Module):
             self.encoder.weight.uniform_(-0.1, 0.1)
             self.decoder.bias.zero_()
             self.decoder.weight.uniform_(-0.1, 0.1)
+
+    forward = rnn_model_forward
+
+    def init_hidden(self, bsz):
+        """utils/lstm_utils.py:195-199: the zero state (h0, c0), each [nlayers, bsz, nhid]."""
+        weight = next(self.parameters())
+        return (weight.new_zeros(self.nlayers, bsz, self.nhid), weight.new_zeros(self.nlayers, bsz, self.nhid))
 
 
 class LM:

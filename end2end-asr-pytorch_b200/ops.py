@@ -1235,10 +1235,12 @@ def _pad8(n):
 class LstmLmOperands:
     """Device operands of an LSTM LM (RNNModel("LSTM"): encoder nn.Embedding, rnn nn.LSTM, decoder nn.Linear), built on the
     GPU by b200asr_lstm_prepare / b200asr_split_bf16: the embedding and decoder weights zero-padded to I / H columns, per layer
-    the gate-interleaved bf16x3 W_ih and W_hh operands and the folded bias.  `fresh()` is False once any parameter's version
-    counter (or storage) moved since the operands were built."""
+    the gate-interleaved bf16x3 W_ih and W_hh operands and the folded bias.  `train` (LstmStackFn) also keeps, per layer,
+    W_hh_p and the transposed bf16x3 operands of both matrices for the data gradients (`grad_layers`), and builds no decoder
+    operands (the decoder runs through LinearFn).  `fresh()` is False once any parameter's version counter (or storage)
+    moved since the operands were built."""
 
-    def __init__(self, model, device):
+    def __init__(self, model, device, train=False):
         rnn = model.rnn
         self.ntoken, self.ninp = model.encoder.weight.shape
         self.nhid, self.nlayers = rnn.hidden_size, rnn.num_layers
@@ -1251,13 +1253,15 @@ class LstmLmOperands:
             dv = lambda t: None if t is None else t.detach().to(**f32).contiguous()
             self.emb = torch.zeros((self.ntoken, self.I), **f32)
             self.emb[:, :self.ninp] = dv(model.encoder.weight)
-            dec = torch.zeros((self.ntoken, self.H), **f32)
-            dec[:, :self.nhid] = dv(model.decoder.weight)
-            self.dec_b = dv(model.decoder.bias) if model.decoder.bias is not None else torch.zeros(self.ntoken, **f32)
-            self.dec_split = self._split(dec)
-            self.dec = dec
+            self.dec = self.dec_b = self.dec_split = None
+            if not train:
+                dec = torch.zeros((self.ntoken, self.H), **f32)
+                dec[:, :self.nhid] = dv(model.decoder.weight)
+                self.dec_b = dv(model.decoder.bias) if model.decoder.bias is not None else torch.zeros(self.ntoken, **f32)
+                self.dec_split = self._split(dec)
+                self.dec = dec
             self.zero_pe = torch.zeros((1, self.I), **f32)
-            self.layers = []
+            self.layers, self.grad_layers = [], []
             for l in range(self.nlayers):
                 K = self.I if l == 0 else self.H
                 kin = self.ninp if l == 0 else self.nhid
@@ -1268,7 +1272,11 @@ class LstmLmOperands:
                 w_ih, w_hh, b_ih, b_hh = g("weight_ih"), g("weight_hh"), g("bias_ih"), g("bias_hh")
                 L.check(_lib().b200asr_lstm_prepare(L.ptr(w_ih), L.ptr(w_hh), L.ptr(b_ih), L.ptr(b_hh), kin, self.nhid, L.ptr(w_ih_p),
                                                     L.ptr(w_hh_p), L.ptr(bias_p), _stream()), "lstm_prepare")
-                self.layers.append((w_ih_p, self._split(w_ih_p), self._split(w_hh_p), bias_p))
+                ih, ih_t = self._split(w_ih_p, train)
+                hh, hh_t = self._split(w_hh_p, train)
+                self.layers.append((w_ih_p, ih, hh, bias_p))
+                if train:
+                    self.grad_layers.append((w_hh_p, ih_t, hh_t))
 
     def _stamp(self):
         return [(p.data_ptr(), p._version) for p in self.params]
@@ -1277,15 +1285,18 @@ class LstmLmOperands:
         return self._stamp() == self.stamp
 
     @staticmethod
-    def _split(w):
+    def _split(w, transposed=None):
+        """bf16x3 operand [2][N][K] of w [N, K]; with `transposed` given (False / True), the pair (that, the transposed
+        operand [2][K][N] or None)."""
         N, K = w.shape
         out = torch.empty((2, N, K), device=w.device, dtype=torch.bfloat16)
-        L.check(_lib().b200asr_split_bf16(L.ptr(w), L.ptr(out), None, N, K, 2, _stream()), "split_bf16")
-        return out
+        out_t = torch.empty((2, K, N), device=w.device, dtype=torch.bfloat16) if transposed else None
+        L.check(_lib().b200asr_split_bf16(L.ptr(w), L.ptr(out), L.ptr(out_t), N, K, 2, _stream()), "split_bf16")
+        return out if transposed is None else (out, out_t)
 
 
 def lstm_lm_operands(model, device) -> LstmLmOperands:
-    """The LM's prepared operands, cached on the module and rebuilt when a parameter changed in place."""
+    """The LM's prepared rescoring operands, cached on the module and rebuilt when a parameter changed in place."""
     device = torch.device(device)
     if device.index is None:
         device = torch.device(device.type, torch.cuda.current_device())
@@ -1367,6 +1378,161 @@ def lstm_lm_nll_sums(model, seqs, device):
     out = np.empty(n, dtype=np.float32)
     out[order] = sums.cpu().numpy()
     return out
+
+
+def _lstm_check(model, input, hidden):
+    """The argument checks of lstm_stack (ValueError), made before anything is launched."""
+    if not torch.is_tensor(input) or input.dtype != torch.int64 or input.dim() != 2 or min(input.shape) < 1:
+        raise ValueError("RNNModel.forward: input must be an int64 tensor [T, B] with T, B >= 1, got "
+                         f"{getattr(input, 'dtype', type(input))} {tuple(getattr(input, 'shape', ()))}")
+    dev = model.encoder.weight.device
+    if not input.is_cuda or input.device != dev:
+        raise ValueError(f"RNNModel.forward: input is on {input.device}, the model on {dev} (a CUDA device is required)")
+    if hidden is None:
+        return
+    if not isinstance(hidden, (tuple, list)) or len(hidden) != 2:
+        raise ValueError("RNNModel.forward: hidden must be the pair (h0, c0)")
+    want = (model.rnn.num_layers, input.shape[1], model.rnn.hidden_size)
+    for name, t in zip(("h0", "c0"), hidden):
+        if not torch.is_tensor(t) or t.dtype != torch.float32 or tuple(t.shape) != want or t.device != dev:
+            raise ValueError(f"RNNModel.forward: {name} must be float32 {list(want)} on {dev}, got "
+                             f"{getattr(t, 'dtype', type(t))} {list(getattr(t, 'shape', ()))} on {getattr(t, 'device', None)}")
+
+
+def _pad_rows(x, H):
+    """x [..., n] -> contiguous fp32 [rows, H] with zero columns n .. H-1."""
+    x2 = x.reshape(-1, x.shape[-1])
+    if x2.shape[1] == H:
+        return x2.contiguous()
+    out = torch.zeros((x2.shape[0], H), device=x.device, dtype=torch.float32)
+    out[:, :x2.shape[1]] = x2
+    return out
+
+
+class LstmStackFn(torch.autograd.Function):
+    """drop(nn.LSTM(drop(encoder(input)), (h0, c0))) of RNNModel("LSTM").forward (utils/lstm_utils.py:185-190) and its
+    backward through time, in the prepared layout of LstmLmOperands(train=True).
+
+    Per layer: the input projection (one bf16x3 GEMM over all T * B rows), b200asr_lstm_layer_train_fwd (gates and cell
+    states saved), the dropout of the layer output (between layers: nn.LSTM's, after the last: the model's).  Backward, per
+    layer from the top: the output's mask applied again, b200asr_lstm_layer_train_bwd, the weight and bias gradients as
+    fixed-order split-K bf16x3 GEMMs, b200asr_lstm_grad_unprepare back to nn.LSTM's layout, dh0 and the input gradient as
+    data-gradient GEMMs; the embedding gradient through b200asr_embed_bwd.  Returns (output [T, B, nhid], h_n, c_n)."""
+
+    @staticmethod
+    def forward(ctx, op, input, h0, c0, p_emb, p_mid, p_out, enc_w, *rnn_params):
+        T, B = input.shape
+        H, I, nl = op.H, op.I, op.nlayers
+        lib, st = _lib(), _stream()
+        dev = input.device
+        f32 = dict(device=dev, dtype=torch.float32)
+        inp = input.contiguous().view(-1)
+        x = torch.empty((T * B, I), **f32)
+        emb_key = rng.next() if p_emb > 0.0 else (0, 0)
+        L.check(lib.b200asr_embed_fwd(L.ptr(inp), L.ptr(op.emb), L.ptr(op.zero_pe), L.ptr(x), T * B, 1, I, op.ntoken, 1.0,
+                                      float(p_emb), emb_key[0], emb_key[1], st), "embed_fwd")
+        has_state = h0 is not None
+        h0p = _pad_rows(h0, H).view(nl, B, H) if has_state else None
+        c0p = _pad_rows(c0, H).view(nl, B, H) if has_state else None
+        saved, keys = [], []
+        for l, (w_ih_p, ih_split, hh_split, bias_p) in enumerate(op.layers):
+            xproj = linear_fwd(x, w_ih_p, bias_p, False, L.PREC_BF16X3, WSplit(ih_split, None))
+            h = torch.empty(((T + 1) * B, H), **f32)
+            c = torch.empty((T * B, H), **f32)
+            gates = torch.empty((T * B, 4 * H), **f32)
+            if has_state:
+                h[:B] = h0p[l]
+            L.check(lib.b200asr_lstm_layer_train_fwd(L.ptr(xproj), L.ptr(hh_split), T, B, H, int(has_state),
+                                                     L.ptr(c0p[l]) if has_state else None, L.ptr(h), L.ptr(c), L.ptr(gates), st),
+                    "lstm_layer_train_fwd")
+            saved += [x, h, c, gates]
+            y = h[B:]
+            p = float(p_mid if l < nl - 1 else p_out)
+            key = rng.next() if p > 0.0 else None
+            if key is not None:
+                yd = torch.empty_like(y)
+                L.check(lib.b200asr_lstm_dropout(L.ptr(y), L.ptr(yd), y.numel(), p, key[0], key[1], st), "lstm_dropout")
+                y = yd
+            keys.append((p, key))
+            x = y
+        n = op.nhid
+        out = x.view(T, B, H)[:, :, :n]
+        h_n = torch.stack([saved[4 * l + 1][T * B:, :n] for l in range(nl)])
+        c_n = torch.stack([saved[4 * l + 2][(T - 1) * B:, :n] for l in range(nl)])
+        ctx.save_for_backward(inp, c0p, *saved)
+        ctx.op, ctx.keys, ctx.emb_key, ctx.p_emb, ctx.TB = op, keys, emb_key, float(p_emb), (T, B)
+        if n != H or keys[-1][1] is None:        # (otherwise out views a saved buffer)
+            out = out.clone(memory_format=torch.contiguous_format)
+        return out, h_n, c_n
+
+    @staticmethod
+    def backward(ctx, d_out, d_hn, d_cn):
+        inp, c0p, *saved = ctx.saved_tensors
+        op, (T, B) = ctx.op, ctx.TB
+        H, I, nl, n = op.H, op.I, op.nlayers, op.nhid
+        lib, st = _lib(), _stream()
+        f32 = dict(device=inp.device, dtype=torch.float32)
+        need = ctx.needs_input_grad
+        grads = [None] * (4 * nl)
+        dh0 = torch.zeros((nl, B, n), **f32) if need[2] else None
+        dc0 = torch.zeros((nl, B, n), **f32) if need[3] else None
+        dy = _pad_rows(d_out, H) if d_out is not None else torch.zeros((T * B, H), **f32)
+        need_emb = need[7]
+        for l in range(nl - 1, -1, -1):
+            x, h, c, gates = saved[4 * l:4 * l + 4]
+            w_ih_p, _, _, _ = op.layers[l]
+            w_hh_p, ih_t, hh_t = op.grad_layers[l]
+            p, key = ctx.keys[l]
+            if key is not None:
+                dym = torch.empty_like(dy)
+                L.check(lib.b200asr_lstm_dropout(L.ptr(dy), L.ptr(dym), dy.numel(), p, key[0], key[1], st), "lstm_dropout")
+                dy = dym
+            dh_n = _pad_rows(d_hn[l], H) if d_hn is not None else None
+            dc_n = _pad_rows(d_cn[l], H) if d_cn is not None else None
+            dgates = torch.empty((T * B, 4 * H), **f32)
+            dc = torch.empty((B, H), **f32)
+            dc0p = torch.empty((B, H), **f32) if dc0 is not None else None
+            L.check(lib.b200asr_lstm_layer_train_bwd(L.ptr(gates), L.ptr(c), L.ptr(c0p[l]) if c0p is not None else None, L.ptr(dy),
+                                                     L.ptr(dh_n), L.ptr(dc_n), L.ptr(hh_t), T, B, H, L.ptr(dc), L.ptr(dgates),
+                                                     L.ptr(dc0p), st), "lstm_layer_train_bwd")
+            if dc0 is not None:
+                dc0[l] = dc0p[:, :n]
+            if dh0 is not None:
+                dh0[l] = linear_bwd_data(dgates[:B], w_hh_p, None, L.PREC_BF16X3, WSplit(None, hh_t))[:, :n]
+            pw = [need[8 + 4 * l + j] for j in range(4)]
+            if any(pw):
+                kin = op.ninp if l == 0 else n
+                dw_ih_p, db_p = linear_bwd_weight(dgates, x, True, L.PREC_BF16X3)
+                dw_hh_p, _ = linear_bwd_weight(dgates, h[:T * B], False, L.PREC_BF16X3)
+                g = [torch.empty((4 * n, kin), **f32) if pw[0] else None, torch.empty((4 * n, n), **f32) if pw[1] else None,
+                     torch.empty(4 * n, **f32) if pw[2] else None, torch.empty(4 * n, **f32) if pw[3] else None]
+                L.check(lib.b200asr_lstm_grad_unprepare(L.ptr(dw_ih_p), L.ptr(dw_hh_p), L.ptr(db_p), kin, n, *[L.ptr(t) for t in g], st),
+                        "lstm_grad_unprepare")
+                grads[4 * l:4 * l + 4] = g
+            if l > 0 or need_emb:
+                dy = linear_bwd_data(dgates, w_ih_p, None, L.PREC_BF16X3, WSplit(None, ih_t))
+        d_enc = None
+        if need_emb:
+            dtable = torch.zeros((op.ntoken, I), **f32)
+            L.check(lib.b200asr_embed_bwd(L.ptr(inp), L.ptr(dy), L.ptr(dtable), T * B, I, op.ntoken, 1.0, ctx.p_emb, ctx.emb_key[0],
+                                          ctx.emb_key[1], -1, st), "embed_bwd")
+            d_enc = dtable[:, :op.ninp] if I != op.ninp else dtable
+        return (None, None, dh0, dc0, None, None, None, d_enc, *grads)
+
+
+def lstm_stack(model, input, hidden, p_emb=0.0, p_mid=0.0, p_out=0.0):
+    """The embedding, the LSTM and the output dropout of RNNModel("LSTM").forward on the device (LstmStackFn): input int64
+    [T, B], hidden (h0, c0) fp32 [nlayers, B, nhid] or None (zero state); p_emb / p_mid / p_out are the dropout
+    probabilities of the embedding, between layers and of the last layer's output.  Returns (output, (h_n, c_n))."""
+    _lstm_check(model, input, hidden)
+    rnn = model.rnn
+    # prepared on every call, not cached by version stamp: the word-language-model loop updates the weights through
+    # `p.data`, which leaves the parameters' version counters unchanged (and in training they change every step anyway)
+    op = LstmLmOperands(model, input.device, train=True)
+    params = [getattr(rnn, f"{nm}_l{l}", None) for l in range(rnn.num_layers) for nm in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")]
+    h0, c0 = hidden if hidden is not None else (None, None)
+    out, h_n, c_n = LstmStackFn.apply(op, input, h0, c0, float(p_emb), float(p_mid), float(p_out), model.encoder.weight, *params)
+    return out, (h_n, c_n)
 
 
 class CrossEntropyFn(torch.autograd.Function):

@@ -396,6 +396,33 @@ int b200asr_lstm_prepare(const float* w_ih, const float* w_hh, const float* b_ih
                          float* w_ih_p, float* w_hh_p, float* bias_p, b200asr_stream_t stream);
 int b200asr_lstm_layer_fwd(const float* xproj, const void* w_hh_split, const int32_t* batch_sizes, int T, int H, float* c, float* h,
                            b200asr_stream_t stream);
+/* LSTM LM training: RNNModel("LSTM").forward (utils/lstm_utils.py:185-193) and its backward through time, replacing the
+ * nn.LSTM of :147 (cuDNN).  One layer over a fixed batch of B sequences and T steps, rows t-major (row t * B + b).
+ *   lstm_layer_train_fwd: xproj [T*B][4H] as for lstm_layer_fwd; h [(T+1)*B][H] with slot 0 (rows 0 .. B-1) = h0 -- read
+ *     when has_state (then c0 [B][H] is read too), written as 0 otherwise -- and slot t + 1 = h_t, so that rows 0 .. T*B-1
+ *     are h_{t-1} for every t; c [T*B][H] = c_t of every step; gates [T*B][4H] = the activated gates i, f, g, o of every step
+ *     (gate-interleaved).  Step 0 is one tensor-core launch of h0 W_hh^T with a state, the zero-state cell without.  The
+ *     same recurrence loop as lstm_layer_fwd, whose results it leaves bit-identical.
+ *   lstm_layer_train_bwd: from the saved gates, c and c0 (NULL: zero state) and dh_out [T*B][H] (the gradient of every
+ *     h_t from above), dh_n / dc_n [B][H] (the gradients of the final state; NULL = 0): dgates [T*B][4H] = the gradients of
+ *     the gate pre-activations (interleaved), dc0 [B][H] = the gradient of c0 (NULL: not wanted), dc [B][H] workspace.
+ *     Step T - 1 is an elementwise kernel; every earlier step one tensor-core launch of dgates_{t+1} W_hh_p (bf16x3,
+ *     w_hh_split_t = the transposed operand dst_t [2][H][4H] of b200asr_split_bf16(w_hh_p, .., 4H, H, 2)) whose epilogue is
+ *     the exact-fp32 cell backward.  The parameter gradients are then b200asr_linear_bwd_weight(dgates, x | h rows
+ *     0 .. T*B-1), dh0 = b200asr_linear_bwd_data(dgates rows 0 .. B-1, w_hh_p) and dx = b200asr_linear_bwd_data(dgates,
+ *     w_ih_p).  H % 8 == 0.
+ *   lstm_dropout: y[i] = x[i] / (1 - p) or 0, kept by the counter-based generator keyed by (seed, offset) at element index
+ *     i (the generator of b200asr_embed_fwd); applied to a gradient with the same key it is the backward.  n % 4 == 0.
+ *   lstm_grad_unprepare: the inverse of lstm_prepare for gradients: dw_ih_p [4H][I], dw_hh_p [4H][H], db_p [4H] ->
+ *     dw_ih [4*nhid][ninp], dw_hh [4*nhid][nhid] and db_ih = db_hh [4*nhid] (each output may be NULL), padding dropped. */
+int b200asr_lstm_layer_train_fwd(const float* xproj, const void* w_hh_split, int T, int B, int H, int has_state, const float* c0,
+                                 float* h, float* c, float* gates, b200asr_stream_t stream);
+int b200asr_lstm_layer_train_bwd(const float* gates, const float* c, const float* c0, const float* dh_out, const float* dh_n,
+                                 const float* dc_n, const void* w_hh_split_t, int T, int B, int H, float* dc, float* dgates, float* dc0,
+                                 b200asr_stream_t stream);
+int b200asr_lstm_dropout(const float* x, float* y, long long n, float p, uint64_t seed, uint64_t offset, b200asr_stream_t stream);
+int b200asr_lstm_grad_unprepare(const float* dw_ih_p, const float* dw_hh_p, const float* db_p, int ninp, int nhid, float* dw_ih,
+                                float* dw_hh, float* db_ih, float* db_hh, b200asr_stream_t stream);
 int b200asr_lm_nll(const float* logits, long long ld, const int64_t* targets, float* nll, int rows, int V, b200asr_stream_t stream);
 int b200asr_lm_seq_sum(const float* nll, const int64_t* offsets, const int64_t* lengths, int nseq, float* sums,
                        b200asr_stream_t stream);
