@@ -595,6 +595,10 @@ int conv3x3_wgrad_simt(const float* x, const float* dy, float* dwr, int B, int T
 
 using namespace b200asr;
 
+// the kernels above move float4 (16 B), the pooling index bytes as uint32 (4 B) and the bf16 pairs as uint2 (8 B); every
+// entry point checks the pointers it hands to them, so a misaligned view is an error rather than a faulting launch
+static inline bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 extern "C" {
 
 size_t b200asr_conv3x3_ws_bytes(int Ci, int Co) { return sizeof(float) * 2 * 9 * (size_t)Ci * Co; }   // [hi | lo] weight halves
@@ -616,6 +620,7 @@ int b200asr_conv3x3_c1_bwd_weight(const float* x, const float* dy, float* dw, fl
                                   b200asr_stream_t stream) {
   B200_REQUIRE(x && dy && dw && dbias, B200ASR_BAD_ARG, "conv3x3_c1_bwd_weight: null pointer");
   B200_REQUIRE(Co % 4 == 0 && 256 % (Co / 4) == 0, B200ASR_BAD_SHAPE, "conv3x3_c1_bwd_weight: Co=%d unsupported", Co);
+  B200_REQUIRE(aligned16(dy), B200ASR_BAD_ALIGN, "conv3x3_c1_bwd_weight: dy alignment");
   cudaStream_t st = (cudaStream_t)stream;
   long long P = (long long)B * T * F;
   if (P <= 0) {
@@ -669,6 +674,8 @@ int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float
   B200_REQUIRE(x && w && y && ws, B200ASR_BAD_ARG, "conv3x3_fwd: null pointer");
   int rc = conv_shape_ok("conv3x3_fwd", Ci, Co);
   if (rc) return rc;
+  if (precision == B200ASR_PREC_FP32)   // the CUDA-core kernel reads x and the repacked weights in ws, writes y, as float4
+    B200_REQUIRE(aligned16(x) && aligned16(y) && aligned16(ws), B200ASR_BAD_ALIGN, "conv3x3_fwd: x, y and ws need 16-byte alignment");
   cudaStream_t st = (cudaStream_t)stream;
   int total = 9 * Ci * Co;
   note_launch(1);
@@ -711,6 +718,9 @@ int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_
   B200_REQUIRE(dy && w && dx && ws, B200ASR_BAD_ARG, "conv3x3_bwd_data: null pointer");
   int rc = conv_shape_ok("conv3x3_bwd_data", Co, Ci);   // roles swap: contraction over Co, output channels Ci
   if (rc) return rc;
+  if (precision == B200ASR_PREC_FP32)
+    B200_REQUIRE(aligned16(dy) && aligned16(relu_out) && aligned16(dx) && aligned16(ws), B200ASR_BAD_ALIGN,
+                 "conv3x3_bwd_data: dy, relu_out, dx and ws need 16-byte alignment");
   cudaStream_t st = (cudaStream_t)stream;
   int total = 9 * Ci * Co;
   note_launch(1);
@@ -733,6 +743,8 @@ int b200asr_conv3x3_bwd_weight(const float* dy, const void* dy16, const float* x
                                int F, int Ci, int Co, int precision, b200asr_stream_t stream) {
   B200_REQUIRE(dy && x && dw && ws, B200ASR_BAD_ARG, "conv3x3_bwd_weight: null pointer");
   B200_REQUIRE(Ci % 64 == 0 && Co % 64 == 0, B200ASR_BAD_SHAPE, "conv3x3_bwd_weight: Ci=%d Co=%d must be multiples of 64", Ci, Co);
+  if (precision == B200ASR_PREC_FP32)   // float4 reads of x and dy; ws is only reached by scalar atomics and loads
+    B200_REQUIRE(aligned16(x) && aligned16(dy), B200ASR_BAD_ALIGN, "conv3x3_bwd_weight: x and dy need 16-byte alignment");
   cudaStream_t st = (cudaStream_t)stream;
   cudaMemsetAsync(ws, 0, sizeof(float) * 9 * (size_t)Ci * Co, st);
   int rc;
@@ -754,6 +766,7 @@ int b200asr_conv3x3_bwd_weight(const float* dy, const void* dy16, const float* x
 
 int b200asr_maxpool2x2_fwd(const float* x, float* y, int B, int T, int F, int C, b200asr_stream_t stream) {
   B200_REQUIRE(x && y && C % 4 == 0, B200ASR_BAD_ARG, "maxpool2x2_fwd: bad arguments");
+  B200_REQUIRE(aligned16(x) && aligned16(y), B200ASR_BAD_ALIGN, "maxpool2x2_fwd: x and y need 16-byte alignment");
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
   if (n <= 0) return B200ASR_OK;
   maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, nullptr, B, T, F, C);
@@ -762,6 +775,8 @@ int b200asr_maxpool2x2_fwd(const float* x, float* y, int B, int T, int F, int C,
 
 int b200asr_maxpool2x2_fwd_idx(const float* x, float* y, unsigned char* idx, int B, int T, int F, int C, b200asr_stream_t stream) {
   B200_REQUIRE(x && y && idx && C % 4 == 0, B200ASR_BAD_ARG, "maxpool2x2_fwd_idx: bad arguments");
+  B200_REQUIRE(aligned16(x) && aligned16(y) && aligned_to(idx, 4), B200ASR_BAD_ALIGN,
+               "maxpool2x2_fwd_idx: x and y need 16-byte alignment, idx 4-byte");
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
   if (n <= 0) return B200ASR_OK;
   maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, idx, B, T, F, C);
@@ -771,6 +786,8 @@ int b200asr_maxpool2x2_fwd_idx(const float* x, float* y, unsigned char* idx, int
 int b200asr_maxpool2x2_bwd_idx(const float* dy, const unsigned char* idx, float* dx, void* dx16, int B, int T, int F, int C,
                                int relu_mask, b200asr_stream_t stream) {
   B200_REQUIRE(dy && idx && dx && C % 4 == 0, B200ASR_BAD_ARG, "maxpool2x2_bwd_idx: bad arguments");
+  B200_REQUIRE(aligned16(dy) && aligned16(dx) && aligned_to(idx, 4) && aligned_to(dx16, 8), B200ASR_BAD_ALIGN,
+               "maxpool2x2_bwd_idx: dy and dx need 16-byte alignment, idx 4-byte, dx16 8-byte");
   cudaStream_t st = (cudaStream_t)stream;
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
   if (n > 0) maxpool2x2_bwd_idx_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(dy, idx, dx, (uint16_t*)dx16, B, T, F, C, relu_mask);
@@ -785,6 +802,8 @@ int b200asr_maxpool2x2_bwd_idx(const float* dy, const unsigned char* idx, float*
 int b200asr_maxpool2x2_bwd(const float* dy, const float* x, float* dx, void* dx16, int B, int T, int F, int C, int relu_mask,
                            b200asr_stream_t stream) {
   B200_REQUIRE(dy && x && dx && C % 4 == 0, B200ASR_BAD_ARG, "maxpool2x2_bwd: bad arguments");
+  B200_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx) && aligned_to(dx16, 8), B200ASR_BAD_ALIGN,
+               "maxpool2x2_bwd: dy, x and dx need 16-byte alignment, dx16 8-byte");
   cudaStream_t st = (cudaStream_t)stream;
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
   if (n > 0) maxpool2x2_bwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(dy, x, dx, (uint16_t*)dx16, B, T, F, C, relu_mask);

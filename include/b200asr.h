@@ -189,14 +189,18 @@ int b200asr_sdpa_mat_bwd(const float* dout, const float* q, const float* k, cons
  * outer spatial axis, [B,T,F,C], so the flatten/transpose of :74-76 becomes a free view [B*T, F*C]
  * (feature index f*C+c; the host permutes input_linear's columns once per step instead).
  * Weights keep the reference layout [Co,Ci,3(freq),3(time)].
+ * Alignment: a pointer the kernels move in vectors must be aligned to the vector -- 16 bytes for the float tensors named
+ * below, 4 bytes for pooling index bytes, 8 bytes for bf16 pairs; otherwise the call returns B200ASR_BAD_ALIGN and writes
+ * nothing.  Fresh allocations always qualify; a view offset by a few floats may not.
  */
-/* x [B,F,T] (the reference's (B,1,F,T) input as is) -> y [B,T,F,Co], bias + optional ReLU fused */
+/* x [B,F,T] (the reference's (B,1,F,T) input as is) -> y [B,T,F,Co], bias + optional ReLU fused.  Co % 4 == 0, Co <= 1024,
+ * 256 % (Co/4) == 0.  y 16-byte aligned. */
 int b200asr_conv3x3_c1_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int T,
                            int Co, int relu, b200asr_stream_t stream);
-/* dw[Co,1,3,3], dbias[Co] overwritten; dy is [B,T,F,Co] (already masked by the ReLU derivative) */
+/* dw[Co,1,3,3], dbias[Co] overwritten; dy is [B,T,F,Co] (already masked by the ReLU derivative), 16-byte aligned */
 int b200asr_conv3x3_c1_bwd_weight(const float* x, const float* dy, float* dw, float* dbias, int B, int F,
                                   int T, int Co, b200asr_stream_t stream);
-/* x [B,T,F,Ci] -> y [B,T,F,Co]; ws: b200asr_conv3x3_ws_bytes(Ci,Co) */
+/* x [B,T,F,Ci] -> y [B,T,F,Co]; ws: b200asr_conv3x3_ws_bytes(Ci,Co).  Precision 0: x, y and ws 16-byte aligned. */
 int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int T,
                         int F, int Ci, int Co, int relu, int precision, b200asr_stream_t stream);
 /* The same convolution followed by MaxPool2d(2, stride 2) (models/asr/transformer.py:44-52: conv, ReLU, pool): y as above AND
@@ -211,22 +215,25 @@ int b200asr_conv3x3_fwd_pool(const float* x, const float* w, const float* bias, 
                              b200asr_stream_t stream);
 /* dx[B,T,F,Ci] = conv_transpose(dy) .* (relu_out > 0 if relu_out != NULL).
  * dx16 (optional, precisions 6 / 2 only): the same gradient additionally as bf16 hi | lo "pairs" [2][B,T,F,Ci] (hi = bf16(v),
- * lo = bf16(v - hi)) -- what b200asr_conv3x3_bwd_weight of the layer below takes as dy16. */
+ * lo = bf16(v - hi)) -- what b200asr_conv3x3_bwd_weight of the layer below takes as dy16.
+ * Precision 0: dy, relu_out, dx and ws 16-byte aligned. */
 int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_out, float* dx, void* dx16, void* ws,
                              int B, int T, int F, int Ci, int Co, int precision, b200asr_stream_t stream);
 /* dw[Co,Ci,3,3], dbias[Co] overwritten.  dy16 (optional, precisions 6 / 2): dy as bf16 pairs [2][B,T,F,Co] written by its
  * producer (b200asr_maxpool2x2_bwd / b200asr_conv3x3_bwd_data): the kernel then takes its B tiles straight from there by TMA
- * instead of converting the fp32 dy tile (the in-kernel conversion is what bounds the bf16 weight gradient). */
+ * instead of converting the fp32 dy tile (the in-kernel conversion is what bounds the bf16 weight gradient).
+ * Precision 0: dy and x 16-byte aligned. */
 int b200asr_conv3x3_bwd_weight(const float* dy, const void* dy16, const float* x, float* dw, float* dbias, void* ws,
                                int B, int T, int F, int Ci, int Co, int precision, b200asr_stream_t stream);
 size_t b200asr_conv3x3_ws_bytes(int Ci, int Co);
-/* MaxPool2d(2, stride 2), floor mode: [B,T,F,C] -> [B,T/2,F/2,C] */
+/* MaxPool2d(2, stride 2), floor mode: [B,T,F,C] -> [B,T/2,F/2,C].  C % 4 == 0; every float tensor of the four pooling
+ * entry points 16-byte aligned, idx 4-byte aligned, dx16 8-byte aligned. */
 int b200asr_maxpool2x2_fwd(const float* x, float* y, int B, int T, int F, int C, b200asr_stream_t stream);
 /* the same pooling, additionally writing the index bytes described at b200asr_conv3x3_fwd_pool */
 int b200asr_maxpool2x2_fwd_idx(const float* x, float* y, unsigned char* idx, int B, int T, int F, int C,
                                b200asr_stream_t stream);
 /* dx[B,T,F,C] = route dy to the first maximum of each window (scan order freq-major, as ATen), then
- * .* (x > 0) when relu_mask != 0 (x is the post-ReLU pool input). */
+ * .* (x > 0) when relu_mask != 0 (x is the post-ReLU pool input).  Rows / columns no window covers (odd T or F) get 0. */
 int b200asr_maxpool2x2_bwd(const float* dy, const float* x, float* dx, void* dx16 /* optional bf16 pairs [2][B,T,F,C] */, int B, int T, int F, int C,
                            int relu_mask, b200asr_stream_t stream);
 /* b200asr_maxpool2x2_bwd from the forward's index bytes instead of the activation (reads 1 byte instead of 16 per pooled
