@@ -87,6 +87,8 @@ SIGNATURES = {
     "b200asr_beam_step": (_i, [_vp, _vp] + [_i] * 7 + [C.c_double, _vp, _vp, _vp, _vp, _vp, _i] + [_vp] * 7 + [_vp]),
     "b200asr_beam_self_attn": (_i, [_vp] * 5 + [_i] * 7 + [_f, _vp]),
     "b200asr_beam_backtrack": (_i, [_vp] * 6 + [_i] * 4 + [_vp]),
+    "b200asr_decode_attn_ws_bytes": (_sz, [_i] * 4),
+    "b200asr_decode_attn": (_i, [_vp] * 5 + [_i] * 5 + [_ll] * 4 + [_f, _vp]),
     "b200asr_beam_step_log": (_i, [_vp, _vp] + [_i] * 7 + [C.c_double, _vp, _vp, _vp, _vp, _vp, _i] + [_vp] * 7 + [_vp] * 3 +
                               [_i, _vp]),
     "b200asr_beam_backtrack_packed": (_i, [_vp] * 4 + [_i, _vp, _vp, _i, _vp, _i, _i, _i, _vp]),

@@ -4,9 +4,11 @@
 
 After this, the reference's own `Transformer` (models/asr/transformer.py), `Trainer` loop
 (trainer/asr/trainer.py), `test.py` and the LSTM LM's `RNNModel.forward` (utils/lstm_utils.py) run on libb200asr kernels:
-module tree, parameter names and checkpoints are untouched; only `forward` attributes, `Decoder.beam_search` and the two
-loss functions are rebound (SURVEY.md §8b).  The replaced methods stay reachable through original(): LM rescoring with an
-LM other than an LSTM LM still runs the reference's beam_search, and a GRU / RNN LM its own RNNModel.forward.
+module tree, parameter names and checkpoints are untouched; only `forward` attributes, `Decoder.beam_search`,
+`Decoder.greedy_search`, `Transformer.evaluate` and the two loss functions are rebound (SURVEY.md §8b).  The replaced methods
+stay reachable through original(): LM rescoring with an LM other than an LSTM LM still runs the reference's beam_search, a
+GRU / RNN LM its own RNNModel.forward, greedy_search with lm_rescoring=True or in training mode and evaluate in training
+mode the reference's own methods.
 """
 from __future__ import annotations
 
@@ -35,7 +37,9 @@ def install(reference_root: str = None):
         (tr.Encoder, "forward", modules.encoder_forward),
         (tr.Decoder, "forward", modules.decoder_forward),
         (tr.Decoder, "beam_search", modules.beam_search),
+        (tr.Decoder, "greedy_search", modules.greedy_search),
         (tr.Transformer, "forward", modules.transformer_forward),
+        (tr.Transformer, "evaluate", modules.transformer_evaluate),
         (um, "calculate_loss", metrics.calculate_loss),
         (um, "calculate_metrics", metrics.calculate_metrics),
         (tr, "calculate_metrics", metrics.calculate_metrics),

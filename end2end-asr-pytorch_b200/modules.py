@@ -8,7 +8,8 @@ the reference's classes (class-level patch, SURVEY.md §8b).
 
 Decoder.beam_search is mirrored (beam_decode: batched, KV-cached, selection on the device), including lm_rescoring=True
 with an LSTM language model (RNNModel / LM below, or the reference's utils/lstm_utils.LM); with any other LM object it runs
-the reference's own method.  Not mirrored (out of scope, SURVEY.md §2): the Linear-variant FFN (dead code).
+the reference's own method.  Decoder.greedy_search (greedy_decode_cached) and Transformer.evaluate are mirrored too.
+Not mirrored (out of scope, SURVEY.md §2): the Linear-variant FFN (dead code).
 """
 from __future__ import annotations
 
@@ -201,8 +202,9 @@ def greedy_decode_ids(self, encoder_padded_outputs, steps=300):
 def greedy_decode_cached(self, encoder_padded_outputs, steps=300, stop_at_eos=False, check_every=8):
     """Incremental greedy decode with self- and cross-attention K/V caches (SURVEY.md §8f row 3): the same token ids as
     greedy_decode_ids / the reference's greedy_search, at O(T) instead of O(T^2) work -- per step only the new position is
-    projected, its K/V rows are appended to per-layer caches, and single-query attention runs over the cache (self) and
-    over the once-projected encoder K/V (cross, no mask as in transformer.py:347).
+    projected, its K/V rows are written by the GEMM into step t of per-layer slab-major caches [steps, B, H*d], and
+    single-query attention (ops.decode_attn, split over keys) runs over the cache (self) and over the encoder K/V projected
+    once per call (cross, no mask as in transformer.py:347), both read in place through strides.
 
     stop_at_eos: the EOS cut of transformer.py:385-393 stays on the device -- ids from an utterance's first EOS on are -1
     (the reference drops them when it builds the strings), a device counter tracks finished utterances and the loop ends
@@ -219,32 +221,36 @@ def greedy_decode_cached(self, encoder_padded_outputs, steps=300, stop_at_eos=Fa
             cross, kc, vc = [], [], []
             for layer in self.layers:
                 ca = layer.encoder_attn
-                k = ops.LinearFn.apply(encoder_padded_outputs, ca.key_linear.weight, ca.key_linear.bias).view(B, Te, H, dk).permute(0, 2, 1, 3)
-                v = ops.LinearFn.apply(encoder_padded_outputs, ca.value_linear.weight, ca.value_linear.bias).view(B, Te, H, dv).permute(0, 2, 1, 3)
+                k = ops.LinearFn.apply(encoder_padded_outputs, ca.key_linear.weight, ca.key_linear.bias)        # [B, Te, H*dk]
+                v = ops.LinearFn.apply(encoder_padded_outputs, ca.value_linear.weight, ca.value_linear.bias)
                 cross.append((k, v))
-                kc.append(torch.empty((B, steps, H * dk), device=dev, dtype=torch.float32))
-                vc.append(torch.empty((B, steps, H * dv), device=dev, dtype=torch.float32))
+                kc.append(torch.empty((steps, B, H * dk), device=dev, dtype=torch.float32))
+                vc.append(torch.empty((steps, B, H * dv), device=dev, dtype=torch.float32))
             ys = torch.full((B, steps), -1, dtype=torch.long, device=dev) if stop_at_eos else torch.empty((B, steps), dtype=torch.long, device=dev)
             tok = torch.full((B, 1), SOS_TOKEN, dtype=torch.long, device=dev)
             finished = torch.zeros(B + 1, dtype=torch.int32, device=dev) if stop_at_eos else None      # [B] flags + [1] counter
+            self_k, self_v = (H * dk, B * H * dk), (H * dv, B * H * dv)               # (row, key) strides of the caches
+            cross_k, cross_v = (Te * H * dk, H * dk), (Te * H * dv, H * dv)           # ... and of the encoder projections
 
-            def attend(mod, x, k4, v4):
-                q = ops.LinearFn.apply(x, mod.query_linear.weight, mod.query_linear.bias).view(B, 1, H, dk).permute(0, 2, 1, 3)
-                o = ops.SdpaFn.apply(q, k4, v4, None, None, False, 1.0 / float(mod.attention.temperature), 0.0)
-                o = ops.LinearFn.apply(o.permute(0, 2, 1, 3).reshape(B, 1, H * dv), mod.output_linear.weight, mod.output_linear.bias)
+            def post(mod, o, x):
+                o = ops.LinearFn.apply(o, mod.output_linear.weight, mod.output_linear.bias).view(B, 1, -1)
                 return ops.AddLNFn.apply(o, x, mod.layer_norm.weight, mod.layer_norm.bias, None, None, mod.layer_norm.eps, 0.0)
 
             for t in range(steps):
                 pe = self.positional_encoding.pe[0, t:t + 1]
                 x = ops.EmbedFn.apply(tok, self.trg_embedding.weight, pe, float(self.x_logit_scale), 0.0, PAD_TOKEN)
                 for li, layer in enumerate(self.layers):
-                    sa = layer.self_attn
-                    kc[li][:, t:t + 1] = ops.LinearFn.apply(x, sa.key_linear.weight, sa.key_linear.bias)
-                    vc[li][:, t:t + 1] = ops.LinearFn.apply(x, sa.value_linear.weight, sa.value_linear.bias)
-                    k4 = kc[li][:, :t + 1].view(B, t + 1, H, dk).permute(0, 2, 1, 3)
-                    v4 = vc[li][:, :t + 1].view(B, t + 1, H, dv).permute(0, 2, 1, 3)
-                    x = attend(sa, x, k4, v4)
-                    x = attend(layer.encoder_attn, x, cross[li][0], cross[li][1])
+                    sa, ca = layer.self_attn, layer.encoder_attn
+                    x2 = x.view(B, -1)
+                    ops.linear_into(x2, sa.key_linear.weight, sa.key_linear.bias, kc[li][t])
+                    ops.linear_into(x2, sa.value_linear.weight, sa.value_linear.bias, vc[li][t])
+                    q = ops.LinearFn.apply(x2, sa.query_linear.weight, sa.query_linear.bias)
+                    o = ops.decode_attn(q, kc[li], vc[li], H, t + 1, self_k, self_v, dv, 1.0 / float(sa.attention.temperature))
+                    x = post(sa, o, x)
+                    q = ops.LinearFn.apply(x.view(B, -1), ca.query_linear.weight, ca.query_linear.bias)
+                    o = ops.decode_attn(q, cross[li][0], cross[li][1], H, Te, cross_k, cross_v, dv,
+                                        1.0 / float(ca.attention.temperature))
+                    x = post(ca, o, x)
                     x = _ffn_core(layer.pos_ffn, x)
                 logits = ops.LinearFn.apply(x.view(B, -1), self.output_linear.weight, None)
                 if stop_at_eos:
@@ -405,6 +411,57 @@ def beam_search(self, encoder_padded_outputs, beam_width=2, nbest=5, lm_rescorin
             ys.append(y)
             strs.append("".join(self.id2label[t] for t in y[1:]))
     return ys, strs
+
+
+GREEDY_STEPS = 300          # Decoder.greedy_search's fixed step count (transformer.py:332)
+
+
+def greedy_strings(ids, id2label):
+    """The strings of Decoder.greedy_search (models/asr/transformer.py:376 and :385-393) from per-utterance token ids: each id
+    maps to id2label[id], except EOS, which maps to EOS_CHAR; the string ends before the first entry EQUAL to EOS_CHAR (a cut
+    on the string, so a non-EOS label equal to EOS_CHAR also ends it).  The reference joins the entries of a numpy array
+    (np.transpose of the per-step label lists), so every label goes through numpy's str conversion, as here.  An id < 0 ends
+    the row as well: greedy_decode_cached(stop_at_eos=True) writes -1 after an utterance's first EOS, where the string has
+    already ended."""
+    out = []
+    for row in ids:
+        labels = []
+        for i in row:
+            if i < 0:
+                break
+            labels.append(EOS_CHAR if i == EOS_TOKEN else id2label[i])
+        st = ""
+        for e in np.array(labels, dtype=str):
+            if e == EOS_CHAR:
+                break
+            st += e
+        out.append(st)
+    return out
+
+
+def _reference_method(self, name, why):
+    from .install import original
+    ref = original(type(self), name)
+    if ref is None:
+        raise NotImplementedError(f"{type(self).__name__}.{name} {why} runs the reference's own method; call b200asr.install() on "
+                                  f"the reference's {type(self).__name__}")
+    return ref
+
+
+def greedy_search(self, encoder_padded_outputs, beam_width=2, lm_rescoring=False, lm=None, lm_weight=0.1, c_weight=1):
+    """Decoder.greedy_search (models/asr/transformer.py:316-394): the B strings of 300 greedy steps, cut at EOS_CHAR.  Decoded
+    by greedy_decode_cached(steps=300, stop_at_eos=True) -- KV-cached, the EOS stop on the device -- with the ids back in one
+    device-to-host copy; the strings follow greedy_strings.  lm_rescoring=True (which fails in the reference itself) and a
+    decoder in training mode (the reference then applies dropout at every step) run the reference's own method."""
+    if lm_rescoring or self.training:
+        ref = _reference_method(self, "greedy_search", "with lm_rescoring=True or in training mode")
+        return ref(self, encoder_padded_outputs, beam_width=beam_width, lm_rescoring=lm_rescoring, lm=lm, lm_weight=lm_weight,
+                   c_weight=c_weight)
+    if int(self.trg_max_length) < GREEDY_STEPS:
+        raise ValueError(f"greedy search decodes {GREEDY_STEPS} positions but the decoder's positional table covers "
+                         f"trg_max_length={self.trg_max_length}: build the model with tgt_max_len >= {GREEDY_STEPS}")
+    ids = greedy_decode_cached(self, encoder_padded_outputs, steps=GREEDY_STEPS, stop_at_eos=True).cpu()
+    return greedy_strings(ids.tolist(), self.id2label)
 
 
 # ------------------------------------------------------------------------------------------------ LM rescoring
@@ -579,6 +636,44 @@ def transformer_forward(self, padded_input, input_lengths, padded_target, verbos
     return pred, gold, hyp_seq, gold
 
 
+def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_search=False, beam_width=0, beam_nbest=0, lm=None,
+                         lm_rescoring=False, lm_weight=0.1, c_weight=1, verbose=False):
+    """Transformer.evaluate (models/asr/transformer.py:87-124) -> ([[None] * L, [None] * L], strs_hyps, strs_gold).
+
+    The front end (_front_end: emb_cnn normalises with BatchNorm's running statistics in eval mode) and the encoder run on the
+    device, then Decoder.beam_search (nbest=1; greedy_search when fewer than B strings come back, :112-118) or
+    Decoder.greedy_search.  The reference's teacher-forced decoder pass and its topk (:107-108) only serve to produce `gold`
+    and are skipped: gold comes from ops.preprocess_targets (raising like the reference for a target longer than
+    tgt_max_len) in one device-to-host copy, and strs_gold joins id2label over all tgt_max_len entries, PAD included (:110).
+    A model in training mode runs the reference's own method."""
+    if self.training:
+        ref = _reference_method(self, "evaluate", "in training mode")
+        return ref(self, padded_input, input_lengths, padded_target, beam_search=beam_search, beam_width=beam_width,
+                   beam_nbest=beam_nbest, lm=lm, lm_rescoring=lm_rescoring, lm_weight=lm_weight, c_weight=c_weight,
+                   verbose=verbose)
+    ops._need_cuda(padded_input, padded_target)
+    dec = self.decoder
+    with torch.no_grad():
+        feats, cf = _front_end(self, padded_input)
+        enc = _encoder_body(self.encoder, feats, input_lengths, cf)
+        _, gold, _, _ = ops.preprocess_targets(padded_target, int(dec.trg_max_length))
+        strs_gold = ["".join([self.id2label[x] for x in g]) for g in gold.cpu().tolist()]
+        B = enc.shape[0]
+        if beam_search:
+            _, strs_hyps = dec.beam_search(enc, beam_width=beam_width, nbest=1, lm=lm, lm_rescoring=lm_rescoring,
+                                           lm_weight=lm_weight, c_weight=c_weight)
+            if len(strs_hyps) != B:
+                print(">>>>>>> switch to greedy")
+                strs_hyps = dec.greedy_search(enc)
+        else:
+            strs_hyps = dec.greedy_search(enc)
+    if verbose:
+        print("GOLD", strs_gold)
+        print("HYP", strs_hyps)
+    n = len(dec.layers)
+    return [[None] * n, [None] * n], strs_hyps, strs_gold
+
+
 # ------------------------------------------------------------------------------------------------ mirror classes
 class PositionalEncoding(nn.Module):
     """models/common_layers.py:76-98."""
@@ -699,11 +794,11 @@ class Decoder(nn.Module):
     greedy_decode_cached = greedy_decode_cached
     beam_decode = beam_decode
     beam_search = beam_search
+    greedy_search = greedy_search
 
 
 class Transformer(nn.Module):
-    """models/asr/transformer.py:16-85 (forward only; evaluate is not mirrored -- on the installed reference it runs its own
-    body, whose beam_search is Decoder.beam_search above)."""
+    """models/asr/transformer.py:16-124: forward and evaluate."""
 
     def __init__(self, encoder, decoder, feat_extractor="vgg_cnn"):
         super().__init__()
@@ -727,6 +822,7 @@ class Transformer(nn.Module):
                 nn.init.xavier_uniform_(p)
 
     forward = transformer_forward
+    evaluate = transformer_evaluate
 
 
 def rnn_model_forward(self, input, hidden):

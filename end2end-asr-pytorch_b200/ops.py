@@ -1175,6 +1175,30 @@ def beam_self_attn(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor
     return out
 
 
+def decode_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, H: int, Tk: int, k_strides, v_strides, dv: int,
+                scale: float) -> torch.Tensor:
+    """Single-query attention of a decode step (include/b200asr.h b200asr_decode_attn): q [R, H*dk] -> out [R, H*dv].  Key j of
+    row r starts at element r * k_strides[0] + j * k_strides[1] of `k` (from its first element), V likewise; (H*d, B*H*d) reads
+    a slab-major cache [steps, B, H*d], (T*H*d, H*d) a token-major projection [B, T, H*d]."""
+    _need_cuda(q, k, v)
+    q = _f32c(q)
+    R = q.shape[0]
+    dk = q.shape[1] // H
+    for t, (rs, ks), d in ((k, k_strides, dk), (v, v_strides, dv)):
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"decode_attn: expected float32 K/V, got {t.dtype}")
+        last = t.storage_offset() + (R - 1) * rs + (Tk - 1) * ks + H * d
+        if last > t.untyped_storage().nbytes() // 4:
+            raise RuntimeError(f"decode_attn: R={R}, Tk={Tk} with strides ({rs}, {ks}) reach past the end of the K/V storage")
+    out = torch.empty((R, H * dv), device=q.device, dtype=torch.float32)
+    nws = _lib().b200asr_decode_attn_ws_bytes(R, H, int(Tk), dv) // 4
+    ws = torch.empty(nws, device=q.device, dtype=torch.float32) if nws else None
+    L.check(_lib().b200asr_decode_attn(L.ptr(q), L.ptr(k), L.ptr(v), L.ptr(out), L.ptr(ws), R, H, dk, dv, int(Tk),
+                                       int(k_strides[0]), int(k_strides[1]), int(v_strides[0]), int(v_strides[1]), float(scale),
+                                       _stream()), "decode_attn")
+    return out
+
+
 def beam_backtrack(buf: BeamBuffers):
     """(ids [B, nbest, steps + 2] int64, lengths [B, nbest] int64) of the pooled hypotheses; see b200asr_beam_backtrack."""
     ids = torch.empty((buf.B, buf.nbest, buf.steps + 2), device=buf.score.device, dtype=torch.long)

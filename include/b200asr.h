@@ -366,6 +366,19 @@ int b200asr_beam_step(const float* logits, const int32_t* word_tab, int B, int W
  * dk, dv in {16, 32, 64, 128}; t < 8192. */
 int b200asr_beam_self_attn(const float* q, const float* k_cache, const float* v_cache, const int32_t* idx, float* out, int R,
                            int H, int W, int dk, int dv, int t, int idx_stride, float scale, b200asr_stream_t stream);
+/* Single-query attention of a decode step (csrc/decode.cu): out[r][h*dv ..] = softmax(scale * q_rh . K_rh^T) . V_rh over Tk
+ * keys, no mask, exact fp32.  q [R][H*dk] and out [R][H*dv] are contiguous; key j of row r starts at
+ * k + r * k_row_stride + j * k_key_stride (elements), head h at column h * dk; V likewise with dv.  So one kernel reads a
+ * slab-major K/V cache [steps][B][H*d] (row stride H*d, key stride B*H*d) and a token-major projection [B*T][H*d] (row
+ * stride T*H*d, key stride H*d) in place.  The keys of each (row, head) are split into chunks of a length that depends on
+ * (R, H, Tk) only; each chunk's partial (max, sum, o) goes to `ws` and a second kernel merges them in chunk order, so
+ * repeated calls give identical bits.  ws: b200asr_decode_attn_ws_bytes(R, H, Tk, dv) bytes (0 = one chunk: ws may be
+ * NULL, one launch).  dk, dv in {16, 32, 64, 128}; 1 <= Tk <= 65536; strides >= 0 (B200ASR_BAD_SHAPE); k, v 16-byte
+ * aligned and every stride a multiple of 4 (B200ASR_BAD_ALIGN).  A rejected call launches nothing. */
+size_t b200asr_decode_attn_ws_bytes(int R, int H, int Tk, int dv);
+int b200asr_decode_attn(const float* q, const float* k, const float* v, float* out, float* ws, int R, int H, int dk, int dv,
+                        int Tk, long long k_row_stride, long long k_key_stride, long long v_row_stride,
+                        long long v_key_stride, float scale, b200asr_stream_t stream);
 /* The n-best yseqs (:500-515): ids [B][nbest][steps + 2] int64 = SOS, the tokens along hist_par from each pool entry, EOS if
  * it was forced, then -1; lengths [B][nbest] int64 (0: no hypothesis). */
 int b200asr_beam_backtrack(const int32_t* hist_tok, const int32_t* hist_par, const int32_t* pool_ref, const int32_t* pool_n,
