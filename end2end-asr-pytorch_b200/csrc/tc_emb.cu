@@ -425,7 +425,6 @@ static inline size_t weight_floats(int KH, int KW) { return ((size_t)2 * KH * KW
 static int make_shifted(const float* src, float* dst, int B, int H, int W, int P, cudaStream_t st) {
   const long long R = (long long)B * EC * H, n = R * (shift_pitch(W) / 4);
   emb_shift4_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(src, dst, R, W, P, shift_pitch(W));
-  note_launch(1);
   return check_launch("conv2d_tc_shift4");
 }
 
@@ -453,7 +452,6 @@ static int emb1_geom(Emb1G& g, const char* who, int B, int H, int W, int Co, int
 static int emb1_prepare(CUtensorMap* m, const float* x, float* copies, const Emb1G& g, cudaStream_t st) {
   const long long R = (long long)g.B * g.H, n = R * (g.pd / 4);
   emb1_prep_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(x, copies, R, g.W, g.pd);
-  note_launch(1);
   if (int rc = check_launch("conv2d_c1_prep")) return rc;
   uint64_t dims[4] = {(uint64_t)g.pd, (uint64_t)g.KH, (uint64_t)g.OH, (uint64_t)8 * g.B};
   uint64_t strides[3] = {(uint64_t)g.pd, (uint64_t)2 * g.pd, (uint64_t)g.H * g.pd};
@@ -587,7 +585,8 @@ int b200asr_conv2d_c1_tc_fwd(const float* x, const float* w, const float* bias, 
   B200_REQUIRE(precision == 3 || precision == 6 || precision == 2, B200ASR_BAD_ARG, "conv2d_c1_tc_fwd: precision must be 3, 6 or 2");
   Emb1G g;
   if (int rc = emb1_geom(g, "conv2d_c1_tc_fwd", B, H, W, Co, KH, KW, PW)) return rc;
-  B200_REQUIRE(y_pitch >= g.OW && aligned16(ws), B200ASR_BAD_ALIGN, "conv2d_c1_tc_fwd: pitch / alignment");
+  B200_REQUIRE(y_pitch >= g.OW, B200ASR_BAD_SHAPE, "conv2d_c1_tc_fwd: y pitch %d does not cover OW=%d", y_pitch, g.OW);
+  B200_REQUIRE(aligned16(ws), B200ASR_BAD_ALIGN, "conv2d_c1_tc_fwd: ws needs a 16-byte aligned base");
   cudaStream_t st = (cudaStream_t)stream;
   const int nkblk = ceil_div(KH, 32), rows = KW * nkblk * EC;
   emb1_repack_kernel<<<ceil_div(rows * 32, 256), 256, 0, st>>>(w, ws, KH, KW, nkblk, precision);
@@ -613,8 +612,9 @@ int b200asr_conv2d_c1_tc_bwd_weight(const float* dy, const float* x, float* dw, 
   B200_REQUIRE(dy && x && dw && ws, B200ASR_BAD_ARG, "conv2d_c1_tc_bwd_weight: null pointer");
   Emb1G g;
   if (int rc = emb1_geom(g, "conv2d_c1_tc_bwd_weight", B, H, W, Co, KH, KW, PW)) return rc;
-  B200_REQUIRE(y_pitch >= g.OW && y_pitch % 4 == 0 && aligned16(dy) && aligned16(ws), B200ASR_BAD_ALIGN,
-               "conv2d_c1_tc_bwd_weight: dy needs a 16-byte aligned base and a row pitch that is a multiple of 4 floats (TMA)");
+  B200_REQUIRE(y_pitch >= g.OW && y_pitch % 4 == 0, B200ASR_BAD_SHAPE,
+               "conv2d_c1_tc_bwd_weight: the dy row pitch must be a multiple of 4 floats (TMA) and cover the row (y pitch %d for OW=%d)", y_pitch, g.OW);
+  B200_REQUIRE(aligned16(dy) && aligned16(ws), B200ASR_BAD_ALIGN, "conv2d_c1_tc_bwd_weight: dy and ws need 16-byte aligned bases (TMA)");
   cudaStream_t st = (cudaStream_t)stream;
   CUtensorMap mx, mdy;
   if (int rc = emb1_prepare(&mx, x, (float*)ws + emb1_weight_floats(KH, KW), g, st)) return rc;

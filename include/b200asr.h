@@ -275,7 +275,13 @@ int b200asr_bn_clamp_bwd(const float* dy, const float* x, const float* y, const 
  * and data gradient; the weight gradient runs 3xTF32, one partial per row split, summed in split order.
  * ws: b200asr_conv2d_tc_ws_bytes(B, H, W, KH, KW) bytes -- the repacked weight slices, and four copies of the tensor whose
  * windows slide (x, or dy for the data gradient) shifted by 0..3 floats, because a TMA box must start on a 16-byte
- * boundary; each call rebuilds what it needs (one HBM-bound pass), so the same buffer may serve all three. */
+ * boundary; each call rebuilds what it needs (one HBM-bound pass), so the same buffer may serve all three.
+ * Returns B200ASR_BAD_SHAPE for Ci or Co != 32, H < KH, W < KW, a non-positive B / KH / KW / SH, or a row pitch that is not
+ * a multiple of 4 or smaller than its row (W, OW); B200ASR_BAD_ARG for a NULL x / dy / w / y / dx / dw / ws (bias and dbias
+ * may be NULL) or a precision other than 3, 6 or 2; B200ASR_BAD_ALIGN when a tensor read by TMA (x for the forward, dy for
+ * the data gradient, both for the weight gradient) or ws is not 16-byte aligned.  A rejected call launches nothing.
+ * Launches: forward and data gradient 3 (weight repack, shifted copies, engine); weight gradient 3 (shifted copies, engine,
+ * split reduction), 5 with dbias (+ bias partials, their reduction). */
 size_t b200asr_conv2d_tc_ws_bytes(int B, int H, int W, int KH, int KW);
 int b200asr_conv2d_tc_fwd(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int Ci, int H,
                           int W, int Co, int KH, int KW, int SH, int x_pitch, int y_pitch, int precision,
@@ -290,7 +296,12 @@ int b200asr_conv2d_tc_bwd_weight(const float* dy, const float* x, float* dw, flo
  * same engine: the KH taps along H play the role of input channels (an overlapping tensor-map view of the activation), the
  * stride along W is removed by de-interleaving x into parity copies (x 4 alignments, see above).  x [B,1,H,W] dense;
  * y / dy [B,32,OH,OW] with row pitch y_pitch (any value >= OW for the forward, a multiple of 4 for the weight gradient: TMA).
- * No data gradient (the input is data).  ws: b200asr_conv2d_c1_tc_ws_bytes(B, H, W, KH, KW) bytes. */
+ * No data gradient (the input is data).  ws: b200asr_conv2d_c1_tc_ws_bytes(B, H, W, KH, KW) bytes.
+ * Returns B200ASR_BAD_SHAPE for Co != 32, KH outside 1..64, H < KH, W + 2 PW < KW, a non-positive B / KW, a negative PW, or
+ * a y_pitch smaller than OW (or, for the weight gradient, not a multiple of 4); B200ASR_BAD_ARG for a NULL x / dy / w / y /
+ * dw / ws (bias and dbias may be NULL) or a precision other than 3, 6 or 2; B200ASR_BAD_ALIGN when ws, or dy for the weight
+ * gradient, is not 16-byte aligned.  A rejected call launches nothing.  Launches: forward 3 (weight repack, de-interleaved
+ * copies, engine); weight gradient 3 (copies, engine, split reduction), 5 with dbias. */
 size_t b200asr_conv2d_c1_tc_ws_bytes(int B, int H, int W, int KH, int KW);
 int b200asr_conv2d_c1_tc_fwd(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int H, int W,
                              int Co, int KH, int KW, int PW, int y_pitch, int precision, b200asr_stream_t stream);

@@ -343,76 +343,6 @@ def test_linear_with_presplit_weights(L, M, N, K):
     assert rel_err(dx, dy.double() @ w.double()) < 1e-4
 
 
-# ------------------------------------------------------------------------------------------------ emb_cnn implicit GEMM
-@pytest.mark.parametrize("B,H,W,KH,KW,SH", [(2, 61, 45, 21, 11, 2), (1, 30, 205, 21, 11, 2), (3, 25, 140, 5, 3, 1), (2, 23, 131, 21, 11, 2)])
-@pytest.mark.parametrize("prec,tol", [(3, 1e-4), (6, 3e-5), (2, 1e-2)])
-def test_conv2d_implicit_gemm_32ch(L, B, H, W, KH, KW, SH, prec, tol):
-    """tc_emb.cu through the raw C ABI: forward, data gradient and weight gradient of Conv2d(32, 32, (KH, KW), stride (SH, 1))
-    on row-pitched NCHW tensors against float64 (W and OW deliberately not multiples of 4 / 32 / 128)."""
-    import torch.nn.functional as F
-    lib = L.load()
-    st = torch.cuda.current_stream().cuda_stream
-    g = torch.Generator().manual_seed(B * 1000 + W)
-    OH, OW = (H - KH) // SH + 1, W - KW + 1
-    xp, yp = (W + 3) // 4 * 4, (OW + 3) // 4 * 4
-    x = torch.randn(B, 32, H, W, generator=g).cuda()
-    w = (torch.randn(32, 32, KH, KW, generator=g) * (32 * KH * KW) ** -0.5).cuda()
-    b = torch.randn(32, generator=g).cuda()
-    dy = torch.randn(B, 32, OH, OW, generator=g).cuda()
-    x64 = x.double().requires_grad_(True)
-    w64 = w.double().requires_grad_(True)
-    y64 = F.conv2d(x64, w64, b.double(), stride=(SH, 1))
-    y64.backward(dy.double())
-    # pitched copies, pad columns poisoned with NaN: nothing may read them
-    xpad = torch.full((B, 32, H, xp), float("nan"), device="cuda"); xpad[..., :W] = x
-    dypad = torch.full((B, 32, OH, yp), float("nan"), device="cuda"); dypad[..., :OW] = dy
-    ypad = torch.full((B, 32, OH, yp), float("nan"), device="cuda")
-    dxpad = torch.full((B, 32, H, xp), float("nan"), device="cuda")
-    ws = torch.empty(lib.b200asr_conv2d_tc_ws_bytes(B, H, W, KH, KW) // 4, device="cuda")
-    L.check(lib.b200asr_conv2d_tc_fwd(L.ptr(xpad), L.ptr(w), L.ptr(b), L.ptr(ypad), L.ptr(ws), B, 32, H, W, 32, KH, KW, SH, xp, yp, prec, st), "fwd")
-    assert rel_err(ypad[..., :OW], y64) < tol
-    L.check(lib.b200asr_conv2d_tc_bwd_data(L.ptr(dypad), L.ptr(w), L.ptr(dxpad), L.ptr(ws), B, 32, H, W, 32, KH, KW, SH, xp, yp, prec, st), "dgrad")
-    assert rel_err(dxpad[..., :W], x64.grad) < tol
-    if prec == 3:
-        dw = torch.empty_like(w)
-        db = torch.empty(32, device="cuda")
-        L.check(lib.b200asr_conv2d_tc_bwd_weight(L.ptr(dypad), L.ptr(xpad), L.ptr(dw), L.ptr(db), L.ptr(ws), B, 32, H, W, 32, KH, KW, SH, xp, yp, st), "wgrad")
-        assert rel_err(dw, w64.grad) < tol
-        assert rel_err(db, dy.double().sum((0, 2, 3))) < 1e-5
-
-
-@pytest.mark.parametrize("B,H,W", [(2, 161, 400), (1, 75, 133), (3, 41, 50)])
-@pytest.mark.parametrize("prec,tol", [(3, 3e-5), (6, 3e-5), (2, 1e-2)])
-def test_conv2d_first_layer_implicit_gemm(L, B, H, W, prec, tol):
-    """tc_emb.cu, Conv2d(1, 32, (41, 11), stride (2, 2), padding (0, 10)) through the raw C ABI: forward and weight gradient
-    against float64 -- the taps along H as the contraction "channels" of an overlapping tensor-map view, the stride along W
-    through de-interleaved copies (odd and even W, tiles with out-of-range columns on both sides)."""
-    import torch.nn.functional as F
-    lib = L.load()
-    g = torch.Generator().manual_seed(7 * B + W)
-    KH, KW, PW = 41, 11, 10
-    OH, OW = (H - KH) // 2 + 1, (W + 2 * PW - KW) // 2 + 1
-    yp = (OW + 3) // 4 * 4
-    x = torch.randn(B, 1, H, W, generator=g).cuda()
-    w = (torch.randn(32, 1, KH, KW, generator=g) * (KH * KW) ** -0.5).cuda()
-    b = torch.randn(32, generator=g).cuda()
-    dy = torch.randn(B, 32, OH, OW, generator=g).cuda()
-    x64, w64 = x.double(), w.double().requires_grad_(True)
-    y64 = F.conv2d(x64, w64, b.double(), stride=(2, 2), padding=(0, PW))
-    y64.backward(dy.double())
-    st = _stream()
-    ws = torch.empty(lib.b200asr_conv2d_c1_tc_ws_bytes(B, H, W, KH, KW) // 4, device="cuda")
-    y = torch.full((B, 32, OH, yp), float("nan"), device="cuda")
-    L.check(lib.b200asr_conv2d_c1_tc_fwd(L.ptr(x), L.ptr(w), L.ptr(b), L.ptr(y), L.ptr(ws), B, H, W, 32, KH, KW, PW, yp, prec, st), "fwd")
-    assert rel_err(y[..., :OW], y64.detach()) < tol
-    if prec == 3:
-        dypad = torch.zeros(B, 32, OH, yp, device="cuda"); dypad[..., :OW] = dy
-        dw = torch.full_like(w, float("nan")); db = torch.full((32,), float("nan"), device="cuda")
-        L.check(lib.b200asr_conv2d_c1_tc_bwd_weight(L.ptr(dypad), L.ptr(x), L.ptr(dw), L.ptr(db), L.ptr(ws), B, H, W, 32, KH, KW, PW, yp, st), "wgrad")
-        assert rel_err(dw, w64.grad) < 3e-5
-        assert rel_err(db, dy.double().sum((0, 2, 3))) < 1e-5
-
-
 @pytest.mark.parametrize("prec", [6, 2, 3, 0])
 @pytest.mark.parametrize("B,T,F_,Ci,Co", [(2, 32, 16, 64, 64), (1, 37, 21, 64, 128), (2, 18, 161, 128, 128)])
 def test_conv3x3_with_fused_max_pool(L, B, T, F_, Ci, Co, prec):
