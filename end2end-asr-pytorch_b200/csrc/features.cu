@@ -176,10 +176,13 @@ int b200asr_stft_features(const float* wave, const int* lens, float* out, int* f
   B200_REQUIRE(n_fft % 32 == 0 && hop % 4 == 0 && hop > 0 && hop <= n_fft, B200ASR_BAD_SHAPE,
                "stft_features: n_fft=%d must be a multiple of 32 and hop=%d a multiple of 4 (<= n_fft)", n_fft, hop);
   B200_REQUIRE(aligned16(ws) && aligned16(out), B200ASR_BAD_ALIGN, "stft_features: alignment");
+  B200_REQUIRE(precision == B200ASR_PREC_FP32 || precision == B200ASR_PREC_TF32 || precision == B200ASR_PREC_TF32X3,
+               B200ASR_BAD_ARG, "stft_features: precision %d (0, 1 or 3: the DFT basis is an fp32 operand)", precision);
+  // the longest utterance that fits in Lmax samples has 1 + Lmax/hop frames
+  B200_REQUIRE(Tmax <= 1 + Lmax / hop, B200ASR_BAD_SHAPE, "stft_features: Tmax=%d exceeds 1 + Lmax/hop = %d", Tmax, 1 + Lmax / hop);
   cudaStream_t st = (cudaStream_t)stream;
   const FeatWs w = feat_ws(B, Lmax, n_fft, hop);
   const int nb = n_fft / 2 + 1;
-  B200_REQUIRE(Tmax <= w.rows_per_utt, B200ASR_BAD_SHAPE, "stft_features: Tmax=%d exceeds 1 + Lmax/hop", Tmax);
   float* base = (float*)ws;
   float* padded = base + w.padded;
   float* basis = base + w.basis;
@@ -196,9 +199,8 @@ int b200asr_stft_features(const float* wave, const int* lens, float* out, int* f
   const int M = B * w.rows_per_utt;
   if (precision == B200ASR_PREC_FP32)
     rc = gemm_simt(padded, true, hop, basis, true, n_fft, spec, w.npad, M, w.npad, n_fft, nullptr, 0, nullptr, 0, false, st);
-  else if (precision == B200ASR_PREC_TF32 || precision == B200ASR_PREC_TF32X3)
+  else
     rc = gemm_tc(padded, true, hop, basis, true, n_fft, spec, w.npad, M, w.npad, n_fft, nullptr, 0, nullptr, 0, precision, st);
-  else { set_error("stft_features: unknown precision %d", precision); return B200ASR_BAD_ARG; }
   if (rc) return rc;
   dim3 grid(ceil_div(Tmax, 32), ceil_div(nb, 32), B);
   feat_mag_kernel<<<grid, 256, 0, st>>>(spec, lens, out, parts, frames_out, w.rows_per_utt, w.npad, nb, Tmax, hop);

@@ -54,11 +54,27 @@ int b200asr_linear_bwd_data(const float* dy, const float* w, const float* relu_o
 int b200asr_linear_bwd_weight(const float* dy, const float* x, float* dw, float* dbias, int M, int N, int K,
                               int accumulate, int precision, b200asr_stream_t stream) {
   B200_REQUIRE(dy && x && dw && M >= 0 && N > 0 && K > 0, B200ASR_BAD_ARG, "linear_bwd_weight: bad arguments");
+  B200_REQUIRE(precision == B200ASR_PREC_FP32 || precision == B200ASR_PREC_TF32 || precision == B200ASR_PREC_TF32X3 ||
+               is_bf16_prec(precision), B200ASR_BAD_ARG, "linear_bwd_weight: unknown precision %d", precision);
   cudaStream_t st = (cudaStream_t)stream;
+  if (M == 0) {
+    // empty batch: the sums over no rows are 0 at every precision (the tensor-core GEMM cannot describe a contraction of
+    // length 0 to TMA, so nothing is dispatched)
+    if (!accumulate) {
+      cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)N * K, st);
+      if (dbias) cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st);
+    }
+    return B200ASR_OK;
+  }
   // dw[n,k] = sum_m dy[m,n] x[m,k]: contraction over m; A(n,m) = dy[m*N + n], B(m,k) = x[m*K + k]
   // db[n] = sum_m dy[m,n] = row sums of A: the 3xTF32 kernel produces them from the tiles it stages (one launch and one
   // HBM pass over dy less); other precisions run the column-sum kernel
-  const bool fuse = dbias && precision != B200ASR_PREC_FP32 && gemm_tc_fuses_rowsum(false, false, precision) && M > 0;
+  const bool fuse = dbias && precision != B200ASR_PREC_FP32 && gemm_tc_fuses_rowsum(false, false, precision);
+  // the fused row sums accumulate into dbias, which is cleared first: reject what gemm_tc rejects before clearing it
+  if (fuse)
+    B200_REQUIRE(aligned16(dy) && aligned16(x) && N % 4 == 0 && K % 4 == 0, B200ASR_BAD_SHAPE,
+                 "linear_bwd_weight: TMA needs 16-byte aligned dy and x, and N=%d and K=%d multiples of 4; use precision 0 for this shape",
+                 N, K);
   if (fuse && !accumulate) cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st);
   int rc = gemm_dispatch(dy, false, N, x, false, K, dw, K, N, K, M, nullptr, 0, nullptr, accumulate, true, precision, st,
                          nullptr, 0, fuse ? dbias : nullptr);

@@ -63,6 +63,26 @@ unsigned long long b200asr_launch_count(void);
  *   position-wise FFN conv_1/conv_2 models/common_layers.py:138   (weights (out,in,1) == (out,in))
  *   decoder output_linear (logits)  models/asr/transformer.py:302
  * y[M,N] = act(x[M,K] * w[N,K]^T + bias[N]);  bias may be NULL; relu != 0 applies max(0, .)
+ *
+ * All three entry points take M >= 0, N > 0, K > 0 and non-NULL x / dy / w / y / dx / dw (bias, relu_out and dbias may be
+ * NULL); otherwise, or for a precision other than 0, 1, 3, 2, 6, they return B200ASR_BAD_ARG.
+ *   precision 0 (fp32 CUDA cores): any N and K, any 4-byte aligned pointers (16-byte alignment and dimensions that are
+ *     multiples of 4 only select vector loads).  Its split-K weight gradient (contraction M >= 1024 and fewer output tiles
+ *     than SMs) adds the splits with atomics, so the bits of dw may differ from call to call there.
+ *   precisions 1, 3 (TF32 / 3xTF32 tensor cores): the operands the GEMM reads by TMA must be 16-byte aligned with row
+ *     pitches that are multiples of 4 floats -- x, w and K for the forward; dy, w, N and K for the data gradient; dy, x, N
+ *     and K for the weight gradient -- otherwise B200ASR_BAD_SHAPE.  The forward's N, bias, relu_out and the outputs
+ *     have no such rule (they take a scalar epilogue).
+ *   precisions 2, 6 (bf16 / bf16x3): w_split is required (see below), otherwise B200ASR_BAD_SHAPE; the weight gradient
+ *     has the rules of precision 3.
+ * A rejected call launches nothing and writes nothing.
+ * M = 0 (an empty batch, pointers still valid): the forward and the data gradient write nothing; the weight gradient sets
+ * dw and dbias to 0, or leaves them unchanged when accumulating.  Same at every precision; nothing is launched.
+ * Kernel launches per call (b200asr_launch_count): forward and data gradient 1; at precisions 1 and 3, 2 when the
+ * contraction is split (no ReLU and no mask, K >= 1024, at most half as many 128 x 128 output tiles as SMs): the GEMM and
+ * the reduction of its partial tiles, which adds the bias.  Weight gradient: precision 0: 1, + 2 with dbias (column sums
+ * and their reduction); precision 1: 1 or 2 split, + 2 with dbias; precisions 3, 2, 6: 1 unsplit, 2 split, + 1 with dbias
+ * when split (the bias gradient is fused into the GEMM; its split partials need a reduction).
  */
 int b200asr_linear_fwd(const float* x, const float* w, const float* bias, float* y, int M, int N, int K,
                        int relu, int precision, const void* w_split, b200asr_stream_t stream);
@@ -519,7 +539,9 @@ int b200asr_permute_cols_cf(const float* src, float* dst, int rows, int C, int F
  * reflected when pad_reflect != 0, zeros otherwise), magnitude, log1p, optional per-utterance mean / unbiased-std
  * normalisation -> out [B,1,n_fft/2+1,Tmax] zero padded; frames_out[b] = 1 + lens[b]/hop (may be NULL).
  * The STFT of the whole batch is ONE GEMM over overlapping frame rows (precision as for b200asr_linear_fwd).
- * ws: b200asr_stft_ws_bytes(B, Lmax, n_fft, hop) bytes.  n_fft % 32 == 0, hop % 4 == 0. */
+ * ws: b200asr_stft_ws_bytes(B, Lmax, n_fft, hop) bytes.  n_fft % 32 == 0, hop % 4 == 0, hop <= n_fft, 1 <= Tmax <=
+ * 1 + Lmax/hop (B200ASR_BAD_SHAPE); ws and out 16-byte aligned (B200ASR_BAD_ALIGN); precision 0, 1 or 3, else
+ * B200ASR_BAD_ARG.  A rejected call launches nothing. */
 size_t b200asr_stft_ws_bytes(int B, int Lmax, int n_fft, int hop);
 int b200asr_stft_features(const float* wave, const int* lens, float* out, int* frames_out, void* ws, int B,
                           int Lmax, int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window_periodic,

@@ -1,6 +1,7 @@
 """-m gpu tests of the edges the tile engine's schedule has (tc_engine.cuh: the k-loop builds k-block kb + 1's A fragments while
 kb's MMAs run, in two fragment buffers, and releases each stage one k-block late; the producer and consumer warpgroups split
-the registers with setmaxnreg), for the default bf16x3 instantiations and the halo convolution that shares the k-loop:
+the registers with setmaxnreg), for the default bf16x3 instantiations, the linear layer's TF32 (NSPLIT 1) and 3xTF32
+(NSPLIT 3) instantiations, whose fragments are built differently, and the halo convolution that shares the k-loop:
 
   * one and two k-blocks (the pipeline's prologue and drain), an odd number of k-blocks (the loop runs two per trip), and
     contractions that end in a partial k-block, in every direction of the linear layer (forward: K, data gradient: N, weight
@@ -16,8 +17,9 @@ the registers with setmaxnreg), for the default bf16x3 instantiations and the ha
   * the LSTM cell policy (one engine launch per time step);
   * schedule independence: the same rows computed in one launch and in two launches (other CTAs) are bit-identical.
 
-Every output is NaN-poisoned first.  Bars are those of tests/test_gpu_default_precision.py (about 3x the error measured on
-one H100 80GB HBM3 at a 700 W limit); the schedule changes no arithmetic, so the errors are the same."""
+Every output is NaN-poisoned first.  The bf16x3 bars are those of tests/test_gpu_default_precision.py (about 3x the error
+measured on one H100 80GB HBM3 at a 700 W limit); the schedule changes no arithmetic, so the errors are the same.  The TF32
+and 3xTF32 bars are about 3x the error measured here on the same card and limit (stated at BARS)."""
 import math
 
 import numpy as np
@@ -29,7 +31,10 @@ from tests.helpers import rel_err
 pytestmark = pytest.mark.gpu
 
 BF16X3 = 6
-BARS = dict(fwd=3e-5, dgrad=6e-5, wgrad=4e-5)
+# TF32 / 3xTF32 measured over EDGE_SHAPES + TILE_SHAPES: forward 3.7e-4 / 1.0e-6 (K <= 96), data gradient 4.3e-4 / 3.5e-5
+# (over N = 4364), weight gradient 3.7e-4 / 1.5e-5
+BARS = {BF16X3: dict(fwd=3e-5, dgrad=6e-5, wgrad=4e-5), 1: dict(fwd=1.2e-3, dgrad=1.3e-3, wgrad=1.2e-3),
+        3: dict(fwd=3e-6, dgrad=1e-4, wgrad=5e-5)}
 
 
 @pytest.fixture(scope="module")
@@ -43,7 +48,10 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _split(L, w):
+def _split(L, w, prec=BF16X3):
+    """The weight operands of the bf16x3 forward and data gradient; TF32 and 3xTF32 split inside the kernel."""
+    if prec != BF16X3:
+        return None, None
     N, K = w.shape
     fwd = torch.empty(2, N, K, device="cuda", dtype=torch.bfloat16)
     bwd = torch.empty(2, K, (N + 7) // 8 * 8, device="cuda", dtype=torch.bfloat16)
@@ -61,9 +69,16 @@ EDGE_SHAPES = [(32, 32, 32), (64, 64, 64), (96, 96, 96), (100, 40, 72), (200, 13
 TILE_SHAPES = [(128 * t, 128, 96) for t in (1, 2, 131, 132, 133, 265)]
 
 
-@pytest.mark.parametrize("M,N,K", EDGE_SHAPES + TILE_SHAPES)
-def test_linear_bf16x3_schedule_edges(L, M, N, K):
-    """b200asr_linear_fwd (bias), _bwd_data (ReLU mask) and _bwd_weight (bias gradient) at bf16x3 against float64."""
+def _with_precisions(rows):
+    """Each row at bf16x3 (its id unchanged), then at TF32 and 3xTF32 (ids suffixed "tf32" / "tf32x3")."""
+    return [pytest.param(*row, prec, id="-".join(map(str, row)) + suffix)
+            for prec, suffix in ((BF16X3, ""), (1, "-tf32"), (3, "-tf32x3")) for row in rows]
+
+
+@pytest.mark.parametrize("M,N,K,prec", _with_precisions(EDGE_SHAPES + TILE_SHAPES))
+def test_linear_bf16x3_schedule_edges(L, M, N, K, prec):
+    """b200asr_linear_fwd (bias), _bwd_data (ReLU mask) and _bwd_weight (bias gradient) at bf16x3, TF32 and 3xTF32 against
+    float64."""
     lib = L.load()
     st = _stream()
     g = torch.Generator().manual_seed(M + 5 * N + 11 * K)
@@ -74,16 +89,17 @@ def test_linear_bf16x3_schedule_edges(L, M, N, K):
     h = torch.randn(M, K, generator=g)
     x64, w64, dy64 = x.double(), w.double(), dy.double()
     xc, wc, bc, dyc, hc = x.cuda(), w.cuda(), b.cuda(), dy.cuda(), h.cuda()
-    fwd, bwd = _split(L, wc)
+    fwd, bwd = _split(L, wc, prec)
+    bars = BARS[prec]
     y = _nan(M, N)
-    L.check(lib.b200asr_linear_fwd(L.ptr(xc), L.ptr(wc), L.ptr(bc), L.ptr(y), M, N, K, 0, BF16X3, L.ptr(fwd), st), "fwd")
-    assert rel_err(y, x64 @ w64.t() + b.double()) < BARS["fwd"]
+    L.check(lib.b200asr_linear_fwd(L.ptr(xc), L.ptr(wc), L.ptr(bc), L.ptr(y), M, N, K, 0, prec, L.ptr(fwd), st), "fwd")
+    assert rel_err(y, x64 @ w64.t() + b.double()) < bars["fwd"]
     dx = _nan(M, K)
-    L.check(lib.b200asr_linear_bwd_data(L.ptr(dyc), L.ptr(wc), L.ptr(hc), L.ptr(dx), M, N, K, 0, BF16X3, L.ptr(bwd), st), "dgrad")
-    assert rel_err(dx, (dy64 @ w64) * (h > 0)) < BARS["dgrad"]
+    L.check(lib.b200asr_linear_bwd_data(L.ptr(dyc), L.ptr(wc), L.ptr(hc), L.ptr(dx), M, N, K, 0, prec, L.ptr(bwd), st), "dgrad")
+    assert rel_err(dx, (dy64 @ w64) * (h > 0)) < bars["dgrad"]
     dw, db = _nan(N, K), _nan(N)
-    L.check(lib.b200asr_linear_bwd_weight(L.ptr(dyc), L.ptr(xc), L.ptr(dw), L.ptr(db), M, N, K, 0, BF16X3, st), "wgrad")
-    assert rel_err(dw, dy64.t() @ x64) < BARS["wgrad"]
+    L.check(lib.b200asr_linear_bwd_weight(L.ptr(dyc), L.ptr(xc), L.ptr(dw), L.ptr(db), M, N, K, 0, prec, st), "wgrad")
+    assert rel_err(dw, dy64.t() @ x64) < bars["wgrad"]
     assert rel_err(db, dy64.sum(0)) < 1e-6
 
 
@@ -109,17 +125,17 @@ def test_linear_bf16x3_weight_gradient_tiles_and_splits(L, M, N, K):
         L.check(lib.b200asr_linear_bwd_weight(L.ptr(dyc), L.ptr(xc), L.ptr(dw), L.ptr(db), M, N, K, 0, BF16X3, st), "wgrad")
         outs.append((dw, db))
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
-    assert rel_err(outs[0][0], ref) < BARS["wgrad"]
+    assert rel_err(outs[0][0], ref) < BARS[BF16X3]["wgrad"]
     assert rel_err(outs[0][1], bref) < 1e-6
     wbase, bbase = torch.randn(N, K, generator=g), torch.randn(N, generator=g)
     dw, db = wbase.cuda(), bbase.cuda()
     L.check(lib.b200asr_linear_bwd_weight(L.ptr(dyc), L.ptr(xc), L.ptr(dw), L.ptr(db), M, N, K, 1, BF16X3, st), "wgrad acc")
-    assert rel_err(dw, wbase.double() + ref) < BARS["wgrad"]
+    assert rel_err(dw, wbase.double() + ref) < BARS[BF16X3]["wgrad"]
     assert rel_err(db, bbase.double() + bref) < 1e-6
 
 
-@pytest.mark.parametrize("M,split", [(128 * 133, 128 * 67), (128 * 265 + 40, 128 * 132)])
-def test_linear_bf16x3_rows_independent_of_launch(L, M, split):
+@pytest.mark.parametrize("M,split,prec", _with_precisions([(128 * 133, 128 * 67), (128 * 265 + 40, 128 * 132)]))
+def test_linear_bf16x3_rows_independent_of_launch(L, M, split, prec):
     """The forward and the data gradient of rows [0, M) in one launch equal, bit for bit, the same rows computed as [0, split)
     and [split, M) in two launches: each tile runs on another CTA, so nothing may depend on which CTA or warpgroup took it."""
     lib = L.load()
@@ -130,14 +146,14 @@ def test_linear_bf16x3_rows_independent_of_launch(L, M, split):
     wc = (torch.randn(N, K, generator=g) * K ** -0.5).cuda()
     bc = torch.randn(N, generator=g).cuda()
     dyc = torch.randn(M, N, generator=g).cuda()
-    fwd, bwd = _split(L, wc)
+    fwd, bwd = _split(L, wc, prec)
 
     def run(rows):
         y, dx = _nan(M, N), _nan(M, K)
         for r0, r1 in rows:
-            L.check(lib.b200asr_linear_fwd(L.ptr(xc[r0:r1]), L.ptr(wc), L.ptr(bc), L.ptr(y[r0:r1]), r1 - r0, N, K, 1, BF16X3,
+            L.check(lib.b200asr_linear_fwd(L.ptr(xc[r0:r1]), L.ptr(wc), L.ptr(bc), L.ptr(y[r0:r1]), r1 - r0, N, K, 1, prec,
                                            L.ptr(fwd), st), "fwd")
-            L.check(lib.b200asr_linear_bwd_data(L.ptr(dyc[r0:r1]), L.ptr(wc), None, L.ptr(dx[r0:r1]), r1 - r0, N, K, 0, BF16X3,
+            L.check(lib.b200asr_linear_bwd_data(L.ptr(dyc[r0:r1]), L.ptr(wc), None, L.ptr(dx[r0:r1]), r1 - r0, N, K, 0, prec,
                                                 L.ptr(bwd), st), "dgrad")
         return y, dx
 

@@ -22,59 +22,6 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-SHAPES = [(128, 128, 32), (128, 128, 128), (256, 384, 512), (300, 512, 512), (77, 52, 164), (6400 // 8, 512, 5120 // 4),
-          (130, 4364, 128), (513, 128, 2048), (1, 8, 4), (200, 64, 96)]
-
-
-@pytest.mark.parametrize("prec,tol", [(1, 2e-3), (3, 2e-5)])
-@pytest.mark.parametrize("M,N,K", SHAPES)
-def test_linear_forward_tensor_core(L, M, N, K, prec, tol):
-    lib = L.load()
-    g = torch.Generator().manual_seed(M + N + K)
-    x = torch.randn(M, K, generator=g).cuda()
-    w = torch.randn(N, K, generator=g).cuda()
-    b = torch.randn(N, generator=g).cuda()
-    ref = (x.double() @ w.double().t() + b.double()).relu()
-    y = torch.full((M, N), float("nan"), device="cuda")
-    L.check(lib.b200asr_linear_fwd(L.ptr(x), L.ptr(w), L.ptr(b), L.ptr(y), M, N, K, 1, prec, None, _stream()), "linear_fwd")
-    torch.cuda.synchronize()
-    assert rel_err(y, ref) < tol
-
-
-@pytest.mark.parametrize("prec,tol", [(1, 2e-3), (3, 1e-4)])   # 3xTF32: operands exact to ~2^-22; the residual is the
-@pytest.mark.parametrize("M,N,K", SHAPES)                      # tensor core's own fp32 accumulation over long K
-def test_linear_backward_tensor_core(L, M, N, K, prec, tol):
-    """bwd_data exercises an MN-major B operand, bwd_weight MN-major A and B.  Every contraction here is below 1024 rows, so
-    the weight gradients run unsplit; the split-K path is tested in test_gpu_default_precision.py."""
-    lib = L.load()
-    g = torch.Generator().manual_seed(M * 3 + N + K)
-    x = torch.randn(M, K, generator=g).cuda()
-    w = torch.randn(N, K, generator=g).cuda()
-    dy = torch.randn(M, N, generator=g).cuda()
-    h = torch.randn(M, K, generator=g).cuda()
-    dx = torch.full((M, K), float("nan"), device="cuda")
-    L.check(lib.b200asr_linear_bwd_data(L.ptr(dy), L.ptr(w), L.ptr(h), L.ptr(dx), M, N, K, 0, prec, None, _stream()), "bwd_data")
-    ref_dx = (dy.double() @ w.double()) * (h > 0)
-    assert rel_err(dx, ref_dx) < tol
-    dw = torch.full((N, K), float("nan"), device="cuda")
-    db = torch.full((N,), float("nan"), device="cuda")
-    L.check(lib.b200asr_linear_bwd_weight(L.ptr(dy), L.ptr(x), L.ptr(dw), L.ptr(db), M, N, K, 0, prec, _stream()), "bwd_weight")
-    assert rel_err(dw, dy.double().t() @ x.double()) < tol
-    assert rel_err(db, dy.double().sum(0)) < 1e-5
-    # accumulate path
-    base = torch.randn(N, K, generator=g).cuda()
-    dw2 = base.clone()
-    L.check(lib.b200asr_linear_bwd_weight(L.ptr(dy), L.ptr(x), L.ptr(dw2), None, M, N, K, 1, prec, _stream()), "bwd_weight acc")
-    assert rel_err(dw2, base.double() + dy.double().t() @ x.double()) < tol
-
-
-def test_unaligned_shapes_are_rejected_not_rerouted(L):
-    lib = L.load()
-    x = torch.randn(8, 161).cuda(); w = torch.randn(16, 161).cuda(); y = torch.empty(8, 16).cuda()
-    rc = lib.b200asr_linear_fwd(L.ptr(x), L.ptr(w), None, L.ptr(y), 8, 16, 161, 0, 3, None, _stream())
-    assert rc == -1 and "multiples of 4" in L.last_error()
-
-
 # ------------------------------------------------------------------------------------------------ convolution
 def _conv_case(L, B, T, F_, Ci, Co, seed=0):
     import torch.nn.functional as F
@@ -323,24 +270,6 @@ def test_conv3x3_weight_gradient_bf16_modes_and_pairs(L, B, T, F_, Ci, Co, prec,
         # from the pairs the bias gradient is the column sum of the bf16 tiles: hi + lo (16 bits) at bf16x3, hi alone at bf16
         db_tol = 1e-5 if pairs is None else (2e-5 if prec == 6 else 1e-2)
         assert rel_err(db, dy.double().sum((0, 2, 3))) < db_tol, ("db", pairs is not None)
-
-
-@pytest.mark.parametrize("M,N,K", [(300, 512, 512), (130, 4364, 128), (77, 52, 164), (800, 512, 1280)])
-def test_linear_with_presplit_weights(L, M, N, K):
-    """3xTF32 GEMM with the weight pre-split once by b200asr_split_tf32 (forward K-major B, data-gradient MN-major B)."""
-    lib = L.load()
-    g = torch.Generator().manual_seed(5 * M + N)
-    x = torch.randn(M, K, generator=g).cuda(); w = torch.randn(N, K, generator=g).cuda(); b = torch.randn(N, generator=g).cuda()
-    dy = torch.randn(M, N, generator=g).cuda()
-    ws = torch.empty(2, N, K, device="cuda")
-    L.check(lib.b200asr_split_tf32(L.ptr(w), L.ptr(ws), N * K, _stream()), "split")
-    assert torch.equal(ws[0] + ws[1], w) and float((ws[1].abs() / w.abs().clamp_min(1e-30)).max()) < 2.0 ** -11
-    y = torch.full((M, N), float("nan"), device="cuda")
-    L.check(lib.b200asr_linear_fwd(L.ptr(x), L.ptr(w), L.ptr(b), L.ptr(y), M, N, K, 0, 3, L.ptr(ws), _stream()), "fwd")
-    assert rel_err(y, x.double() @ w.double().t() + b.double()) < 2e-5
-    dx = torch.full((M, K), float("nan"), device="cuda")
-    L.check(lib.b200asr_linear_bwd_data(L.ptr(dy), L.ptr(w), None, L.ptr(dx), M, N, K, 0, 3, L.ptr(ws), _stream()), "dgrad")
-    assert rel_err(dx, dy.double() @ w.double()) < 1e-4
 
 
 @pytest.mark.parametrize("prec", [6, 2, 3, 0])
