@@ -6,7 +6,7 @@ needs the built library and an H100.
 """
 from . import _lib
 from .config import ASRConfig, BASELINE_CONFIGS
-from .features import spectrogram_batch
+from .features import NoiseBank, collate_waves, spectrogram_batch
 from .install import install, uninstall
 from .metrics import calculate_loss, calculate_metrics, loss_and_stats
 from .modules import (LM, Decoder, DecoderLayer, Encoder, EncoderLayer, MultiHeadAttention, PositionalEncoding,
@@ -18,4 +18,4 @@ from .parallel import DataParallelStep, HostBatchPrefetcher, shard_batch
 __all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "calculate_loss", "calculate_metrics",
            "loss_and_stats", "Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
            "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model", "RNNModel", "LM",
-           "precision", "manual_seed", "spectrogram_batch", "FlatParams", "FusedAdam", "NoamOpt", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]
+           "precision", "manual_seed", "spectrogram_batch", "NoiseBank", "collate_waves","FlatParams", "FusedAdam", "NoamOpt", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]

@@ -1,27 +1,157 @@
-"""GPU feature front end: waveforms -> the `(inputs, input_percentages, input_sizes)` triple of the reference's loader.
+"""GPU feature front end: waveforms -> the batches of the reference's loader.
 
-Mirrors `SpectrogramParser.parse_audio` (utils/data_loader.py:60-91) + the padded batch of `_collate_fn` (:182-214):
-STFT (n_fft = sample_rate * window_size, hop = sample_rate * window_stride, symmetric Hamming window -- the reference
-passes the callable scipy.signal.hamming, which librosa evaluates as window(n_fft), i.e. sym=True --, centred frames),
-magnitude, log1p, per-utterance mean / unbiased-std normalisation, zero padding to the longest utterance.  One C-ABI call
-(`b200asr_stft_features`): the STFT of the whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
+Mirrors `SpectrogramParser.parse_audio` (utils/data_loader.py:60-91), `SpectrogramDataset.__getitem__` (:126-133) and
+`_collate_fn` (:182-214): optional noise injection (`NoiseInjection`, :147-179), STFT (n_fft = sample_rate * window_size,
+hop = sample_rate * window_stride, the symmetric window -- the reference passes the callable scipy.signal.<window>, which
+librosa evaluates as window(n_fft), i.e. sym=True --, centred frames), magnitude, log1p, per-utterance mean /
+unbiased-std normalisation, the src_max_len cut, zero padding to the longest utterance.  One C-ABI call
+(`b200asr_stft_features_ex`): the STFT of the whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
+
+`spectrogram_batch` returns the device triple `(inputs, input_percentages, input_sizes)`; `collate_waves` returns
+`_collate_fn`'s 5-tuple, sorted, with everything but `inputs` on the host.  `NoiseBank` holds the noise clips on the
+device and makes the reference's random draws.
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import Sequence
 
+import numpy as np
 import torch
 
 from . import _lib as L
 from . import ops
 
 
+# utils/data_loader.py:20-21; any other name falls back to Hamming (:52)
+WINDOWS = {"hamming": 0, "hann": 1, "blackman": 2, "bartlett": 3}
+NO_CUT = 2 ** 31 - 1
+
+
+def _pinned_to(a: np.ndarray, device) -> torch.Tensor:
+    """Host array -> device tensor without a host synchronisation (a pinned staging copy, then an async upload)."""
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(device, non_blocking=True)
+
+
+@dataclass
+class NoiseDraws:
+    """The reference's noise draws for a batch, per utterance in batch order: `add` (binomial outcome), `clip` (index into
+    the bank's clips, -1 without noise), `level` (uniform), `rand` (the segment position draw), `start` (first sample of
+    the segment in the bank, -1 without noise)."""
+    bank: "NoiseBank"
+    add: np.ndarray
+    clip: np.ndarray
+    level: np.ndarray
+    rand: np.ndarray
+    start: np.ndarray
+
+    def take(self, order) -> "NoiseDraws":
+        order = np.asarray(order, dtype=np.int64)
+        return NoiseDraws(self.bank, self.add[order], self.clip[order], self.level[order], self.rand[order], self.start[order])
+
+
+class NoiseBank:
+    """Noise clips for `NoiseInjection` (utils/data_loader.py:147-179), back to back in one device buffer.
+
+    `clips` are 1-D fp32 waveforms at `sample_rate`, in the order `librosa.util.find_files(noise_dir)` lists them (sorted
+    paths): `draw` picks clips by index, so that order is what makes its choices the reference's.  Reading and resampling
+    the files is the caller's job."""
+
+    def __init__(self, clips, sample_rate: int, device=None):
+        arrays = [np.asarray(c.detach().cpu() if isinstance(c, torch.Tensor) else c, dtype=np.float32).reshape(-1) for c in clips]
+        if not arrays:
+            raise ValueError("NoiseBank needs at least one clip")
+        self.sample_rate = int(sample_rate)
+        self.lengths = np.array([len(a) for a in arrays], dtype=np.int64)
+        self.offsets = np.concatenate([[0], np.cumsum(self.lengths)[:-1]]).astype(np.int64)
+        device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.bank = torch.from_numpy(np.concatenate(arrays)).to(device)
+
+    def __len__(self):
+        return len(self.lengths)
+
+    def draw(self, lengths, noise_prob: float, noise_levels, rng=np.random) -> NoiseDraws:
+        """The reference's draws for utterances of `lengths` samples, each in batch order, with its numpy calls in its
+        order (data_loader.py:68-69, 164-165, 171): binomial(1, noise_prob), and only for a 1: choice over the clips,
+        uniform(*noise_levels), rand().  `rng` is np.random (the reference's global state) or a RandomState.
+
+        The segment start is noise_start = rand * (clip_len / sr - L / sr) seconds, in float64 as :169-172.  The reference
+        then cuts the segment with sox `trim` (utils/audio.py:21-32); that cut is not pinned here but restated as the
+        sample round(noise_start * sr), clamped so that the L samples fit in the clip.  A clip shorter than the utterance,
+        where the reference fails its assert (:175), raises ValueError."""
+        B = len(lengths)
+        add, clip = np.zeros(B, np.int64), np.full(B, -1, np.int64)
+        level, rand = np.full(B, np.nan), np.full(B, np.nan)
+        start = np.full(B, -1, np.int64)
+        sr = self.sample_rate
+        for b, n in enumerate(lengths):
+            n = int(n)
+            add[b] = rng.binomial(1, noise_prob)
+            if not add[b]:
+                continue
+            c = int(rng.choice(len(self)))            # np.random.choice(paths): one randint(0, len(paths)) draw
+            level[b] = rng.uniform(*noise_levels)
+            rand[b] = rng.rand()
+            clip_len = int(self.lengths[c])
+            if clip_len < n:
+                raise ValueError(f"noise clip {c} has {clip_len} samples, fewer than utterance {b}'s {n}")
+            noise_start = rand[b] * (clip_len / sr - n / sr)
+            clip[b] = c
+            start[b] = self.offsets[c] + min(max(round(noise_start * sr), 0), clip_len - n)
+        return NoiseDraws(self, add, clip, level, rand, start)
+
+    def _device_args(self, draws: NoiseDraws, lengths, device):
+        """(bank, bank_len, start, level) for b200asr_stft_features_ex, or None when no utterance takes noise."""
+        if draws.bank is not self:
+            raise ValueError("the draws were made by another NoiseBank")
+        if len(draws.start) != len(lengths):
+            raise ValueError(f"{len(draws.start)} noise draws for {len(lengths)} utterances")
+        noisy = draws.start >= 0
+        if not noisy.any():
+            return None
+        lengths = np.asarray(lengths, dtype=np.int64)
+        c = draws.clip[noisy]
+        if ((c < 0) | (c >= len(self))).any() or (draws.start[noisy] < self.offsets[c]).any() or \
+                (draws.start[noisy] + lengths[noisy] > self.offsets[c] + self.lengths[c]).any():
+            raise ValueError("a noise segment does not lie inside its clip")
+        if self.bank.device != torch.device(device):
+            raise ValueError(f"the noise bank is on {self.bank.device}, the batch on {device}")
+        return (self.bank, self.bank.numel(), _pinned_to(draws.start.astype(np.int64), device),
+                _pinned_to(draws.level.astype(np.float32), device))
+
+
+def _geometry(sample_rate, window_size, window_stride):
+    return int(sample_rate * window_size), int(sample_rate * window_stride)
+
+
+def _features(wave, lens, t_max, n_fft, hop, normalize, reflect, precision, window, window_periodic, noise, max_frames):
+    """One b200asr_stft_features_ex call on a [B, Lmax] device batch: (inputs [B,1,F,t_max], frames [B] int32)."""
+    B, Lmax = wave.shape
+    nb = n_fft // 2 + 1
+    lib = ops._lib()
+    ws = torch.empty(lib.b200asr_stft_features_ex_ws_bytes(B, Lmax, n_fft, hop) // 4, device=wave.device, dtype=torch.float32)
+    out = torch.empty((B, 1, nb, t_max), device=wave.device, dtype=torch.float32)
+    frames = torch.empty(B, device=wave.device, dtype=torch.int32)
+    prec = ops.config.linear if precision is None else precision
+    prec = {L.PREC_BF16X3: L.PREC_TF32X3, L.PREC_BF16: L.PREC_TF32}.get(prec, prec)      # the DFT basis is an fp32 operand: tf32 grades
+    bank, bank_len, start, level = noise if noise is not None else (None, 0, None, None)
+    L.check(lib.b200asr_stft_features_ex(L.ptr(wave), L.ptr(lens), L.ptr(out), L.ptr(frames), L.ptr(ws), B, Lmax, t_max, n_fft,
+                                         hop, int(reflect), int(normalize), WINDOWS.get(window, 0), int(window_periodic),
+                                         L.ptr(bank), bank_len, L.ptr(start), L.ptr(level), NO_CUT if max_frames is None else max_frames,
+                                         prec, ops._stream()), "stft_features_ex")
+    return out, frames
+
+
 def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: torch.Tensor | None = None, sample_rate: int = 16000,
                       window_size: float = 0.02, window_stride: float = 0.01, normalize: bool = True, reflect: bool = True,
-                      precision: int | None = None, window_periodic: bool = False):
+                      precision: int | None = None, window_periodic: bool = False, window: str = "hamming",
+                      noise: NoiseDraws | None = None, max_frames: int | None = None):
     """waves: list of 1-D CUDA float tensors, or a zero-padded [B, L_max] CUDA tensor with `lengths` (int32 samples).
+    `window`: "hamming", "hann", "blackman" or "bartlett" (any other name: Hamming, as the reference).  `noise`: draws of
+    `NoiseBank.draw` for these utterances, in this order.  `max_frames`: keep at most this many frames of each utterance
+    after normalising over all of them (the reference's src_max_len cut).
     Returns (inputs [B,1,F,T_max] fp32, input_percentages [B] fp32, input_sizes [B] int32), all on the device."""
-    n_fft, hop = int(sample_rate * window_size), int(sample_rate * window_stride)
+    n_fft, hop = _geometry(sample_rate, window_size, window_stride)
     if isinstance(waves, torch.Tensor):
         if lengths is None:
             raise ValueError("a padded batch needs `lengths`")
@@ -35,15 +165,63 @@ def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: tor
             wave[b, : w.numel()] = w
     ops._need_cuda(wave, lens)
     wave = ops._f32c(wave)
-    B, Lmax = wave.shape
+    if max_frames is not None and max_frames < 1:
+        raise ValueError(f"max_frames={max_frames}")
     t_max = 1 + int(lens.max().item()) // hop
-    nb = n_fft // 2 + 1
-    lib = ops._lib()
-    ws = torch.empty(lib.b200asr_stft_ws_bytes(B, Lmax, n_fft, hop) // 4, device=wave.device, dtype=torch.float32)
-    out = torch.empty((B, 1, nb, t_max), device=wave.device, dtype=torch.float32)
-    frames = torch.empty(B, device=wave.device, dtype=torch.int32)
-    prec = ops.config.linear if precision is None else precision
-    prec = {L.PREC_BF16X3: L.PREC_TF32X3, L.PREC_BF16: L.PREC_TF32}.get(prec, prec)      # the DFT basis is an fp32 operand: tf32 grades
-    L.check(lib.b200asr_stft_features(L.ptr(wave), L.ptr(lens), L.ptr(out), L.ptr(frames), L.ptr(ws), B, Lmax, t_max, n_fft, hop,
-                                      int(reflect), int(normalize), int(window_periodic), prec, ops._stream()), "stft_features")
+    if max_frames is not None:
+        t_max = min(t_max, max_frames)
+    dev_noise = None if noise is None else noise.bank._device_args(noise, lens.cpu().numpy(), wave.device)
+    out, frames = _features(wave, lens, t_max, n_fft, hop, normalize, reflect, precision, window, window_periodic, dev_noise,
+                            max_frames)
     return out, frames.float() / float(t_max), frames
+
+
+def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBank | None = None, normalize: bool = True,
+                  rng=np.random, precision: int | None = None, reflect: bool = True):
+    """`_collate_fn` (utils/data_loader.py:182-214) over waveforms: what a DataLoader over the reference's
+    `SpectrogramDataset` yields, computed on the device.
+
+    batch: list of (waveform, transcript ids); waveforms are 1-D fp32 host arrays (numpy or CPU tensors).  audio_conf: the
+    dict train.py builds (sample_rate, window_size, window_stride, window, noise_dir, noise_prob, noise_levels).  With
+    audio_conf["noise_dir"] set, noise is drawn from `noise_bank` (ValueError without one) in batch order, before
+    sorting, as `__getitem__` draws it.  Each spectrogram is normalised over the whole utterance, then cut to
+    `src_max_len` frames (:131).
+
+    Returns (inputs [B,1,F,T] fp32 on the current CUDA device, targets [B,max_tgt] int64, input_percentages [B] fp32,
+    input_sizes [B] int32, target_sizes [B] int32), the last four on the host, sorted by frame count, longest first
+    (stable).  It launches CUDA work and does not synchronise with the host, so it belongs in the main process rather than
+    in DataLoader workers: let the workers return (waveform, ids) lists and call this on each batch."""
+    sr = audio_conf["sample_rate"]
+    n_fft, hop = _geometry(sr, audio_conf["window_size"], audio_conf["window_stride"])
+    if src_max_len < 1:
+        raise ValueError(f"src_max_len={src_max_len}")
+    waves = [np.asarray(w.detach().cpu() if isinstance(w, torch.Tensor) else w, dtype=np.float32).reshape(-1) for w, _ in batch]
+    lens = [len(w) for w in waves]
+    draws = None
+    if audio_conf.get("noise_dir") is not None:
+        if noise_bank is None:
+            raise ValueError("audio_conf['noise_dir'] is set but no noise_bank was given")
+        draws = noise_bank.draw(lens, audio_conf["noise_prob"], audio_conf["noise_levels"], rng)
+    frames = [min(1 + n // hop, src_max_len) for n in lens]
+    order = sorted(range(len(batch)), key=frames.__getitem__, reverse=True)          # sorted(..., reverse=True) is stable
+    B, Lmax = len(batch), max(1, max(lens))
+    host = torch.empty((B, Lmax), dtype=torch.float32, pin_memory=True)           # packed in place, uploaded without a sync
+    h = host.numpy()
+    for r, i in enumerate(order):
+        h[r, :lens[i]] = waves[i]
+        h[r, lens[i]:] = 0.0
+    device = torch.device("cuda", torch.cuda.current_device())
+    slens = np.array([lens[i] for i in order], dtype=np.int32)
+    dev_noise = None if draws is None else noise_bank._device_args(draws.take(order), slens, device)
+    t_max = frames[order[0]]
+    inputs, _ = _features(host.to(device, non_blocking=True), _pinned_to(slens, device), t_max, n_fft, hop, normalize, reflect,
+                          precision, audio_conf.get("window", "hamming"), False, dev_noise, src_max_len)
+    targets_list = [batch[i][1] for i in order]
+    max_tgt = max(len(t) for t in targets_list)
+    targets = torch.zeros(B, max_tgt, dtype=torch.int64)
+    for r, t in enumerate(targets_list):
+        targets[r, :len(t)] = torch.tensor(list(t), dtype=torch.int32)
+    input_sizes = torch.tensor([frames[i] for i in order], dtype=torch.int32)
+    input_percentages = torch.tensor([frames[i] / float(t_max) for i in order], dtype=torch.float32)
+    target_sizes = torch.tensor([len(t) for t in targets_list], dtype=torch.int32)
+    return inputs, targets, input_percentages, input_sizes, target_sizes

@@ -546,6 +546,31 @@ size_t b200asr_stft_ws_bytes(int B, int Lmax, int n_fft, int hop);
 int b200asr_stft_features(const float* wave, const int* lens, float* out, int* frames_out, void* ws, int B,
                           int Lmax, int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window_periodic,
                           int precision, b200asr_stream_t stream);
+/* The same front end with the rest of the reference's loader options (utils/data_loader.py:20-21,52,126-179):
+ *   window: 0 Hamming, 1 Hann, 2 Blackman, 3 Bartlett (scipy's definitions; symmetric unless window_periodic), else
+ *     B200ASR_BAD_ARG.
+ *   Noise injection (NoiseInjection.inject_noise_sample, :168-179): noise_bank [noise_bank_len] fp32 holds the noise clips
+ *     back to back; per utterance noise_start[b] (int64) is the first sample of its segment in the bank, < 0 for no noise,
+ *     and noise_level[b] its level.  A noisy utterance of len samples becomes, before framing,
+ *       x + ((level * n) * e_x) / e_n   (fp32, in numpy's order),  n = bank[start : start + len],
+ *     with e_x, e_n = sqrt(sum of squares / len) of x and n, the sums in double with a fixed reduction order.  A silent
+ *     segment gives NaN features (0/0, as in the reference); a silent utterance is unchanged.  All three pointers are
+ *     device arrays, NULL together (no noise; otherwise B200ASR_BAD_ARG), and noise_bank_len > 0 with a bank
+ *     (B200ASR_BAD_SHAPE).  The caller guarantees start + lens[b] <= noise_bank_len: the starts are device data, which the
+ *     library does not read on the host; an utterance whose segment leaves the bank comes back NaN, nothing outside the
+ *     bank is read.
+ *   max_frames >= 1 (else B200ASR_BAD_SHAPE): the src_max_len cut (:131).  The statistics cover all 1 + lens[b]/hop
+ *     frames of each utterance; frames t < min(1 + lens[b]/hop, max_frames, Tmax) are stored and frames_out[b] reports
+ *     that count.  A max_frames no utterance reaches gives the bits of an uncut call.
+ * With window 0, no noise and Tmax >= every utterance's 1 + lens[b]/hop frames, the output equals b200asr_stft_features's
+ * bit for bit.  Other arguments and rejections as b200asr_stft_features; ws: b200asr_stft_features_ex_ws_bytes(B, Lmax,
+ * n_fft, hop) bytes.  Launches: as b200asr_stft_features, + 2 with noise (energies, their reduction).  A rejected call
+ * launches nothing. */
+size_t b200asr_stft_features_ex_ws_bytes(int B, int Lmax, int n_fft, int hop);
+int b200asr_stft_features_ex(const float* wave, const int* lens, float* out, int* frames_out, void* ws, int B, int Lmax,
+                             int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window, int window_periodic,
+                             const float* noise_bank, long long noise_bank_len, const long long* noise_start,
+                             const float* noise_level, int max_frames, int precision, b200asr_stream_t stream);
 
 #ifdef __cplusplus
 }
