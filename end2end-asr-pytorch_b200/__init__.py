@@ -7,15 +7,15 @@ needs the built library and an H100.
 from . import _lib
 from .config import ASRConfig, BASELINE_CONFIGS
 from .features import NoiseBank, collate_waves, spectrogram_batch
-from .install import install, uninstall
-from .metrics import calculate_loss, calculate_metrics, loss_and_stats
+from .install import install, original, uninstall
+from .metrics import LabelTable, calculate_loss, calculate_metrics, edit_counts, loss_and_stats
 from .modules import (LM, Decoder, DecoderLayer, Encoder, EncoderLayer, MultiHeadAttention, PositionalEncoding,
                       PositionwiseFeedForwardWithConv, RNNModel, ScaledDotProductAttention, Transformer, build_model)
 from .ops import config as precision, manual_seed
 from .optim import FlatParams, FusedAdam, NoamOpt
 from .parallel import DataParallelStep, HostBatchPrefetcher, shard_batch
 
-__all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "calculate_loss", "calculate_metrics",
-           "loss_and_stats", "Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
+__all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "original", "calculate_loss", "calculate_metrics",
+           "loss_and_stats", "LabelTable", "edit_counts","Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
            "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model", "RNNModel", "LM",
            "precision", "manual_seed", "spectrogram_batch", "NoiseBank", "collate_waves","FlatParams", "FusedAdam", "NoamOpt", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]

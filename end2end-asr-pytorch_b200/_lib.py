@@ -112,6 +112,8 @@ SIGNATURES = {
     "b200asr_sumsq": (_i, [_vp, _ll, _vp, _vp]),
     "b200asr_grad_scale": (_i, [_vp, _ll, _vp, _f, _vp, _vp, _vp]),
     "b200asr_permute_cols_cf": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "b200asr_edit_counts_ws_bytes": (_sz, [_i, _i, _i, _i]),
+    "b200asr_edit_counts": (_i, [_vp, _i, _ll, _i, _vp, _i, _ll, _i, _i] + [_vp] * 5 + [_i, _i, _ll, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -5,7 +5,8 @@
 After this, the reference's own `Transformer` (models/asr/transformer.py), `Trainer` loop
 (trainer/asr/trainer.py), `test.py` and the LSTM LM's `RNNModel.forward` (utils/lstm_utils.py) run on libb200asr kernels:
 module tree, parameter names and checkpoints are untouched; only `forward` attributes, `Decoder.beam_search`,
-`Decoder.greedy_search`, `Transformer.evaluate` and the two loss functions are rebound (SURVEY.md §8b).  The replaced methods
+`Decoder.greedy_search`, `Transformer.evaluate`, the two loss functions and, when trainer/asr/trainer.py is imported,
+`Trainer.train` (trainer.trainer_train: the CER / WER counts on the device) are rebound (SURVEY.md §8b).  The replaced methods
 stay reachable through original(): LM rescoring with an LM other than an LSTM LM still runs the reference's beam_search, a
 GRU / RNN LM its own RNNModel.forward, greedy_search with lm_rescoring=True or in training mode and evaluate in training
 mode the reference's own methods.
@@ -15,7 +16,7 @@ from __future__ import annotations
 import importlib
 import sys
 
-from . import metrics, modules
+from . import metrics, modules, trainer
 
 _PATCHED = {}
 
@@ -53,6 +54,7 @@ def install(reference_root: str = None):
     t_mod = sys.modules.get("trainer.asr.trainer")      # `from utils.metrics import calculate_metrics` binds by value
     if t_mod is not None:
         targets.append((t_mod, "calculate_metrics", metrics.calculate_metrics))
+        targets.append((t_mod.Trainer, "train", trainer.trainer_train))
     for obj, name, new in targets:
         key = (id(obj), name)
         if key not in _PATCHED:

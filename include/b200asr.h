@@ -572,6 +572,41 @@ int b200asr_stft_features_ex(const float* wave, const int* lens, float* out, int
                              const float* noise_bank, long long noise_bank_len, const long long* noise_start,
                              const float* noise_level, int max_frames, int precision, b200asr_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Edit counts of the training loop's CER / WER (trainer/asr/trainer.py:60-79, 96-104 and 153-182), with no host read per
+ * token.  Per utterance b the strings h (from hyp row b) and g (from gold row b) are built as the trainer builds them: the
+ * ids in order up to the first pad_id, the labels of the ids joined.  Then
+ *   per_utt[b][0] = cer_edits  = Levenshtein(h without ' ', g without ' ') over code points   (calculate_cer)
+ *   per_utt[b][1] = wer_edits  = Levenshtein over words, a word being a maximal run of code points that are not
+ *                                str.isspace(); two words are equal when their code points are      (calculate_wer)
+ *   per_utt[b][2] = gold_chars = number of code points of g other than ' '
+ *   per_utt[b][3] = gold_words = (number of ' ' in g) + 1                                          (len(g.split(" ")))
+ *   totals[0..3]  = the sums of the four columns over b = 0 .. B-1 in order; totals[4] = the first invalid id met in the
+ *                   trainer's order -- every gold row before any hyp row, tokens in order within a row, each row up to its
+ *                   first pad_id -- or -1 when every such id is valid (an id of -1 itself is therefore not told apart).
+ *   An invalid id contributes no code points.
+ * hyp [B][T_h] and gold [B][T_g]: ids, int64 (*_int64 = 1) or int32 (0), row b at hyp + b * hyp_row_stride (elements);
+ *   row strides >= T.  T_h, T_g >= 0, B >= 1.
+ * The label table (CSR, device arrays): for id in [0, V), label_valid[id] != 0 marks a valid id, whose label is the
+ *   label_len[id] code points code_points[label_off[id] ..] (int32, 0 .. 0x10FFFF); per code point, cp_flags bit 0 = the
+ *   code point is ' ' (U+0020) and bit 1 = str.isspace().  Ids < 0 or >= V are invalid.  Every label_len[id] <=
+ *   max_label_len: an utterance whose strings outgrow what that bound allows gets -1 in its four counts.  The trainer's
+ *   SOS / EOS removal is the table builder's: it drops those code points from every label.
+ * ws: b200asr_edit_counts_ws_bytes(B, T_h, T_g, max_label_len) bytes, 16-byte aligned, caller-owned: 16 * B bytes for the
+ *   first invalid position of every row, plus, when the longest strings the shapes allow would not fit in 46 KB of shared
+ *   memory, a buffer per utterance that utterances too long for shared memory expand into.  Its size grows as
+ *   B * (T_h + T_g) * max_label_len; 0 for shapes whose per-utterance buffer would pass 2^30 int32 entries (about
+ *   (T_h + T_g) * max_label_len > 2^28; the call rejects those shapes).
+ * Return: B200ASR_BAD_ARG for a NULL pointer or an *_int64 other than 0 / 1, B200ASR_BAD_SHAPE for the shapes above,
+ *   B200ASR_BAD_ALIGN for ids / table / outputs not aligned to their element or ws not to 16 bytes.  A rejected call launches
+ *   nothing.  Launches: 2 (one CTA per utterance, then one for the totals).  No host synchronisation and no atomics: repeated
+ *   calls give identical bits.  Exact anti-diagonal DP, O(|h| |g|) work and |h| + |g| barriers per utterance. */
+size_t b200asr_edit_counts_ws_bytes(int B, int T_h, int T_g, int max_label_len);
+int b200asr_edit_counts(const void* hyp, int hyp_int64, long long hyp_row_stride, int T_h, const void* gold, int gold_int64,
+                        long long gold_row_stride, int T_g, int B, const int* label_off, const int* label_len,
+                        const int* code_points, const uint8_t* cp_flags, const uint8_t* label_valid, int V, int max_label_len,
+                        long long pad_id, int64_t* per_utt, int64_t* totals, void* ws, b200asr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
