@@ -61,6 +61,11 @@ SIGNATURES = {
     "b200asr_maxpool2x2_fwd_idx": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200asr_maxpool2x2_bwd_idx": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_bwd_data": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200asr_conv3x3_c1_fwd_bits": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "b200asr_conv3x3_fwd_bits": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "b200asr_conv3x3_bwd_data_bits": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200asr_conv3x3_fwd_pool_codes": (_i, [_vp] * 7 + [_i] * 7 + [_vp]),
+    "b200asr_maxpool2x2_bwd_codes": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_bwd_weight": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_ws_bytes": (_sz, [_i, _i]),
     "b200asr_maxpool2x2_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),

@@ -15,11 +15,14 @@ namespace b200asr {
 // x [B,F,T] -> y [B,T,F,Co]; weights w[Co][1][3(f)][3(t)].  A CTA owns a 32 (time) x 8 (freq) pixel tile: the input patch
 // with halo (10 x 34 floats) is staged in shared memory with loads coalesced along time, and each thread owns one channel
 // quad, so a warp stores 2 pixels x 256 B = 512 contiguous bytes.  Store-bound by design (1.06 GB at cfg2).
+// bits (optional, Co % 32 == 0): y > 0 packed as [B,T,F,Co/32] words, bit c % 32 of word c / 32; the 8 lanes holding a word's
+// channel quads OR their nibbles together.  Every lane runs the same number of pixel trips (256 % slots == 0), so the shuffles
+// see the whole warp; pixels outside the image are computed from the zero-filled patch and not stored.
 constexpr int C1_TT = 32, C1_TF = 8;
 
 __global__ void __launch_bounds__(256) conv3x3_c1_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                              const float* __restrict__ bias, float* __restrict__ y,
-                                                             int B, int F, int T, int Co, int relu) {
+                                                             uint32_t* __restrict__ bits, int B, int F, int T, int Co, int relu) {
   __shared__ float patch[C1_TF + 2][C1_TT + 2 + 1];
   const int cqs = Co >> 2;
   const int cq = threadIdx.x % cqs;
@@ -43,7 +46,8 @@ __global__ void __launch_bounds__(256) conv3x3_c1_fwd_kernel(const float* __rest
   for (int px = slot; px < C1_TT * C1_TF; px += slots) {      // pixel order: freq fastest -> contiguous output
     const int tl = px / C1_TF, fl = px - tl * C1_TF;
     const int t = t0 + tl, f = f0 + fl;
-    if (t >= T || f >= F) continue;
+    const bool inside = t < T && f < F;
+    if (!inside && !bits) continue;
     float o[4] = {br[0], br[1], br[2], br[3]};
 #pragma unroll
     for (int df = 0; df < 3; df++)
@@ -54,7 +58,15 @@ __global__ void __launch_bounds__(256) conv3x3_c1_fwd_kernel(const float* __rest
         for (int c = 0; c < 4; c++) o[c] = fmaf(v, wr[c][df * 3 + dt], o[c]);
       }
     if (relu) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); o[2] = fmaxf(o[2], 0.f); o[3] = fmaxf(o[3], 0.f); }
-    *reinterpret_cast<float4*>(y + (((size_t)b * T + t) * F + f) * Co + cq * 4) = make_float4(o[0], o[1], o[2], o[3]);
+    const size_t pix = ((size_t)b * T + t) * F + f;
+    if (inside) *reinterpret_cast<float4*>(y + pix * Co + cq * 4) = make_float4(o[0], o[1], o[2], o[3]);
+    if (bits) {
+      uint32_t wd = ((o[0] > 0.f ? 1u : 0u) | (o[1] > 0.f ? 2u : 0u) | (o[2] > 0.f ? 4u : 0u) | (o[3] > 0.f ? 8u : 0u)) << (4 * (cq & 7));
+      wd |= __shfl_xor_sync(0xffffffffu, wd, 1);
+      wd |= __shfl_xor_sync(0xffffffffu, wd, 2);
+      wd |= __shfl_xor_sync(0xffffffffu, wd, 4);
+      if (inside && (cq & 7) == 0) bits[pix * (Co >> 5) + (cq >> 3)] = wd;
+    }
   }
 }
 
@@ -190,8 +202,9 @@ constexpr int CBM = 128, CBK = 16, CLD = 132;
 template <int BN>
 __global__ void __launch_bounds__(256) conv3x3_igemm_kernel(const float* __restrict__ in, const float* __restrict__ wr,
                                                             const float* __restrict__ bias,
-                                                            const float* __restrict__ mask, float* __restrict__ out,
-                                                            int B, int T, int F, int Cin, int Cout, int relu) {
+                                                            const float* __restrict__ mask, const uint32_t* __restrict__ mask_bits,
+                                                            float* __restrict__ out, int B, int T, int F, int Cin, int Cout,
+                                                            int relu) {
   __shared__ __align__(16) float As[2][CBK][CLD];
   __shared__ __align__(16) float Bs[2][CBK][BN + 4];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -299,6 +312,11 @@ __global__ void __launch_bounds__(256) conv3x3_igemm_kernel(const float* __restr
         float4 m = *reinterpret_cast<const float4*>(mask + off);
         v[0] = m.x > 0.f ? v[0] : 0.f; v[1] = m.y > 0.f ? v[1] : 0.f;
         v[2] = m.z > 0.f ? v[2] : 0.f; v[3] = m.w > 0.f ? v[3] : 0.f;
+      }
+      if (mask_bits) {   // the four bits of col .. col + 3 (col % 4 == 0) of the pixel's words
+        const uint32_t m = __ldg(mask_bits + (size_t)p * (Cout >> 5) + (col >> 5)) >> (col & 31);
+#pragma unroll
+        for (int j = 0; j < 4; j++) v[j] = (m >> j) & 1u ? v[j] : 0.f;
       }
       *reinterpret_cast<float4*>(out + off) = make_float4(v[0], v[1], v[2], v[3]);
     }
@@ -415,7 +433,9 @@ __device__ __forceinline__ uint32_t pool_code(float a0, float a1, float a2, floa
   return (uint32_t)best | (m > 0.f ? 0u : 4u);
 }
 
-__global__ void maxpool2x2_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, uint8_t* __restrict__ idx, int B, int T, int F, int C) {
+// codes (optional): the same codes as nibbles, 8 channels per 32-bit word (the layout of b200asr_conv3x3_fwd_pool_codes)
+__global__ void maxpool2x2_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, uint8_t* __restrict__ idx,
+                                      uint16_t* __restrict__ codes, int B, int T, int F, int C) {
   const int T2 = T / 2, F2 = F / 2, C4 = C / 4;
   long long n = (long long)B * T2 * F2 * C4;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -440,6 +460,9 @@ __global__ void maxpool2x2_fwd_kernel(const float* __restrict__ x, float* __rest
   if (idx)      // scan order: (f, t) = a, (f, t+1) = cq, (f+1, t) = bq, (f+1, t+1) = d
     *reinterpret_cast<uint32_t*>(idx + po) = pool_code(a.x, cq.x, bq.x, d.x) | (pool_code(a.y, cq.y, bq.y, d.y) << 8) |
                                              (pool_code(a.z, cq.z, bq.z, d.z) << 16) | (pool_code(a.w, cq.w, bq.w, d.w) << 24);
+  if (codes)    // four channels = the low or high half of a word (c % 4 == 0)
+    codes[po >> 2] = (uint16_t)(pool_code(a.x, cq.x, bq.x, d.x) | (pool_code(a.y, cq.y, bq.y, d.y) << 4) |
+                                (pool_code(a.z, cq.z, bq.z, d.z) << 8) | (pool_code(a.w, cq.w, bq.w, d.w) << 12));
 }
 
 // one thread = one 2x2 window x 4 channels; writes all four dx positions (and zeroes are written for the odd tails
@@ -500,7 +523,9 @@ __global__ void maxpool2x2_bwd_kernel(const float* __restrict__ dy, const float*
     for (int k = 0; k < 4; k++) store_pairs4(dx16, lo_off, base + offs[k], out[k]);
   }
 }
-// the same routing from the forward's index bytes: reads dy and one byte per pooled element instead of the activation
+// the same routing from the forward's codes: reads dy and one byte (kNibble: half a byte) per pooled element instead of the
+// activation
+template <bool kNibble>
 __global__ void maxpool2x2_bwd_idx_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ idx, float* __restrict__ dx,
                                           uint16_t* __restrict__ dx16, int B, int T, int F, int C, int relu_mask) {
   const int T2 = T / 2, F2 = F / 2, C4 = C / 4;
@@ -514,12 +539,13 @@ __global__ void maxpool2x2_bwd_idx_kernel(const float* __restrict__ dy, const ui
   int b = (int)(r / T2);
   const size_t po = (((size_t)b * T2 + t2) * F2 + f2) * C + c;
   const float4 g = *reinterpret_cast<const float4*>(dy + po);
-  const uint32_t codes = *reinterpret_cast<const uint32_t*>(idx + po);
+  const uint32_t codes = kNibble ? (uint32_t)reinterpret_cast<const uint16_t*>(idx)[po >> 2] : *reinterpret_cast<const uint32_t*>(idx + po);
+  constexpr int kS = kNibble ? 4 : 8;                       // bits per code slot
   const size_t base = (((size_t)b * T + 2 * t2) * F + 2 * f2) * C + c;
   const size_t o_f = C, o_t = (size_t)F * C;
   const size_t offs[4] = {0, o_t, o_f, o_f + o_t};         // scan order, as in maxpool2x2_bwd_kernel
   const uint32_t dead = relu_mask ? 4u : 8u;                // bit 2 = "maximum not positive" counts only behind a ReLU
-  const uint32_t c0 = codes & 7u, c1 = (codes >> 8) & 7u, c2 = (codes >> 16) & 7u, c3 = (codes >> 24) & 7u;
+  const uint32_t c0 = codes & 7u, c1 = (codes >> kS) & 7u, c2 = (codes >> (2 * kS)) & 7u, c3 = (codes >> (3 * kS)) & 7u;
   float4 out[4];
 #pragma unroll
   for (int k = 0; k < 4; k++) {
@@ -561,16 +587,25 @@ __global__ void maxpool2x2_bwd_tail_kernel(float* __restrict__ dx, uint16_t* __r
   }
 }
 
+// bits[i / 32] bit i % 32 = (y[i] > 0) for i < n (n % 32 == 0): one warp ballot per word.  The forward of the precisions
+// whose epilogue cannot gather a word (precision 0 here) packs its ReLU decisions with this pass.
+__global__ void relu_bits_kernel(const float* __restrict__ y, uint32_t* __restrict__ bits, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i - (threadIdx.x & 31) >= n) return;   // whole warps leave together
+  const uint32_t wd = __ballot_sync(0xffffffffu, i < n && y[i] > 0.f);
+  if ((threadIdx.x & 31) == 0) bits[i >> 5] = wd;
+}
+
 // host-side launchers used by the API and (for precision 0) nothing else
 int conv3x3_simt(const float* in, const float* wr, const float* bias, const float* mask, float* out, int B, int T, int F,
-                 int Cin, int Cout, int relu, cudaStream_t st) {
+                 int Cin, int Cout, int relu, cudaStream_t st, const uint32_t* mask_bits = nullptr) {
   long long P = (long long)B * T * F;
   if (Cout % 128 == 0) {
     dim3 grid(Cout / 128, (unsigned)ceil_div_ll(P, CBM));
-    conv3x3_igemm_kernel<128><<<grid, 256, 0, st>>>(in, wr, bias, mask, out, B, T, F, Cin, Cout, relu);
+    conv3x3_igemm_kernel<128><<<grid, 256, 0, st>>>(in, wr, bias, mask, mask_bits, out, B, T, F, Cin, Cout, relu);
   } else {
     dim3 grid(Cout / 64, (unsigned)ceil_div_ll(P, CBM));
-    conv3x3_igemm_kernel<64><<<grid, 256, 0, st>>>(in, wr, bias, mask, out, B, T, F, Cin, Cout, relu);
+    conv3x3_igemm_kernel<64><<<grid, 256, 0, st>>>(in, wr, bias, mask, mask_bits, out, B, T, F, Cin, Cout, relu);
   }
   return check_launch("conv3x3_igemm");
 }
@@ -599,12 +634,8 @@ using namespace b200asr;
 // entry point checks the pointers it hands to them, so a misaligned view is an error rather than a faulting launch
 static inline bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
 
-extern "C" {
-
-size_t b200asr_conv3x3_ws_bytes(int Ci, int Co) { return sizeof(float) * 2 * 9 * (size_t)Ci * Co; }   // [hi | lo] weight halves
-
-int b200asr_conv3x3_c1_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int T, int Co,
-                           int relu, b200asr_stream_t stream) {
+static int conv_c1_fwd(const float* x, const float* w, const float* bias, float* y, uint32_t* bits, int B, int F, int T, int Co,
+                       int relu, b200asr_stream_t stream) {
   B200_REQUIRE(x && w && y, B200ASR_BAD_ARG, "conv3x3_c1_fwd: null pointer");
   B200_REQUIRE(Co % 4 == 0 && Co <= 1024 && 256 % (Co / 4) == 0, B200ASR_BAD_SHAPE, "conv3x3_c1_fwd: Co=%d unsupported", Co);
   B200_REQUIRE(aligned16(y), B200ASR_BAD_ALIGN, "conv3x3_c1_fwd: y alignment");
@@ -612,8 +643,25 @@ int b200asr_conv3x3_c1_fwd(const float* x, const float* w, const float* bias, fl
   if (P <= 0) return B200ASR_OK;
   B200_REQUIRE(B <= 65535 && ceil_div(F, C1_TF) <= 65535, B200ASR_BAD_SHAPE, "conv3x3_c1_fwd: grid too large");
   dim3 grid(ceil_div(T, C1_TT), ceil_div(F, C1_TF), B);
-  conv3x3_c1_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, bias, y, B, F, T, Co, relu);
+  conv3x3_c1_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, bias, y, bits, B, F, T, Co, relu);
   return check_launch("conv3x3_c1_fwd");
+}
+
+extern "C" {
+
+size_t b200asr_conv3x3_ws_bytes(int Ci, int Co) { return sizeof(float) * 2 * 9 * (size_t)Ci * Co; }   // [hi | lo] weight halves
+
+int b200asr_conv3x3_c1_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int T, int Co,
+                           int relu, b200asr_stream_t stream) {
+  return conv_c1_fwd(x, w, bias, y, nullptr, B, F, T, Co, relu, stream);
+}
+
+int b200asr_conv3x3_c1_fwd_bits(const float* x, const float* w, const float* bias, float* y, int B, int F, int T, int Co,
+                                int relu, uint32_t* y_bits, b200asr_stream_t stream) {
+  B200_REQUIRE(y_bits, B200ASR_BAD_ARG, "conv3x3_c1_fwd_bits: null pointer");
+  B200_REQUIRE(Co % 32 == 0, B200ASR_BAD_SHAPE, "conv3x3_c1_fwd_bits: Co=%d must be a multiple of 32", Co);
+  B200_REQUIRE(aligned_to(y_bits, 4), B200ASR_BAD_ALIGN, "conv3x3_c1_fwd_bits: y_bits needs 4-byte alignment");
+  return conv_c1_fwd(x, w, bias, y, y_bits, B, F, T, Co, relu, stream);
 }
 
 int b200asr_conv3x3_c1_bwd_weight(const float* x, const float* dy, float* dw, float* dbias, int B, int F, int T, int Co,
@@ -669,8 +717,10 @@ static int conv_shape_ok(const char* who, int Ci, int Co) {
   return B200ASR_OK;
 }
 
-int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int T, int F,
-                        int Ci, int Co, int relu, int precision, b200asr_stream_t stream) {
+// y_bits (optional): [B,T,F,Co/32] words of (y > 0), written by the convolution's epilogue -- except at precision 0, whose
+// CUDA-core kernel has no lane group holding a word's 32 channels: it packs them in a ballot pass over y (one more launch)
+static int conv_fwd(const float* x, const float* w, const float* bias, float* y, uint32_t* y_bits, void* ws, int B, int T, int F,
+                    int Ci, int Co, int relu, int precision, b200asr_stream_t stream) {
   B200_REQUIRE(x && w && y && ws, B200ASR_BAD_ARG, "conv3x3_fwd: null pointer");
   int rc = conv_shape_ok("conv3x3_fwd", Ci, Co);
   if (rc) return rc;
@@ -681,25 +731,46 @@ int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float
   note_launch(1);
   if (precision == B200ASR_PREC_FP32) {
     conv_repack_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (float*)ws, Ci, Co, 0);
-    return conv3x3_simt(x, (const float*)ws, bias, nullptr, y, B, T, F, Ci, Co, relu, st);
+    rc = conv3x3_simt(x, (const float*)ws, bias, nullptr, y, B, T, F, Ci, Co, relu, st);
+    const long long n = (long long)B * T * F * Co;
+    if (rc || !y_bits || n <= 0) return rc;
+    relu_bits_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(y, y_bits, n);
+    return check_launch("relu_bits");
   }
   if (conv_is_bf16(precision)) {
     B200_REQUIRE(Ci % 32 == 0 && (Co == 64 || Co == 128), B200ASR_BAD_SHAPE, "conv3x3_fwd (bf16): needs Ci %% 32 == 0 and Co in {64,128}");
     conv_repack_k_bf16_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (uint16_t*)ws, Ci, Co, 0, precision == B200ASR_PREC_BF16X3 ? 2 : 1);
-    return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st);
+    return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st, nullptr, nullptr, nullptr, y_bits);
   }
   conv_repack_k_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (float*)ws, Ci, Co, 0, precision == B200ASR_PREC_TF32X3);
-  if (precision == B200ASR_PREC_TF32X3) return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st);
-  return conv3x3_tc(x, (const float*)ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st);
+  if (precision == B200ASR_PREC_TF32X3)
+    return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st, nullptr, nullptr, nullptr, y_bits);
+  return conv3x3_tc(x, (const float*)ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st, nullptr, y_bits);
 }
 
-int b200asr_conv3x3_fwd_pool(const float* x, const float* w, const float* bias, float* y, float* pooled, unsigned char* pool_idx, void* ws,
-                             int B, int T, int F, int Ci, int Co, int relu, int precision, b200asr_stream_t stream) {
-  B200_REQUIRE(x && w && y && pooled && ws, B200ASR_BAD_ARG, "conv3x3_fwd_pool: null pointer");
+int b200asr_conv3x3_fwd(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int T, int F,
+                        int Ci, int Co, int relu, int precision, b200asr_stream_t stream) {
+  return conv_fwd(x, w, bias, y, nullptr, ws, B, T, F, Ci, Co, relu, precision, stream);
+}
+
+int b200asr_conv3x3_fwd_bits(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int T, int F, int Ci,
+                             int Co, int relu, int precision, uint32_t* y_bits, b200asr_stream_t stream) {
+  B200_REQUIRE(y_bits, B200ASR_BAD_ARG, "conv3x3_fwd_bits: null pointer");
+  B200_REQUIRE(aligned_to(y_bits, 4), B200ASR_BAD_ALIGN, "conv3x3_fwd_bits: y_bits needs 4-byte alignment");
+  return conv_fwd(x, w, bias, y, y_bits, ws, B, T, F, Ci, Co, relu, precision, stream);
+}
+
+// pool_codes (optional): the pooling decisions as nibbles (b200asr_conv3x3_fwd_pool_codes); y may be NULL when the pooling
+// runs in the epilogue (bf16 modes without index bytes), since nothing then reads it back
+static int conv_fwd_pool(const float* x, const float* w, const float* bias, float* y, float* pooled, unsigned char* pool_idx,
+                         uint32_t* pool_codes, void* ws, int B, int T, int F, int Ci, int Co, int relu, int precision,
+                         b200asr_stream_t stream) {
   // the pooling rides in the convolution's epilogue (tc_conv_halo.cu) -- unless the arg-max bytes are wanted as well: computing
   // them there was measured to lengthen the epilogue (the critical path of the Cout = 64 kernel) by more than the index-based
   // pooling backward saves, so that request runs the stand-alone pooling kernel
-  if (conv_is_bf16(precision) && !pool_idx) {
+  const bool epilogue = conv_is_bf16(precision) && !pool_idx;
+  B200_REQUIRE(x && w && pooled && ws && (y || epilogue), B200ASR_BAD_ARG, "conv3x3_fwd_pool: null pointer");
+  if (epilogue) {
     int rc = conv_shape_ok("conv3x3_fwd_pool", Ci, Co);
     if (rc) return rc;
     B200_REQUIRE(Ci % 32 == 0 && (Co == 64 || Co == 128), B200ASR_BAD_SHAPE, "conv3x3_fwd_pool (bf16): needs Ci %% 32 == 0 and Co in {64,128}");
@@ -707,14 +778,37 @@ int b200asr_conv3x3_fwd_pool(const float* x, const float* w, const float* bias, 
     cudaStream_t st = (cudaStream_t)stream;
     note_launch(1);
     conv_repack_k_bf16_kernel<<<ceil_div(9 * Ci * Co, 256), 256, 0, st>>>(w, (uint16_t*)ws, Ci, Co, 0, precision == B200ASR_PREC_BF16X3 ? 2 : 1);
-    return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st, nullptr, pooled);
+    return conv3x3_tc_halo(x, ws, bias, nullptr, y, B, T, F, Ci, Co, relu, precision, st, nullptr, pooled, nullptr, nullptr,
+                           (uint8_t*)pool_codes);
   }
   if (int rc = b200asr_conv3x3_fwd(x, w, bias, y, ws, B, T, F, Ci, Co, relu, precision, stream)) return rc;
-  return pool_idx ? b200asr_maxpool2x2_fwd_idx(y, pooled, pool_idx, B, T, F, Co, stream) : b200asr_maxpool2x2_fwd(y, pooled, B, T, F, Co, stream);
+  if (!pool_codes)
+    return pool_idx ? b200asr_maxpool2x2_fwd_idx(y, pooled, pool_idx, B, T, F, Co, stream) : b200asr_maxpool2x2_fwd(y, pooled, B, T, F, Co, stream);
+  B200_REQUIRE(aligned16(pooled) && aligned_to(pool_idx, 4), B200ASR_BAD_ALIGN, "conv3x3_fwd_pool: pooled needs 16-byte alignment, idx 4-byte");
+  long long n = (long long)B * (T / 2) * (F / 2) * (Co / 4);
+  if (n <= 0) return B200ASR_OK;
+  maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(y, pooled, pool_idx, (uint16_t*)pool_codes,
+                                                                                       B, T, F, Co);
+  return check_launch("maxpool2x2_fwd_codes");
 }
 
-int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_out, float* dx, void* dx16, void* ws, int B, int T,
-                             int F, int Ci, int Co, int precision, b200asr_stream_t stream) {
+int b200asr_conv3x3_fwd_pool(const float* x, const float* w, const float* bias, float* y, float* pooled, unsigned char* pool_idx, void* ws,
+                             int B, int T, int F, int Ci, int Co, int relu, int precision, b200asr_stream_t stream) {
+  B200_REQUIRE(y, B200ASR_BAD_ARG, "conv3x3_fwd_pool: null pointer");
+  return conv_fwd_pool(x, w, bias, y, pooled, pool_idx, nullptr, ws, B, T, F, Ci, Co, relu, precision, stream);
+}
+
+int b200asr_conv3x3_fwd_pool_codes(const float* x, const float* w, const float* bias, float* y, float* pooled, uint32_t* pool_codes,
+                                   void* ws, int B, int T, int F, int Ci, int Co, int relu, int precision, b200asr_stream_t stream) {
+  B200_REQUIRE(pool_codes, B200ASR_BAD_ARG, "conv3x3_fwd_pool_codes: null pointer");
+  B200_REQUIRE(aligned_to(pool_codes, 4), B200ASR_BAD_ALIGN, "conv3x3_fwd_pool_codes: pool_codes needs 4-byte alignment");
+  B200_REQUIRE(Co % 8 == 0, B200ASR_BAD_SHAPE, "conv3x3_fwd_pool_codes: Co=%d must be a multiple of 8", Co);
+  return conv_fwd_pool(x, w, bias, y, pooled, nullptr, pool_codes, ws, B, T, F, Ci, Co, relu, precision, stream);
+}
+
+// relu_out (floats) or relu_bits (the same decisions packed as b200asr_conv3x3_fwd_bits writes them) or neither
+static int conv_bwd_data(const float* dy, const float* w, const float* relu_out, const uint32_t* relu_bits, float* dx, void* dx16,
+                         void* ws, int B, int T, int F, int Ci, int Co, int precision, b200asr_stream_t stream) {
   B200_REQUIRE(dy && w && dx && ws, B200ASR_BAD_ARG, "conv3x3_bwd_data: null pointer");
   int rc = conv_shape_ok("conv3x3_bwd_data", Co, Ci);   // roles swap: contraction over Co, output channels Ci
   if (rc) return rc;
@@ -726,17 +820,30 @@ int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_
   note_launch(1);
   if (precision == B200ASR_PREC_FP32) {
     conv_repack_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (float*)ws, Ci, Co, 1);
-    return conv3x3_simt(dy, (const float*)ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, st);
+    return conv3x3_simt(dy, (const float*)ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, st, relu_bits);
   }
   if (conv_is_bf16(precision)) {
     B200_REQUIRE(Co % 32 == 0 && (Ci == 64 || Ci == 128), B200ASR_BAD_SHAPE, "conv3x3_bwd_data (bf16): needs Co %% 32 == 0 and Ci in {64,128}");
     conv_repack_k_bf16_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (uint16_t*)ws, Ci, Co, 1, precision == B200ASR_PREC_BF16X3 ? 2 : 1);
-    return conv3x3_tc_halo(dy, ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st, dx16);
+    return conv3x3_tc_halo(dy, ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st, dx16, nullptr, relu_bits);
   }
   B200_REQUIRE(!dx16, B200ASR_BAD_ARG, "conv3x3_bwd_data: the bf16 pair output exists in the bf16 modes only");
   conv_repack_k_kernel<<<ceil_div(total, 256), 256, 0, st>>>(w, (float*)ws, Ci, Co, 1, precision == B200ASR_PREC_TF32X3);
-  if (precision == B200ASR_PREC_TF32X3) return conv3x3_tc_halo(dy, ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st);
-  return conv3x3_tc(dy, (const float*)ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st);
+  if (precision == B200ASR_PREC_TF32X3)
+    return conv3x3_tc_halo(dy, ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st, nullptr, nullptr, relu_bits);
+  return conv3x3_tc(dy, (const float*)ws, nullptr, relu_out, dx, B, T, F, Co, Ci, 0, precision, st, relu_bits);
+}
+
+int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_out, float* dx, void* dx16, void* ws, int B, int T,
+                             int F, int Ci, int Co, int precision, b200asr_stream_t stream) {
+  return conv_bwd_data(dy, w, relu_out, nullptr, dx, dx16, ws, B, T, F, Ci, Co, precision, stream);
+}
+
+int b200asr_conv3x3_bwd_data_bits(const float* dy, const float* w, const uint32_t* relu_bits, float* dx, void* dx16, void* ws,
+                                  int B, int T, int F, int Ci, int Co, int precision, b200asr_stream_t stream) {
+  B200_REQUIRE(relu_bits, B200ASR_BAD_ARG, "conv3x3_bwd_data_bits: null pointer");
+  B200_REQUIRE(aligned_to(relu_bits, 4), B200ASR_BAD_ALIGN, "conv3x3_bwd_data_bits: relu_bits needs 4-byte alignment");
+  return conv_bwd_data(dy, w, nullptr, relu_bits, dx, dx16, ws, B, T, F, Ci, Co, precision, stream);
 }
 
 int b200asr_conv3x3_bwd_weight(const float* dy, const void* dy16, const float* x, float* dw, float* dbias, void* ws, int B, int T,
@@ -769,7 +876,7 @@ int b200asr_maxpool2x2_fwd(const float* x, float* y, int B, int T, int F, int C,
   B200_REQUIRE(aligned16(x) && aligned16(y), B200ASR_BAD_ALIGN, "maxpool2x2_fwd: x and y need 16-byte alignment");
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
   if (n <= 0) return B200ASR_OK;
-  maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, nullptr, B, T, F, C);
+  maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, nullptr, nullptr, B, T, F, C);
   return check_launch("maxpool2x2_fwd");
 }
 
@@ -779,24 +886,37 @@ int b200asr_maxpool2x2_fwd_idx(const float* x, float* y, unsigned char* idx, int
                "maxpool2x2_fwd_idx: x and y need 16-byte alignment, idx 4-byte");
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
   if (n <= 0) return B200ASR_OK;
-  maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, idx, B, T, F, C);
+  maxpool2x2_fwd_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, idx, nullptr, B, T, F, C);
   return check_launch("maxpool2x2_fwd_idx");
 }
 
-int b200asr_maxpool2x2_bwd_idx(const float* dy, const unsigned char* idx, float* dx, void* dx16, int B, int T, int F, int C,
-                               int relu_mask, b200asr_stream_t stream) {
-  B200_REQUIRE(dy && idx && dx && C % 4 == 0, B200ASR_BAD_ARG, "maxpool2x2_bwd_idx: bad arguments");
+static int maxpool_bwd_codes(const char* who, bool nibbles, const float* dy, const uint8_t* idx, float* dx, void* dx16, int B, int T,
+                             int F, int C, int relu_mask, b200asr_stream_t stream) {
+  B200_REQUIRE(dy && idx && dx && C % (nibbles ? 8 : 4) == 0, B200ASR_BAD_ARG, "%s: bad arguments", who);
   B200_REQUIRE(aligned16(dy) && aligned16(dx) && aligned_to(idx, 4) && aligned_to(dx16, 8), B200ASR_BAD_ALIGN,
-               "maxpool2x2_bwd_idx: dy and dx need 16-byte alignment, idx 4-byte, dx16 8-byte");
+               "%s: dy and dx need 16-byte alignment, the codes 4-byte, dx16 8-byte", who);
   cudaStream_t st = (cudaStream_t)stream;
   long long n = (long long)B * (T / 2) * (F / 2) * (C / 4);
-  if (n > 0) maxpool2x2_bwd_idx_kernel<<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(dy, idx, dx, (uint16_t*)dx16, B, T, F, C, relu_mask);
+  if (n > 0 && nibbles)
+    maxpool2x2_bwd_idx_kernel<true><<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(dy, idx, dx, (uint16_t*)dx16, B, T, F, C, relu_mask);
+  if (n > 0 && !nibbles)
+    maxpool2x2_bwd_idx_kernel<false><<<(unsigned)ceil_div_ll(n, 256), 256, 0, st>>>(dy, idx, dx, (uint16_t*)dx16, B, T, F, C, relu_mask);
   if ((T & 1) || (F & 1)) {
     long long tot = ((F & 1) ? (long long)B * (T / 2) * 2 * (C / 4) : 0) + ((T & 1) ? (long long)B * F * (C / 4) : 0);
     maxpool2x2_bwd_tail_kernel<<<(unsigned)ceil_div_ll(tot, 256), 256, 0, st>>>(dx, (uint16_t*)dx16, B, T, F, C);
     note_launch(1);
   }
-  return check_launch("maxpool2x2_bwd_idx");
+  return check_launch(who);
+}
+
+int b200asr_maxpool2x2_bwd_idx(const float* dy, const unsigned char* idx, float* dx, void* dx16, int B, int T, int F, int C,
+                               int relu_mask, b200asr_stream_t stream) {
+  return maxpool_bwd_codes("maxpool2x2_bwd_idx", false, dy, idx, dx, dx16, B, T, F, C, relu_mask, stream);
+}
+
+int b200asr_maxpool2x2_bwd_codes(const float* dy, const uint32_t* codes, float* dx, void* dx16, int B, int T, int F, int C,
+                                 int relu_mask, b200asr_stream_t stream) {
+  return maxpool_bwd_codes("maxpool2x2_bwd_codes", true, dy, (const uint8_t*)codes, dx, dx16, B, T, F, C, relu_mask, stream);
 }
 
 int b200asr_maxpool2x2_bwd(const float* dy, const float* x, float* dx, void* dx16, int B, int T, int F, int C, int relu_mask,

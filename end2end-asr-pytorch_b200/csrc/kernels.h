@@ -33,13 +33,18 @@ int bgemm_tc(const BOperand& A, bool a_kmaj, const BOperand& B, bool b_kmaj, flo
 // Tensor-core implicit-GEMM convolution (tc_conv.cu); takes K-major repacked weights wk[9][Cout][Cin]
 // (conv_repack_k_kernel); the weight-gradient variant takes/produces dwr[9][Ci][Co].  conv3x3_tc is the TF32 forward /
 // data gradient (precision 1 only).
+// mask_bits / out_bits (optional, here and in conv3x3_tc_halo): the ReLU decisions as packed bits [pixels][Cout / 32],
+// bit c % 32 of word c / 32 = (value > 0) -- mask_bits replaces `mask` (relu_out > 0), out_bits receives (out > 0)
 int conv3x3_tc(const float* in, const float* wr, const float* bias, const float* mask, float* out, int B, int T, int F,
-               int Cin, int Cout, int relu, int precision, cudaStream_t st);
+               int Cin, int Cout, int relu, int precision, cudaStream_t st, const uint32_t* mask_bits = nullptr,
+               uint32_t* out_bits = nullptr);
 // Forward / data gradient of the 3xTF32 and bf16 modes, with the input patch (incl. halo) fetched once per 32-channel slice
 // (tc_conv_halo.cu).  mode 3 = 3xTF32 (fp32 hi | lo weights), 6 = bf16x3 / 2 = bf16 (bf16 weights from conv_repack_k_bf16)
 int conv3x3_tc_halo(const float* in, const void* wk, const float* bias, const float* mask, float* out, int B, int T, int F,
-                    int Cin, int Cout, int relu, int mode, cudaStream_t st, void* out16 = nullptr, float* pool = nullptr);
-// out16: optional bf16 hi | lo pairs [2][B,T,F,Cout] of the output, written by the epilogue next to `out`
+                    int Cin, int Cout, int relu, int mode, cudaStream_t st, void* out16 = nullptr, float* pool = nullptr,
+                    const uint32_t* mask_bits = nullptr, uint32_t* out_bits = nullptr, uint8_t* pool_codes = nullptr);
+// out16: optional bf16 hi | lo pairs [2][B,T,F,Cout] of the output, written by the epilogue next to `out`; out may be nullptr
+// when `pool` is given.  pool_codes: the pooling decisions [B,T/2,F/2,Cout/8] words as b200asr_conv3x3_fwd_pool_codes documents
 int conv3x3_wgrad_tc(const float* x, const float* dy, float* dwr, int B, int T, int F, int Ci, int Co, int precision,
                      cudaStream_t st, float* dbias = nullptr, int* dbias_done = nullptr, const void* dy16 = nullptr);
 // dy16 (bf16 modes only): dy as bf16 hi | lo pairs [2][B,T,F,Co] written by its producer -> B tiles arrive by TMA

@@ -37,6 +37,8 @@ struct ConvEpi {
   float* out;
   const float* bias;
   const float* mask;
+  const uint32_t* mask_bits;   // see conv3x3_tc in kernels.h
+  uint32_t* out_bits;
   int relu, B, T, F, Cin, Cout;
 };
 
@@ -84,6 +86,10 @@ struct ConvPolicy {
     const size_t pix = ((size_t)t.b * e.T + tt) * e.F + ff;
     float* orow = e.out + pix * e.Cout;
     const float* mrow = e.mask ? e.mask + pix * e.Cout : nullptr;
+    // c0 is a multiple of 32: the piece is exactly one word of the ReLU bits
+    const size_t word = pix * (e.Cout >> 5) + (c0 >> 5);
+    const uint32_t mbits = e.mask_bits ? __ldg(e.mask_bits + word) : ~0u;
+    uint32_t obits = 0u;
     // all loads of a 16-channel half before its first store (see GemmPolicy::store)
 #pragma unroll
     for (int half = 0; half < 2; half++) {
@@ -101,9 +107,18 @@ struct ConvPolicy {
         if (e.relu) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); o[2] = fmaxf(o[2], 0.f); o[3] = fmaxf(o[3], 0.f); }
         o[0] = mm[q].x > 0.f ? o[0] : 0.f; o[1] = mm[q].y > 0.f ? o[1] : 0.f;
         o[2] = mm[q].z > 0.f ? o[2] : 0.f; o[3] = mm[q].w > 0.f ? o[3] : 0.f;
+        if (e.mask_bits) {
+#pragma unroll
+          for (int k = 0; k < 4; k++) o[k] = (mbits >> (j + k)) & 1u ? o[k] : 0.f;
+        }
+        if (e.out_bits) {
+#pragma unroll
+          for (int k = 0; k < 4; k++) obits |= o[k] > 0.f ? 1u << (j + k) : 0u;
+        }
         *reinterpret_cast<float4*>(orow + col) = make_float4(o[0], o[1], o[2], o[3]);
       }
     }
+    if (e.out_bits) e.out_bits[word] = obits;
   }
 };
 
@@ -220,9 +235,10 @@ static int launch_wgrad(const CUtensorMap& mx, const CUtensorMap& mdy, const WgP
 
 // wk: [9][Cout][Cin] K-major weights (conv_repack_k_kernel).
 int conv3x3_tc(const float* in, const float* wk, const float* bias, const float* mask, float* out, int B, int T, int F,
-               int Cin, int Cout, int relu, int precision, cudaStream_t st) {
+               int Cin, int Cout, int relu, int precision, cudaStream_t st, const uint32_t* mask_bits, uint32_t* out_bits) {
   using namespace tc;
   B200_REQUIRE(precision == 1, B200ASR_BAD_ARG, "conv3x3_tc: precision must be 1");
+  B200_REQUIRE(!(mask && mask_bits), B200ASR_BAD_ARG, "conv3x3_tc: pass the ReLU mask as floats or as bits, not both");
   B200_REQUIRE(Cin % 32 == 0 && (Cout == 64 || Cout == 128), B200ASR_BAD_SHAPE,
                "conv3x3_tc: needs Cin %% 32 == 0 and Cout in {64,128} (Cin=%d Cout=%d)", Cin, Cout);
   B200_REQUIRE(aligned16(in) && aligned16(wk) && aligned16(out) && (!bias || aligned16(bias)) && (!mask || aligned16(mask)),
@@ -242,7 +258,7 @@ int conv3x3_tc(const float* in, const float* wk, const float* bias, const float*
     int rc = make_tensor_map_f32(&mb, wk, 2, dims, strides, box, true);
     if (rc) return rc;
   }
-  ConvEpi e{out, bias, mask, relu, B, T, F, Cin, Cout};
+  ConvEpi e{out, bias, mask, mask_bits, out_bits, relu, B, T, F, Cin, Cout};
   return Cout == 64 ? launch_conv_persistent<64>(ma, mb, e, st) : launch_conv_persistent<128>(ma, mb, e, st);
 }
 

@@ -38,9 +38,14 @@ constexpr int HALO_ORDER_BAR = 2;                      // named barriers 2 / 3: 
 struct HaloP {
   uint16_t* out16;       // optional bf16 hi | lo pairs of the output, [2][pixels][Cout] (lo at + npix * Cout), or nullptr
   float* pool;           // optional MaxPool2d(2, 2) of the output, [B, T/2, F/2, Cout] (floor mode), or nullptr
-  float* out;
+  // optional pooling decisions next to `pool`: a nibble per pooled element, window index in ATen's scan order | 4 when the
+  // maximum is not positive; byte (element / 2), low nibble = even channel, or nullptr
+  uint8_t* pool_codes;
+  float* out;            // the convolution's output, or nullptr (only the pooled output and its codes are wanted)
   const float* bias;
   const float* mask;
+  const uint32_t* mask_bits;   // optional ReLU decisions instead of `mask`: [pixels][Cout / 32] words, bit c % 32 = (relu_out > 0)
+  uint32_t* out_bits;          // optional bits of (out > 0) in the same layout, or nullptr
   int relu, B, T, F, Cin, Cout, nft, ntt, cch;
 };
 
@@ -330,10 +335,12 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
     // ---- epilogue straight from the accumulator layout: bias, ReLU, mask, optional bf16 pairs and fused 2 x 2 max-pool.
     // In row block mb this thread holds time steps tt / tt + 1 (rows r0 / r0 + 8) of freq bin ff, columns 8 j + 2 q, + 1;
     // bin ff + 1 is in lane + 4, so a 2 x 2 window is one register pair here and one in lane ^ 4 (the even-g lane stores).
+    // A 32-channel word of the ReLU bits is j = 4 w .. 4 w + 3 of the four lanes of a quad (q = 0..3): bit 8 (j % 4) + 2 q, + 1.
     int f0, t0, b;
     decode(tile, f0, t0, b);
     const int ff = f0 + g;
     const size_t lo_off = (size_t)p.B * p.T * p.F * p.Cout;
+    const int wpp = p.Cout >> 5;                         // bit words per pixel
 #pragma unroll
     for (int mb = 0; mb < 2; mb++) {
       const int tt = t0 + mb * 8 + cw * 2;
@@ -341,10 +348,15 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
       const size_t pix = ((size_t)b * p.T + tt) * p.F + ff;
       const bool pool_st = p.pool && (g & 1) == 0 && tt + 1 < p.T && ff + 1 < p.F;
       float* prow_out = pool_st ? p.pool + (((size_t)b * (p.T >> 1) + (tt >> 1)) * (p.F >> 1) + (ff >> 1)) * p.Cout : nullptr;
+      uint32_t mw[2] = {0u, 0u}, ob[2] = {0u, 0u};     // mask word in use / output bits gathered, per time row
 #pragma unroll
       for (int j = 0; j < BN / 8; j++) {
-        const int col = j * 8 + 2 * q;
+        const int col = j * 8 + 2 * q, sh = col & 31;
         const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+        if (p.mask_bits && (j & 3) == 0) {
+#pragma unroll
+          for (int h = 0; h < 2; h++) mw[h] = valid[h] ? __ldg(p.mask_bits + (pix + (size_t)h * p.F) * wpp + (j >> 2)) : 0u;
+        }
         float2 o[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
@@ -354,7 +366,12 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
           if (p.relu) { o[h].x = fmaxf(o[h].x, 0.f); o[h].y = fmaxf(o[h].y, 0.f); }
           o[h].x = mm.x > 0.f ? o[h].x : 0.f;
           o[h].y = mm.y > 0.f ? o[h].y : 0.f;
-          if (valid[h]) *reinterpret_cast<float2*>(p.out + off) = o[h];
+          if (p.mask_bits) {
+            o[h].x = (mw[h] >> sh) & 1u ? o[h].x : 0.f;
+            o[h].y = (mw[h] >> (sh + 1)) & 1u ? o[h].y : 0.f;
+          }
+          if (p.out_bits) ob[h] |= (o[h].x > 0.f ? 1u << sh : 0u) | (o[h].y > 0.f ? 2u << sh : 0u);
+          if (p.out && valid[h]) *reinterpret_cast<float2*>(p.out + off) = o[h];
           if (p.out16 && valid[h]) {   // the same values as bf16 pairs: the weight-gradient kernel's B operand (WgradPairPolicy)
             uint32_t hi, lo;
             split_bf16_pair(o[h].x, o[h].y, hi, lo);
@@ -363,10 +380,29 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_co
           }
         }
         if (p.pool) {                  // every lane takes part in the shuffles
-          float mx = fmaxf(o[0].x, o[1].x), my = fmaxf(o[0].y, o[1].y);
-          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 4));
-          my = fmaxf(my, __shfl_xor_sync(0xffffffffu, my, 4));
+          const float lx = fmaxf(o[0].x, o[1].x), ly = fmaxf(o[0].y, o[1].y);
+          const float rx = __shfl_xor_sync(0xffffffffu, lx, 4), ry = __shfl_xor_sync(0xffffffffu, ly, 4);
+          const float mx = fmaxf(lx, rx), my = fmaxf(ly, ry);
           if (pool_st) *reinterpret_cast<float2*>(prow_out + col) = make_float2(mx, my);
+          if (p.pool_codes) {
+            // window positions in ATen's scan order: this lane's (ff, tt) / (ff, tt + 1) = 0 / 1, lane ^ 4's bin ff + 1 = 2 / 3.
+            // The first maximum of each pair, then the later pair only if strictly larger: the same position as the
+            // sequential scan of maxpool2x2_bwd for every non-NaN window (post-ReLU values are never NaN)
+            const uint32_t sel = (o[1].x > o[0].x ? 1u : 0u) | (o[1].y > o[0].y ? 2u : 0u);
+            const uint32_t rsel = __shfl_xor_sync(0xffffffffu, sel, 4);
+            const uint32_t cx = (rx > lx ? 2u | (rsel & 1u) : (sel & 1u)) | (mx > 0.f ? 0u : 4u);
+            const uint32_t cy = (ry > ly ? 2u | (rsel >> 1) : (sel >> 1)) | (my > 0.f ? 0u : 4u);
+            if (pool_st) p.pool_codes[(prow_out - p.pool + col) >> 1] = (uint8_t)(cx | (cy << 4));
+          }
+        }
+        if (p.out_bits && (j & 3) == 3) {   // the quad's word is complete: OR it over the quad, lane q = h stores row h
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            ob[h] |= __shfl_xor_sync(0xffffffffu, ob[h], 1);
+            ob[h] |= __shfl_xor_sync(0xffffffffu, ob[h], 2);
+            if (q == h && valid[h]) p.out_bits[(pix + (size_t)h * p.F) * wpp + (j >> 2)] = ob[h];
+            ob[h] = 0u;
+          }
         }
       }
     }
@@ -393,13 +429,16 @@ static int launch_halo(const CUtensorMap& ma, const CUtensorMap& mb, const HaloP
 // wk: mode 3: [2][9][Cout][Cin] fp32 pre-split K-major weights (hi | lo), as for conv3x3_tc with precision 3;
 //     mode 6 / 2: [2 or 1][9][Cout][Cin] bf16 (conv_repack_k_bf16_kernel)
 int conv3x3_tc_halo(const float* in, const void* wk, const float* bias, const float* mask, float* out, int B, int T, int F,
-                    int Cin, int Cout, int relu, int mode, cudaStream_t st, void* out16, float* pool) {
+                    int Cin, int Cout, int relu, int mode, cudaStream_t st, void* out16, float* pool,
+                    const uint32_t* mask_bits, uint32_t* out_bits, uint8_t* pool_codes) {
   using namespace tc;
   B200_REQUIRE(mode == 3 || mode == 6 || mode == 2, B200ASR_BAD_ARG, "conv3x3_tc_halo: mode must be 3 (3xTF32), 6 (bf16x3) or 2 (bf16)");
   B200_REQUIRE(Cin % 32 == 0 && (Cout == 64 || Cout == 128), B200ASR_BAD_SHAPE,
                "conv3x3_tc_halo: needs Cin %% 32 == 0 and Cout in {64,128} (Cin=%d Cout=%d)", Cin, Cout);
+  B200_REQUIRE((out || pool) && (!pool_codes || pool), B200ASR_BAD_ARG, "conv3x3_tc_halo: nothing to write");
   B200_REQUIRE(aligned16(in) && aligned16(wk) && aligned16(out) && (!bias || aligned16(bias)) && (!mask || aligned16(mask)),
                B200ASR_BAD_ALIGN, "conv3x3_tc_halo: pointers must be 16-byte aligned");
+  B200_REQUIRE(!(mask && mask_bits), B200ASR_BAD_ARG, "conv3x3_tc_halo: pass the ReLU mask as floats or as bits, not both");
   CUtensorMap ma, mb;
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)F, (uint64_t)T, (uint64_t)B};
@@ -415,7 +454,7 @@ int conv3x3_tc_halo(const float* in, const void* wk, const float* bias, const fl
     int rc = mode == 3 ? make_tensor_map_f32(&mb, wk, 2, dims, strides, box, false) : make_tensor_map_bf16(&mb, wk, 2, dims, strides, box);
     if (rc) return rc;
   }
-  HaloP p{(uint16_t*)out16, pool, out, bias, mask, relu, B, T, F, Cin, Cout, ceil_div(F, HF), ceil_div(T, HT), Cin / 32};
+  HaloP p{(uint16_t*)out16, pool, pool_codes, out, bias, mask, mask_bits, out_bits, relu, B, T, F, Cin, Cout, ceil_div(F, HF), ceil_div(T, HT), Cin / 32};
   if (mode == 3) return Cout == 64 ? launch_halo<64, 3>(ma, mb, p, st) : launch_halo<128, 3>(ma, mb, p, st);
   if (mode == 6) return Cout == 64 ? launch_halo<64, 6>(ma, mb, p, st) : launch_halo<128, 6>(ma, mb, p, st);
   return Cout == 64 ? launch_halo<64, 2>(ma, mb, p, st) : launch_halo<128, 2>(ma, mb, p, st);

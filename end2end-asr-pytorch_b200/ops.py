@@ -776,24 +776,36 @@ class VggFrontendFn(torch.autograd.Function):
         C1, C2 = w0.shape[0], w5.shape[0]
         new = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)
         ws = new(lib.b200asr_conv3x3_ws_bytes(C2, C2) // 4)
+        # the ReLU decisions of y1 and y3 also as packed bits [B,T,F,C/32], and the pooling decisions of y2 and y4 as packed
+        # codes [B,T/2,F/2,C/8] (1/32 of the bytes each): the backward takes its masks and routes from these instead of reading
+        # fp32 activations back.  In the bf16 modes y2 / y4 are not written at all (the pooling is the convolution's epilogue);
+        # the other precisions pool in a kernel of their own, which reads them, and drop them after the forward.
+        bits = lambda *s: torch.empty(s[:-1] + (s[-1] // 32,), device=dev, dtype=torch.int32)
+        codes = lambda *s: torch.empty(s[:-1] + (s[-1] // 8,), device=dev, dtype=torch.int32)
+        keep_y = decision_capture is not None or prec not in _BF16_PRECS
         y1 = new(B, T, F, C1)
-        L.check(lib.b200asr_conv3x3_c1_fwd(L.ptr(x), L.ptr(_f32c(w0)), L.ptr(b0), L.ptr(y1), B, F, T, C1, 1, st), "conv1")
-        y2 = new(B, T, F, C1)
+        y1b = bits(B, T, F, C1)
+        L.check(lib.b200asr_conv3x3_c1_fwd_bits(L.ptr(x), L.ptr(_f32c(w0)), L.ptr(b0), L.ptr(y1), B, F, T, C1, 1, L.ptr(y1b), st),
+                "conv1")
+        y2 = new(B, T, F, C1) if keep_y else None
         T2, F2 = T // 2, F // 2
         p1 = new(B, T2, F2, C1)
+        c1 = codes(B, T2, F2, C1)
         # (pool_idx = None: asking for the arg-max bytes of b200asr_maxpool2x2_bwd_idx runs the stand-alone pooling kernel)
         # conv + ReLU + MaxPool2d(2, 2): in the bf16 modes the pooling is the convolution's epilogue
-        L.check(lib.b200asr_conv3x3_fwd_pool(L.ptr(y1), L.ptr(_f32c(w2)), L.ptr(b2), L.ptr(y2), L.ptr(p1), None, L.ptr(ws), B, T, F, C1, C1, 1,
-                                             prec, st), "conv2+pool1")
+        L.check(lib.b200asr_conv3x3_fwd_pool_codes(L.ptr(y1), L.ptr(_f32c(w2)), L.ptr(b2), L.ptr(y2), L.ptr(p1), L.ptr(c1), L.ptr(ws),
+                                                   B, T, F, C1, C1, 1, prec, st), "conv2+pool1")
         y3 = new(B, T2, F2, C2)
-        L.check(lib.b200asr_conv3x3_fwd(L.ptr(p1), L.ptr(_f32c(w5)), L.ptr(b5), L.ptr(y3), L.ptr(ws), B, T2, F2, C1, C2, 1,
-                                        prec, st), "conv3")
-        y4 = new(B, T2, F2, C2)
+        y3b = bits(B, T2, F2, C2)
+        L.check(lib.b200asr_conv3x3_fwd_bits(L.ptr(p1), L.ptr(_f32c(w5)), L.ptr(b5), L.ptr(y3), L.ptr(ws), B, T2, F2, C1, C2, 1,
+                                             prec, L.ptr(y3b), st), "conv3")
+        y4 = new(B, T2, F2, C2) if keep_y else None
         T4, F4 = T2 // 2, F2 // 2
         p2 = new(B, T4, F4, C2)
-        L.check(lib.b200asr_conv3x3_fwd_pool(L.ptr(y3), L.ptr(_f32c(w7)), L.ptr(b7), L.ptr(y4), L.ptr(p2), None, L.ptr(ws), B, T2, F2, C2, C2, 1,
-                                             prec, st), "conv4+pool2")
-        ctx.save_for_backward(x, y1, y2, p1, y3, y4, w0, w2, w5, w7)
+        c2 = codes(B, T4, F4, C2)
+        L.check(lib.b200asr_conv3x3_fwd_pool_codes(L.ptr(y3), L.ptr(_f32c(w7)), L.ptr(b7), L.ptr(y4), L.ptr(p2), L.ptr(c2), L.ptr(ws),
+                                                   B, T2, F2, C2, C2, 1, prec, st), "conv4+pool2")
+        ctx.save_for_backward(x, y1, p1, y3, y1b, y3b, c1, c2, w0, w2, w5, w7)
         if decision_capture is not None:      # channels-last [B,T,F,C] -> the reference's (B,C,F,T)
             nchw = lambda t: t.permute(0, 3, 2, 1)
             decision_capture.extend([("relu", nchw(y1)), ("relu", nchw(y2)), ("pool", nchw(y2)), ("relu", nchw(y3)), ("relu", nchw(y4)),
@@ -805,7 +817,7 @@ class VggFrontendFn(torch.autograd.Function):
     def backward(ctx, dp2):
         if frontend_backward_hook is not None:
             frontend_backward_hook()
-        x, y1, y2, p1, y3, y4, w0, w2, w5, w7 = ctx.saved_tensors
+        x, y1, p1, y3, y1b, y3b, c1, c2, w0, w2, w5, w7 = ctx.saved_tensors
         lib, st, prec, prec_w = _lib(), _stream(), ctx.prec, ctx.prec_w
         B, _, F, T = x.shape
         C1, C2 = w0.shape[0], w5.shape[0]
@@ -819,13 +831,13 @@ class VggFrontendFn(torch.autograd.Function):
         pairs = prec_w in _BF16_PRECS and prec in _BF16_PRECS
         new16 = lambda *s_: torch.empty((2,) + s_, device=dev, dtype=torch.bfloat16) if pairs else None
         d4, d4p = new(B, T2, F2, C2), new16(B, T2, F2, C2)
-        L.check(lib.b200asr_maxpool2x2_bwd(L.ptr(dp2), L.ptr(y4), L.ptr(d4), L.ptr(d4p), B, T2, F2, C2, 1, st), "pool2_bwd")
+        L.check(lib.b200asr_maxpool2x2_bwd_codes(L.ptr(dp2), L.ptr(c2), L.ptr(d4), L.ptr(d4p), B, T2, F2, C2, 1, st), "pool2_bwd")
         dw7, db7 = torch.empty_like(w7), new(C2)
         L.check(lib.b200asr_conv3x3_bwd_weight(L.ptr(d4), L.ptr(d4p), L.ptr(y3), L.ptr(dw7), L.ptr(db7), L.ptr(ws), B, T2, F2, C2, C2,
                                                prec_w, st), "conv4_wgrad")
         d3, d3p = new(B, T2, F2, C2), new16(B, T2, F2, C2)
-        L.check(lib.b200asr_conv3x3_bwd_data(L.ptr(d4), L.ptr(_f32c(w7)), L.ptr(y3), L.ptr(d3), L.ptr(d3p), L.ptr(ws), B, T2, F2, C2, C2,
-                                             prec, st), "conv4_dgrad")
+        L.check(lib.b200asr_conv3x3_bwd_data_bits(L.ptr(d4), L.ptr(_f32c(w7)), L.ptr(y3b), L.ptr(d3), L.ptr(d3p), L.ptr(ws), B, T2, F2,
+                                                  C2, C2, prec, st), "conv4_dgrad")
         del d4, d4p
         dw5, db5 = torch.empty_like(w5), new(C2)
         L.check(lib.b200asr_conv3x3_bwd_weight(L.ptr(d3), L.ptr(d3p), L.ptr(p1), L.ptr(dw5), L.ptr(db5), L.ptr(ws), B, T2, F2, C1, C2,
@@ -835,13 +847,13 @@ class VggFrontendFn(torch.autograd.Function):
                                              prec, st), "conv3_dgrad")
         del d3, d3p
         d2, d2p = new(B, T, F, C1), new16(B, T, F, C1)
-        L.check(lib.b200asr_maxpool2x2_bwd(L.ptr(dp1), L.ptr(y2), L.ptr(d2), L.ptr(d2p), B, T, F, C1, 1, st), "pool1_bwd")
+        L.check(lib.b200asr_maxpool2x2_bwd_codes(L.ptr(dp1), L.ptr(c1), L.ptr(d2), L.ptr(d2p), B, T, F, C1, 1, st), "pool1_bwd")
         dw2, db2 = torch.empty_like(w2), new(C1)
         L.check(lib.b200asr_conv3x3_bwd_weight(L.ptr(d2), L.ptr(d2p), L.ptr(y1), L.ptr(dw2), L.ptr(db2), L.ptr(ws), B, T, F, C1, C1,
                                                prec_w, st), "conv2_wgrad")
         d1 = new(B, T, F, C1)
-        L.check(lib.b200asr_conv3x3_bwd_data(L.ptr(d2), L.ptr(_f32c(w2)), L.ptr(y1), L.ptr(d1), None, L.ptr(ws), B, T, F, C1, C1,
-                                             prec, st), "conv2_dgrad")
+        L.check(lib.b200asr_conv3x3_bwd_data_bits(L.ptr(d2), L.ptr(_f32c(w2)), L.ptr(y1b), L.ptr(d1), None, L.ptr(ws), B, T, F, C1, C1,
+                                                  prec, st), "conv2_dgrad")
         del d2, d2p
         dw0, db0 = torch.empty_like(w0), new(C1)
         L.check(lib.b200asr_conv3x3_c1_bwd_weight(L.ptr(x), L.ptr(d1), L.ptr(dw0), L.ptr(db0), B, F, T, C1, st), "conv1_wgrad")

@@ -239,6 +239,20 @@ int b200asr_conv3x3_fwd_pool(const float* x, const float* w, const float* bias, 
  * Precision 0: dy, relu_out, dx and ws 16-byte aligned. */
 int b200asr_conv3x3_bwd_data(const float* dy, const float* w, const float* relu_out, float* dx, void* dx16, void* ws,
                              int B, int T, int F, int Ci, int Co, int precision, b200asr_stream_t stream);
+/* ReLU decisions as packed bits (models/asr/transformer.py:44-52: the ReLUs after conv1 and conv3, whose outputs the backward
+ * needs only as "> 0" to mask the data gradient of the next convolution): uint32 [B,T,F,C/32], bit c % 32 of word c / 32 =
+ * (y > 0) for channel c -- exactly the test the data gradient applies to relu_out (-0.0 and NaN give 0).  1/32 of the bytes of
+ * the fp32 activation.  Pointers to bits need 4-byte alignment; otherwise B200ASR_BAD_ALIGN.
+ * b200asr_conv3x3_c1_fwd / b200asr_conv3x3_fwd that additionally write y_bits (required; Co % 32 == 0): the epilogue gathers
+ * them at every precision but 0, where one more kernel packs them from y. */
+int b200asr_conv3x3_c1_fwd_bits(const float* x, const float* w, const float* bias, float* y, int B, int F, int T, int Co,
+                                int relu, uint32_t* y_bits, b200asr_stream_t stream);
+int b200asr_conv3x3_fwd_bits(const float* x, const float* w, const float* bias, float* y, void* ws, int B, int T, int F, int Ci,
+                             int Co, int relu, int precision, uint32_t* y_bits, b200asr_stream_t stream);
+/* b200asr_conv3x3_bwd_data with the mask given as relu_bits [B,T,F,Ci/32] (required) instead of relu_out: the same bits of dx
+ * and dx16 at every precision, reading 1 bit instead of 4 bytes per element. */
+int b200asr_conv3x3_bwd_data_bits(const float* dy, const float* w, const uint32_t* relu_bits, float* dx, void* dx16, void* ws,
+                                  int B, int T, int F, int Ci, int Co, int precision, b200asr_stream_t stream);
 /* dw[Co,Ci,3,3], dbias[Co] overwritten.  dy16 (optional, precisions 6 / 2): dy as bf16 pairs [2][B,T,F,Co] written by its
  * producer (b200asr_maxpool2x2_bwd / b200asr_conv3x3_bwd_data): the kernel then takes its B tiles straight from there by TMA
  * instead of converting the fp32 dy tile (the in-kernel conversion is what bounds the bf16 weight gradient).
@@ -260,6 +274,19 @@ int b200asr_maxpool2x2_bwd(const float* dy, const float* x, float* dx, void* dx1
  * element): identical result.  relu_mask != 0: a window whose maximum is not positive passes no gradient. */
 int b200asr_maxpool2x2_bwd_idx(const float* dy, const unsigned char* idx, float* dx, void* dx16, int B, int T, int F, int C,
                                int relu_mask, b200asr_stream_t stream);
+/* Pooling decisions as packed codes (models/asr/transformer.py:44-52, the two MaxPool2d(2, 2) after a ReLU, whose input the
+ * backward needs only to route the gradient): uint32 [B,T/2,F/2,C/8], nibble c % 8 of word c / 8 = the window position of the
+ * first maximum in ATen's scan order (0..3, as the index bytes) | 4 when that maximum is not positive.  1/32 of the bytes of the
+ * fp32 pool input.  Needs C % 8 == 0 and pool_codes 4-byte aligned.
+ * b200asr_conv3x3_fwd_pool that writes pool_codes (required) next to pooled.  In the bf16 modes the codes come from the
+ * convolution's epilogue, and y may be NULL: the full-resolution output is then not written at all.  Other precisions run the
+ * stand-alone pooling kernel on y, which must be given. */
+int b200asr_conv3x3_fwd_pool_codes(const float* x, const float* w, const float* bias, float* y, float* pooled, uint32_t* pool_codes,
+                                   void* ws, int B, int T, int F, int Ci, int Co, int relu, int precision, b200asr_stream_t stream);
+/* b200asr_maxpool2x2_bwd from those codes instead of the activation: with relu_mask != 0 the same dx and dx16 bits as
+ * b200asr_maxpool2x2_bwd(dy, x, ..., relu_mask = 1) for the pool input x the codes were taken from. */
+int b200asr_maxpool2x2_bwd_codes(const float* dy, const uint32_t* codes, float* dx, void* dx16, int B, int T, int F, int C,
+                                 int relu_mask, b200asr_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * emb_cnn front end (models/asr/transformer.py:33-40): generic strided NCHW convolution, BatchNorm2d
