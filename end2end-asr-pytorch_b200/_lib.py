@@ -116,7 +116,12 @@ SIGNATURES = {
     "b200asr_adam_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _i, _f, _vp, _vp]),
     "b200asr_sumsq": (_i, [_vp, _ll, _vp, _vp]),
     "b200asr_grad_scale": (_i, [_vp, _ll, _vp, _f, _vp, _vp, _vp]),
-    "b200asr_permute_cols_cf": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "b200asr_optim_table_capacity": (_i, []),
+    "b200asr_adam_multi": (_i, [_vp, _vp, _vp, _vp, _i, _f, _f, _f, _f, _vp]),
+    "b200asr_norm_multi": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "b200asr_clip_coef": (_i, [_vp, _i, _f, _vp, _vp]),
+    "b200asr_scale_multi": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "b200asr_permute_cols_cf":(_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "b200asr_edit_counts_ws_bytes": (_sz, [_i, _i, _i, _i]),
     "b200asr_edit_counts": (_i, [_vp, _i, _ll, _i, _vp, _i, _ll, _i, _i] + [_vp] * 5 + [_i, _i, _ll, _vp, _vp, _vp, _vp]),
 }

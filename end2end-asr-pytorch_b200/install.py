@@ -6,9 +6,10 @@ After this, the reference's own `Transformer` (models/asr/transformer.py), `Trai
 (trainer/asr/trainer.py), `test.py` and the LSTM LM's `RNNModel.forward` (utils/lstm_utils.py) run on libb200asr kernels:
 module tree, parameter names and checkpoints are untouched; only `forward` attributes, `Decoder.beam_search`,
 `Decoder.greedy_search`, `Transformer.evaluate`, the two loss functions and, when trainer/asr/trainer.py is imported,
-`Trainer.train` (trainer.trainer_train: the CER / WER counts on the device) are rebound (SURVEY.md §8b).  The replaced methods
+`Trainer.train` (trainer.trainer_train: the CER / WER counts and the gradient clip on the device) and `NoamOpt.step`
+(optim.noam_step: torch.optim.Adam's step on the device, in the optimizer's own state) are rebound (SURVEY.md §8b).  The replaced methods
 stay reachable through original(): LM rescoring with an LM other than an LSTM LM still runs the reference's beam_search, a
-GRU / RNN LM its own RNNModel.forward, greedy_search with lm_rescoring=True or in training mode and evaluate in training
+GRU / RNN LM its own RNNModel.forward, an optimizer other than a plain fp32 CUDA torch.optim.Adam its own NoamOpt.step, greedy_search with lm_rescoring=True or in training mode and evaluate in training
 mode the reference's own methods.
 """
 from __future__ import annotations
@@ -16,7 +17,7 @@ from __future__ import annotations
 import importlib
 import sys
 
-from . import metrics, modules, trainer
+from . import metrics, modules, optim, trainer
 
 _PATCHED = {}
 
@@ -51,6 +52,12 @@ def install(reference_root: str = None):
         lu = None
     if lu is not None:
         targets.append((lu.RNNModel, "forward", modules.rnn_model_forward))
+    try:                                                # NoamOpt.step: Adam on the device (optim.noam_step)
+        uo = importlib.import_module("utils.optimizer")
+    except ImportError:
+        uo = None
+    if uo is not None:
+        targets.append((uo.NoamOpt, "step", optim.noam_step))
     t_mod = sys.modules.get("trainer.asr.trainer")      # `from utils.metrics import calculate_metrics` binds by value
     if t_mod is not None:
         targets.append((t_mod, "calculate_metrics", metrics.calculate_metrics))

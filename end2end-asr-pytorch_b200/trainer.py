@@ -7,6 +7,8 @@ skips, its prints, logging lines, progress-bar texts, metrics and checkpoints, b
   * training: the row is read before the loss, because an id missing from id2label skips the batch before the loss is
     computed (:60-79); the loss is then read once, for the infinity check (:87) and for total_loss (:113);
   * validation: the loss comes first there (:145-151), so the loss and the row are read in one copy.
+With --clip, the gradients are clipped by optim.clip_grad_norm_ on the device when every gradient is an fp32 CUDA tensor on
+one device, by torch.nn.utils.clip_grad_norm_ otherwise (:108-109).
 A batch with an id missing from id2label, or whose ids are not [B, T] integer CUDA tensors, builds its strings on the host
 exactly as the reference does, which prints the same exception.
 
@@ -22,6 +24,7 @@ import sys
 import torch
 
 from .metrics import LabelTable, edit_counts
+from .optim import clip_grads
 
 
 def _device_totals(hyp_seq, gold_seq, table):
@@ -151,7 +154,7 @@ def trainer_train(self, model, train_loader, train_sampler, valid_loader_list, o
             loss.backward()
 
             if constant.args.clip:
-                torch.nn.utils.clip_grad_norm_(model.parameters(), constant.args.max_norm)
+                clip_grads(model.parameters(), constant.args.max_norm)
 
             opt.step()
 

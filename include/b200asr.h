@@ -553,6 +553,31 @@ int b200asr_sumsq(const float* g, long long n, float* out, b200asr_stream_t stre
  * token-normalised gradient; out[1] = that norm (0 without clipping).  scratch: 1 float.  No host synchronisation. */
 int b200asr_grad_scale(const float* g, long long n, const float* n_tokens, float max_norm, float* scratch, float* out,
                        b200asr_stream_t stream);
+/* ------------------------------------------------------------------------------------------------
+ * Step tail over a list of separate tensors, as torch.optim.Adam holds them: NoamOpt.step (utils/optimizer.py:15-22) around
+ * torch.optim.Adam (utils/functions.py:107) and torch.nn.utils.clip_grad_norm_ (trainer/asr/trainer.py:108-109).
+ * `tensors` and the other per-tensor arrays are HOST arrays; each entry of `tensors` is a device address.  A call takes
+ * 1 .. b200asr_optim_table_capacity() tensors (a longer list is split by the caller, one call per table); every address must
+ * be non-NULL and 4-byte aligned (BAD_ARG / BAD_ALIGN), numel >= 0 (0 = nothing to do).  The table travels in the kernel
+ * parameters: no host-to-device copy, no allocation, no host synchronisation.  Each call is one launch, except norm_multi
+ * (two). */
+int b200asr_optim_table_capacity(void);
+/* tensors [count][4]: param, grad, exp_avg, exp_avg_sq, numel[count] elements each.  Per element, torch 2.11's foreach Adam
+ * (torch/optim/adam.py, _multi_tensor_adam, non-capturable) op by op with the same fp32 roundings:
+ *   m = lerp(m, g, lerp_weight); v = v * beta2; v = v + one_minus_beta2 * (g * g);
+ *   d = sqrt(v) / bc2_sqrt[k] + eps; p = p + step_size[k] * (m / d)
+ * with step_size[k] = -lr / (1 - beta1^step) and bc2_sqrt[k] = (1 - beta2^step)^0.5 of tensor k (lerp_weight = 1 - beta1 and
+ * one_minus_beta2 = 1 - beta2 as the host rounds them).  Bit-identical to torch on the same inputs. */
+int b200asr_adam_multi(const uint64_t* tensors, const long long* numel, const float* step_size, const float* bc2_sqrt, int count,
+                       float lerp_weight, float beta2, float one_minus_beta2, float eps, b200asr_stream_t stream);
+/* norms[k] (device, [count]) = ||tensors[k]||_2 (fp32, fixed-order sums: the same bits on every call). */
+int b200asr_norm_multi(const uint64_t* tensors, const long long* numel, int count, float* norms, b200asr_stream_t stream);
+/* out[0] (device) = sqrt(sum of norms[k]^2), out[1] = min(1, max_norm / (out[0] + 1e-6)) formed as clip_grad_norm_ forms it:
+ * reciprocal(out[0] + 1e-6) * max_norm, then clamp(max=1) (NaN stays NaN).  One CTA. */
+int b200asr_clip_coef(const float* norms, int count, float max_norm, float* out, b200asr_stream_t stream);
+/* tensors[k] *= *coef (device scalar) for every element, in place. */
+int b200asr_scale_multi(const uint64_t* tensors, const long long* numel, int count, const float* coef, b200asr_stream_t stream);
+
 /* dst = src permuted: dst[r, f*C + c] = src[r, c*F + f] (input_linear column order, see VGG note);
  * inverse != 0 applies the inverse permutation. */
 int b200asr_permute_cols_cf(const float* src, float* dst, int rows, int C, int F, int inverse,
