@@ -11,20 +11,25 @@ module tree, parameter names and checkpoints are untouched; only `forward` attri
 stay reachable through original(): LM rescoring with an LM other than an LSTM LM still runs the reference's beam_search, a
 GRU / RNN LM its own RNNModel.forward, an optimizer other than a plain fp32 CUDA torch.optim.Adam its own NoamOpt.step, greedy_search with lm_rescoring=True or in training mode and evaluate in training
 mode the reference's own methods.
+
+Data-parallel training: when the environment of `python -m b200asr.launch` describes more than one rank (WORLD_SIZE > 1),
+or `process_group=` is passed, install() joins that process group and the bound Trainer.train trains across it
+(trainer.trainer_train, parallel.join).  Otherwise nothing about a single process changes.
 """
 from __future__ import annotations
 
 import importlib
 import sys
 
-from . import metrics, modules, optim, trainer
+from . import metrics, modules, optim, parallel, trainer
 
 _PATCHED = {}
 
 
-def install(reference_root: str = None):
+def install(reference_root: str = None, process_group=None):
     """Patch models.common_layers / models.asr.transformer / utils.metrics (+ trainer's imported name).
-    Returns the dict of original attributes (pass it to uninstall())."""
+    process_group: a torch.distributed group the bound Trainer.train trains across; without it the launcher's environment
+    (WORLD_SIZE > 1) is joined, if present.  Returns the dict of original attributes (pass it to uninstall())."""
     if reference_root and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
     cl = importlib.import_module("models.common_layers")
@@ -67,6 +72,7 @@ def install(reference_root: str = None):
         if key not in _PATCHED:
             _PATCHED[key] = (obj, name, getattr(obj, name))
         setattr(obj, name, new)
+    parallel.join(process_group)
     return dict(_PATCHED)
 
 
@@ -74,6 +80,7 @@ def uninstall():
     for obj, name, old in _PATCHED.values():
         setattr(obj, name, old)
     _PATCHED.clear()
+    parallel.leave()
 
 
 def original(cls, name):

@@ -8,6 +8,10 @@ gathered global batch (trainer.py:84 + metrics.py:127-130).
 """
 from __future__ import annotations
 
+import os
+import random
+
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -24,6 +28,137 @@ def shard_batch(src, lengths, tgt, rank: int, world: int):
     n = B // world
     sl = slice(rank * n, (rank + 1) * n)
     return src[sl], lengths[sl], tgt[sl]
+
+
+BACKEND_ENV = "B200ASR_DIST_BACKEND"      # set by b200asr.launch: "nccl", or "gloo" when two ranks share a GPU
+_group = None                             # (process group, rank, world size) the bound Trainer.train trains across
+
+
+def join(process_group=None):
+    """Make the bound Trainer.train data-parallel across `process_group` (a torch.distributed group, or None for the default
+    group).  Without a group: join the one the launcher's environment describes (WORLD_SIZE > 1, RANK, MASTER_ADDR,
+    MASTER_PORT, B200ASR_DIST_BACKEND), initialising torch.distributed if needed.  Returns (group, rank, world) or None when
+    there is nothing to join."""
+    global _group
+    if process_group is None:
+        if int(os.environ.get("WORLD_SIZE", "1")) <= 1:
+            return _group
+        if not dist.is_initialized():
+            dist.init_process_group(os.environ.get(BACKEND_ENV, "nccl"), init_method="env://")
+        process_group = dist.group.WORLD
+    world = dist.get_world_size(process_group)
+    _group = (process_group, dist.get_rank(process_group), world) if world > 1 else None
+    return _group
+
+
+def leave():
+    """Forget the group join() recorded (the process group itself stays as it is)."""
+    global _group
+    _group = None
+
+
+def joined():
+    """(group, rank, world) the bound Trainer.train trains across, or None."""
+    return _group
+
+
+def shard_range(B: int, rank: int, world: int):
+    """[start, stop) of rank's utterances in a batch of B: chunk `rank` of `torch.arange(B).chunk(world)`, which is how
+    nn.DataParallel.scatter splits a batch (chunks of ceil(B / world); the ranks past the last chunk get an empty range)."""
+    if world < 1 or not 0 <= rank < world:
+        raise ValueError(f"shard_range: rank {rank} of world {world}")
+    n = -(-B // world)
+    return min(B, rank * n), min(B, (rank + 1) * n)
+
+
+def broadcast_params(flat, process_group=None):
+    """Replicas start identical: rank 0's flat parameter buffer is broadcast to every rank.  nn.DataParallel re-replicates
+    from device 0 every step (utils/functions.py:154-160); once is enough here because every rank applies the same update."""
+    src = dist.get_global_rank(process_group, 0) if process_group is not None else 0
+    dist.broadcast(flat.flat, src=src, group=process_group)
+
+
+def broadcast_module_state(module, flat, process_group=None):
+    """Rank 0's copy of everything in `module` that the flat buffer does not hold -- frozen parameters and buffers
+    (BatchNorm running statistics, num_batches_tracked, the positional table) -- broadcast to every rank, so that
+    replicas built or loaded differently start identical."""
+    src = dist.get_global_rank(process_group, 0) if process_group is not None else 0
+    held = {id(p) for p in flat.params}
+    for t in [p for p in module.parameters() if id(p) not in held] + list(module.buffers()):
+        if t.data.is_contiguous():
+            dist.broadcast(t.data, src=src, group=process_group)
+        else:
+            c = t.data.contiguous()
+            dist.broadcast(c, src=src, group=process_group)
+            t.data.copy_(c)
+
+
+def seed_host_rngs(process_group=None):
+    """Seed Python's `random`, numpy's global generator and torch's CPU generator identically on every rank, from a seed
+    rank 0 draws from its own `random` and broadcasts.  The reference's data order comes from these generators:
+    BucketingSampler shuffles its bins (`shuffle(epoch)`) and the ids inside each bin with np.random, SpectrogramDataset
+    picks a manifest with random.randint, and the DataLoader draws its workers' base seed from torch's CPU generator.  With
+    the same seed every rank's loader yields the same global batches, of which each rank then trains its own chunk.
+    Returns the seed."""
+    src = dist.get_global_rank(process_group, 0) if process_group is not None else 0
+    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(process_group) == "nccl" else torch.device("cpu")
+    seed = torch.tensor([random.getrandbits(62)], dtype=torch.int64, device=dev)
+    dist.broadcast(seed, src=src, group=process_group)
+    s = int(seed.item())
+    random.seed(s)
+    np.random.seed(s % 2 ** 32)
+    torch.manual_seed(s)
+    return s
+
+
+def fold_rank_into_dropout(rank: int):
+    """Ranks draw DIFFERENT dropout masks for their shards: the kernels' counter-based generator is seeded per process."""
+    ops.rng.seed = (ops.rng.seed ^ (0x9E3779B97F4A7C15 * (rank + 1))) & 0xFFFFFFFFFFFFFFFF
+
+
+class GradAllReduce:
+    """ONE logical all-reduce(SUM) of a FlatParams gradient buffer (with its extras) per step.  When the CNN front end's
+    parameters sit at the tail of the buffer (0 < flat.tail_offset < numel) it goes out in two pieces: the head -- every
+    gradient before tail_offset, final once the front end's backward starts -- is issued from ops.frontend_backward_hook on
+    the process group's own stream and runs under the convolution backward; the tail follows after backward.  A rank whose
+    backward did not reach the hook (an empty shard) issues the head itself, so every rank issues the same collectives."""
+
+    def __init__(self, flat, process_group=None):
+        self.flat = flat
+        self.pg = process_group
+        self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
+        self._early = None
+
+    def _split(self) -> bool:
+        return 0 < self.flat.tail_offset < self.flat.numel
+
+    def _reduce_head_early(self):
+        if self.world > 1 and self._early is None and self._split():
+            self._early = dist.all_reduce(self.flat.flat_grad[:self.flat.tail_offset], op=dist.ReduceOp.SUM, group=self.pg,
+                                          async_op=True)
+
+    def backward(self, loss):
+        """loss.backward() with the head of the all-reduce issued under the front end's backward."""
+        self._early = None
+        prev, ops.frontend_backward_hook = ops.frontend_backward_hook, self._reduce_head_early
+        try:
+            loss.backward()
+        finally:
+            ops.frontend_backward_hook = prev
+
+    def finish(self):
+        """The rest of the all-reduce; on return the whole buffer holds the sums over the ranks."""
+        if self.world <= 1:
+            return
+        g = self.flat.flat_grad
+        if self._split():
+            if self._early is None:
+                self._reduce_head_early()
+            dist.all_reduce(g[self.flat.tail_offset:], op=dist.ReduceOp.SUM, group=self.pg)
+            self._early.wait()
+            self._early = None
+        else:
+            dist.all_reduce(g, op=dist.ReduceOp.SUM, group=self.pg)
 
 
 class HostBatchPrefetcher:
@@ -76,36 +211,21 @@ class DataParallelStep:
         self.opt = NoamOpt(model_size, k_lr, warmup, self.adam, min_lr=min_lr)
         self.smoothing = smoothing
         self.pg = process_group
-        self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
+        self.reducer = GradAllReduce(self.flat, process_group)
+        self.world = self.reducer.world
         self.clip = clip_max_norm
-        self._early = None          # the all-reduce of the gradients before flat.tail_offset, issued by _reduce_head_early
         self._scale = torch.zeros(4, device=self.flat.flat.device, dtype=torch.float32)    # [scale, grad norm, scratch, -]
         self._host_tail = loss_fn is not None or adam_factory is not None                  # CPU stand-ins (gloo tests)
         if self.world > 1:
-            # replicas start identical (nn.DataParallel re-replicates from device 0 every step, utils/functions.py:158-160;
-            # here once is enough because every rank applies the identical update) ...
-            dist.broadcast(self.flat.flat, src=dist.get_global_rank(process_group, 0) if process_group is not None else 0,
-                           group=process_group)
-            # ... but draw DIFFERENT dropout masks for their shards (the kernels' counter-based generator is seeded per process)
-            ops.rng.seed = (ops.rng.seed ^ (0x9E3779B97F4A7C15 * (dist.get_rank(process_group) + 1))) & 0xFFFFFFFFFFFFFFFF
-
-    def _reduce_head_early(self):
-        """Runs at the start of the CNN front end's backward (ops.frontend_backward_hook): every gradient before
-        flat.tail_offset is final, so their all-reduce is issued now, on NCCL's own stream, under the convolution backward."""
-        if self.world > 1 and self._early is None and 0 < self.flat.tail_offset < self.flat.numel:
-            self._early = dist.all_reduce(self.flat.flat_grad[:self.flat.tail_offset], op=dist.ReduceOp.SUM, group=self.pg, async_op=True)
+            broadcast_params(self.flat, process_group)
+            fold_rank_into_dropout(dist.get_rank(process_group))
 
     def forward_backward(self, src, lengths, tgt):
         """Local shard fwd+bwd with the un-normalised loss; gradients land in the flat buffer."""
         self.flat.zero_grad()
         pred, gold, hyp, _ = self.model(src, lengths, tgt)
         loss_sum, stats = self.loss_fn(pred, gold, self.smoothing, reduction="sum")
-        self._early = None
-        prev, ops.frontend_backward_hook = ops.frontend_backward_hook, self._reduce_head_early
-        try:
-            loss_sum.backward()
-        finally:
-            ops.frontend_backward_hook = prev
+        self.reducer.backward(loss_sum)
         self.flat.ensure_grad_views()
         self.flat.extras.copy_(stats[0:2])            # [sum-loss, n_tokens] ride with the gradients
         return pred, hyp, stats
@@ -113,15 +233,9 @@ class DataParallelStep:
     def all_reduce(self):
         """ONE logical all-reduce(SUM) of [flat grads | sum-loss | n_tokens] per step (the reference's --parallel reduce,
         utils/functions.py:154-160): issued as a head part that overlaps the front end's backward (when forward_backward
-        could launch it) and the remaining tail (front-end gradients + the two scalars), or in one piece otherwise."""
-        if self.world <= 1:
-            return
-        if self._early is not None:
-            dist.all_reduce(self.flat.flat_grad[self.flat.tail_offset:], op=dist.ReduceOp.SUM, group=self.pg)
-            self._early.wait()
-            self._early = None
-        else:
-            dist.all_reduce(self.flat.flat_grad, op=dist.ReduceOp.SUM, group=self.pg)
+        could launch it) and the remaining tail (front-end gradients + the two scalars), or in one piece when the model has no
+        front end at the tail of the buffer (GradAllReduce)."""
+        self.reducer.finish()
 
     def optimizer_step(self):
         """Adam with the gradient read as g * (1 / global n_tokens) * clip coefficient -- both computed on the device
