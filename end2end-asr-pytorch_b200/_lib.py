@@ -54,6 +54,7 @@ SIGNATURES = {
     "b200asr_stft_features": (_i, [_vp] * 5 + [_i] * 9 + [_vp]),
     "b200asr_stft_features_ex_ws_bytes": (_sz, [_i, _i, _i, _i]),
     "b200asr_stft_features_ex": (_i, [_vp] * 5 + [_i] * 9 + [_vp, _ll, _vp, _vp, _i, _i, _vp]),
+    "b200asr_stft_features_packed": (_i, [_vp] * 6 + [_i] * 9 + [_vp, _ll, _vp, _vp, _i, _i, _vp]),
     "b200asr_conv3x3_c1_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_c1_bwd_weight": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),

@@ -45,10 +45,17 @@ static FeatWs feat_ws(int B, int Lmax, int n_fft, int hop) {
 //   x[s] + ((level * n[s]) * e_x) / e_n,   n = bank[nstart[b] : nstart[b] + len],   e = sqrt(sum of squares / len)
 // with the sums of squares from feat_energy_kernel + feat_stats_kernel.  A silent segment gives 0/0 = NaN, a silent
 // utterance x + 0, as numpy does.  A segment that leaves the bank makes the whole utterance NaN instead of being read.
+// Utterance b starts at wave + utt_base(b): offsets[b] in a packed batch, b * Lmax in a [B, Lmax] one (offsets NULL); a
+// negative offset makes the utterance NaN instead of being read.
+__device__ __forceinline__ long long utt_base(const long long* __restrict__ offsets, int b, int Lmax) {
+  return offsets ? offsets[b] : (long long)b * Lmax;
+}
+
 template <bool kNoise>
-__global__ void feat_pad_kernel(const float* __restrict__ wave, const int* __restrict__ lens, float* __restrict__ padded,
-                                int B, int Lmax, int Lp, int half, int reflect, size_t total, const float* __restrict__ bank,
-                                long long bank_len, const long long* __restrict__ nstart, const float* __restrict__ nlevel,
+__global__ void feat_pad_kernel(const float* __restrict__ wave, const long long* __restrict__ offsets,
+                                const int* __restrict__ lens, float* __restrict__ padded, int B, int Lmax, int Lp, int half,
+                                int reflect, size_t total, const float* __restrict__ bank, long long bank_len,
+                                const long long* __restrict__ nstart, const float* __restrict__ nlevel,
                                 const double* __restrict__ estats) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -68,7 +75,9 @@ __global__ void feat_pad_kernel(const float* __restrict__ wave, const int* __res
           src = m < len ? m : period - m;
         }
       }
-      if (src >= 0) v = wave[(size_t)b * Lmax + src];
+      const long long base = utt_base(offsets, b, Lmax);
+      if (base < 0) src = -1, v = __int_as_float(0x7fc00000);
+      if (src >= 0) v = wave[base + src];
       if (kNoise && src >= 0) {
         const long long st = nstart[b];
         if (st >= 0) {
@@ -89,18 +98,18 @@ __global__ void feat_pad_kernel(const float* __restrict__ wave, const int* __res
 // parts[b][c][2] for feat_stats_kernel to add up in chunk order (no atomics: the same bits every call).
 constexpr int kEnergyChunk = 4096;
 
-__global__ void feat_energy_kernel(const float* __restrict__ wave, const int* __restrict__ lens, const float* __restrict__ bank,
-                                   long long bank_len, const long long* __restrict__ nstart, double* __restrict__ parts,
-                                   int Lmax) {
+__global__ void feat_energy_kernel(const float* __restrict__ wave, const long long* __restrict__ offsets,
+                                   const int* __restrict__ lens, const float* __restrict__ bank, long long bank_len,
+                                   const long long* __restrict__ nstart, double* __restrict__ parts, int Lmax) {
   __shared__ double red[2][8];
   const int b = blockIdx.y, c = blockIdx.x;
   const int len = lens[b];
-  const long long st = nstart[b];
+  const long long st = nstart[b], base = utt_base(offsets, b, Lmax);
   double sx = 0.0, sn = 0.0;
-  if (st >= 0 && st <= bank_len - len) {
+  if (st >= 0 && st <= bank_len - len && base >= 0) {
     const int hi = min(len, (c + 1) * kEnergyChunk);
     for (int i = c * kEnergyChunk + (int)threadIdx.x; i < hi; i += 256) {
-      const double x = wave[(size_t)b * Lmax + i], n = bank[st + i];
+      const double x = wave[base + i], n = bank[st + i];
       sx += x * x;
       sn += n * n;
     }
@@ -255,7 +264,7 @@ static int feat_check(const float* wave, const int* lens, const float* out, cons
 
 // Enqueues the front end on checked arguments.  Statistics cover min(frames, stat_cap) frames of each utterance, with
 // gx_stat >= ceil(Tmax / 32) frame tiles; min(frames, keep_cap) frames are stored.
-static int feat_run(const float* wave, const int* lens, float* out, int* frames_out, void* ws, int B, int Lmax, int Tmax,
+static int feat_run(const float* wave, const long long* offsets, const int* lens, float* out, int* frames_out, void* ws, int B, int Lmax, int Tmax,
                     int n_fft, int hop, int pad_reflect, int normalize, int window, int window_periodic, const FeatNoise* noise,
                     int stat_cap, int keep_cap, int gx_stat, int precision, cudaStream_t st) {
   const FeatWs w = feat_ws(B, Lmax, n_fft, hop);
@@ -273,18 +282,18 @@ static int feat_run(const float* wave, const int* lens, float* out, int* frames_
     // energies: partials in the workspace past the front end's own part, then (sum x^2, sum n^2) per utterance
     double* eparts = (double*)(base + w.total);
     double* estats = eparts + 2 * (size_t)B * feat_energy_chunks(Lmax);
-    feat_energy_kernel<<<dim3((unsigned)feat_energy_chunks(Lmax), B), 256, 0, st>>>(wave, lens, noise->bank, noise->bank_len,
-                                                                                   noise->start, eparts, Lmax);
+    feat_energy_kernel<<<dim3((unsigned)feat_energy_chunks(Lmax), B), 256, 0, st>>>(wave, offsets, lens, noise->bank,
+                                                                                   noise->bank_len, noise->start, eparts, Lmax);
     rc = check_launch("feat_energy");
     if (rc) return rc;
     feat_stats_kernel<<<B, 32, 0, st>>>(eparts, estats, (int)feat_energy_chunks(Lmax), (int)feat_energy_chunks(Lmax));
     rc = check_launch("feat_energy_stats");
     if (rc) return rc;
-    feat_pad_kernel<true><<<pad_blocks, 256, 0, st>>>(wave, lens, padded, B, Lmax, w.Lp, n_fft / 2, pad_reflect, total, noise->bank,
-                                                       noise->bank_len, noise->start, noise->level, estats);
+    feat_pad_kernel<true><<<pad_blocks, 256, 0, st>>>(wave, offsets, lens, padded, B, Lmax, w.Lp, n_fft / 2, pad_reflect, total,
+                                                       noise->bank, noise->bank_len, noise->start, noise->level, estats);
   } else {
-    feat_pad_kernel<false><<<pad_blocks, 256, 0, st>>>(wave, lens, padded, B, Lmax, w.Lp, n_fft / 2, pad_reflect, total, nullptr,
-                                                        0, nullptr, nullptr, nullptr);
+    feat_pad_kernel<false><<<pad_blocks, 256, 0, st>>>(wave, offsets, lens, padded, B, Lmax, w.Lp, n_fft / 2, pad_reflect, total,
+                                                        nullptr, 0, nullptr, nullptr, nullptr);
   }
   rc = check_launch("feat_pad");
   if (rc) return rc;
@@ -331,7 +340,7 @@ int b200asr_stft_features(const float* wave, const int* lens, float* out, int* f
                           b200asr_stream_t stream) {
   const int rc = feat_check(wave, lens, out, ws, B, Lmax, Tmax, n_fft, hop, precision);
   if (rc) return rc;
-  return feat_run(wave, lens, out, frames_out, ws, B, Lmax, Tmax, n_fft, hop, pad_reflect, normalize, 0, window_periodic, nullptr,
+  return feat_run(wave, nullptr, lens, out, frames_out, ws, B, Lmax, Tmax, n_fft, hop, pad_reflect, normalize, 0, window_periodic, nullptr,
                   Tmax, Tmax, ceil_div(Tmax, 32), precision, (cudaStream_t)stream);
 }
 
@@ -341,24 +350,51 @@ size_t b200asr_stft_features_ex_ws_bytes(int B, int Lmax, int n_fft, int hop) {
   return (feat_ws(B, Lmax, n_fft, hop).total + 4 * (size_t)B * (feat_energy_chunks(Lmax) + 1)) * sizeof(float);
 }
 
-int b200asr_stft_features_ex(const float* wave, const int* lens, float* out, int* frames_out, void* ws, int B, int Lmax,
-                             int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window, int window_periodic,
-                             const float* noise_bank, long long noise_bank_len, const long long* noise_start,
-                             const float* noise_level, int max_frames, int precision, b200asr_stream_t stream) {
-  B200_REQUIRE(window >= 0 && window <= 3, B200ASR_BAD_ARG, "stft_features_ex: window %d (0 Hamming, 1 Hann, 2 Blackman, 3 Bartlett)",
+}  // extern "C"
+
+// b200asr_stft_features_ex (offsets NULL: utterance b at wave + b * Lmax) and b200asr_stft_features_packed (at
+// wave + offsets[b]): one path
+static int feat_ex(const char* what, const float* wave, const long long* offsets, const int* lens, float* out, int* frames_out,
+                   void* ws, int B, int Lmax, int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window,
+                   int window_periodic, const float* noise_bank, long long noise_bank_len, const long long* noise_start,
+                   const float* noise_level, int max_frames, int precision, cudaStream_t stream) {
+  B200_REQUIRE(window >= 0 && window <= 3, B200ASR_BAD_ARG, "%s: window %d (0 Hamming, 1 Hann, 2 Blackman, 3 Bartlett)", what,
                window);
   B200_REQUIRE((noise_bank == nullptr) == (noise_start == nullptr) && (noise_bank == nullptr) == (noise_level == nullptr),
-               B200ASR_BAD_ARG, "stft_features_ex: noise_bank, noise_start and noise_level go together");
-  B200_REQUIRE(noise_bank == nullptr || noise_bank_len > 0, B200ASR_BAD_SHAPE, "stft_features_ex: noise_bank_len=%lld",
-               noise_bank_len);
-  B200_REQUIRE(max_frames > 0, B200ASR_BAD_SHAPE, "stft_features_ex: max_frames=%d", max_frames);
+               B200ASR_BAD_ARG, "%s: noise_bank, noise_start and noise_level go together", what);
+  B200_REQUIRE(noise_bank == nullptr || noise_bank_len > 0, B200ASR_BAD_SHAPE, "%s: noise_bank_len=%lld", what, noise_bank_len);
+  B200_REQUIRE(max_frames > 0, B200ASR_BAD_SHAPE, "%s: max_frames=%d", what, max_frames);
   const int rc = feat_check(wave, lens, out, ws, B, Lmax, Tmax, n_fft, hop, precision);
   if (rc) return rc;
   const FeatNoise noise = {noise_bank, noise_bank_len, noise_start, noise_level};
   // statistics over every frame an utterance of at most Lmax samples can have, whatever is stored
-  return feat_run(wave, lens, out, frames_out, ws, B, Lmax, Tmax, n_fft, hop, pad_reflect, normalize, window, window_periodic,
-                  noise_bank ? &noise : nullptr, INT_MAX, min(max_frames, Tmax), ceil_div(1 + Lmax / hop, 32), precision,
-                  (cudaStream_t)stream);
+  return feat_run(wave, offsets, lens, out, frames_out, ws, B, Lmax, Tmax, n_fft, hop, pad_reflect, normalize, window,
+                  window_periodic, noise_bank ? &noise : nullptr, INT_MAX, min(max_frames, Tmax), ceil_div(1 + Lmax / hop, 32),
+                  precision, stream);
+}
+
+extern "C" {
+
+int b200asr_stft_features_ex(const float* wave, const int* lens, float* out, int* frames_out, void* ws, int B, int Lmax,
+                             int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window, int window_periodic,
+                             const float* noise_bank, long long noise_bank_len, const long long* noise_start,
+                             const float* noise_level, int max_frames, int precision, b200asr_stream_t stream) {
+  return feat_ex("stft_features_ex", wave, nullptr, lens, out, frames_out, ws, B, Lmax, Tmax, n_fft, hop, pad_reflect, normalize, window,
+                 window_periodic, noise_bank, noise_bank_len, noise_start, noise_level, max_frames, precision,
+                 (cudaStream_t)stream);
+}
+
+int b200asr_stft_features_packed(const float* wave, const long long* offsets, const int* lens, float* out, int* frames_out,
+                                 void* ws, int B, int Lmax, int Tmax, int n_fft, int hop, int pad_reflect, int normalize,
+                                 int window, int window_periodic, const float* noise_bank, long long noise_bank_len,
+                                 const long long* noise_start, const float* noise_level, int max_frames, int precision,
+                                 b200asr_stream_t stream) {
+  B200_REQUIRE(offsets, B200ASR_BAD_ARG, "stft_features_packed: null offsets");
+  B200_REQUIRE(((uintptr_t)offsets & 7) == 0 && ((uintptr_t)wave & 3) == 0, B200ASR_BAD_ALIGN,
+               "stft_features_packed: offsets must be 8-byte and wave 4-byte aligned");
+  return feat_ex("stft_features_packed", wave, offsets, lens, out, frames_out, ws, B, Lmax, Tmax, n_fft, hop, pad_reflect, normalize, window,
+                 window_periodic, noise_bank, noise_bank_len, noise_start, noise_level, max_frames, precision,
+                 (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -5,11 +5,13 @@ Mirrors `SpectrogramParser.parse_audio` (utils/data_loader.py:60-91), `Spectrogr
 hop = sample_rate * window_stride, the symmetric window -- the reference passes the callable scipy.signal.<window>, which
 librosa evaluates as window(n_fft), i.e. sym=True --, centred frames), magnitude, log1p, per-utterance mean /
 unbiased-std normalisation, the src_max_len cut, zero padding to the longest utterance.  One C-ABI call
-(`b200asr_stft_features_ex`): the STFT of the whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
+(`b200asr_stft_features_ex`, or `b200asr_stft_features_packed` over utterances packed back to back): the STFT of the
+whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
 
 `spectrogram_batch` returns the device triple `(inputs, input_percentages, input_sizes)`; `collate_waves` returns
-`_collate_fn`'s 5-tuple, sorted, with everything but `inputs` on the host.  `NoiseBank` holds the noise clips on the
-device and makes the reference's random draws.
+`_collate_fn`'s 5-tuple, sorted, with everything but `inputs` on the host.  `NoiseClips` holds the noise clips' lengths
+and makes the reference's random draws (host data: DataLoader workers draw with it); `NoiseBank` adds the clips on the
+device.  loader.py feeds the reference's AudioDataLoader from here.
 """
 from __future__ import annotations
 
@@ -50,83 +52,116 @@ class NoiseDraws:
         return NoiseDraws(self.bank, self.add[order], self.clip[order], self.level[order], self.rand[order], self.start[order])
 
 
+class NoiseClips:
+    """Where the noise clips of `NoiseInjection` (utils/data_loader.py:147-179) lie in a `NoiseBank`: their lengths in
+    samples, their offsets when back to back, and their sample rate.  Host data that pickles, so DataLoader workers make
+    the reference's draws with it (loader.py) while the samples stay on the device."""
+
+    def __init__(self, lengths, sample_rate: int):
+        self.lengths = np.asarray(lengths, dtype=np.int64).reshape(-1)
+        if len(self.lengths) == 0:
+            raise ValueError("NoiseBank needs at least one clip")
+        self.offsets = np.concatenate([[0], np.cumsum(self.lengths)[:-1]]).astype(np.int64)
+        self.sample_rate = int(sample_rate)
+
+    def __len__(self):
+        return len(self.lengths)
+
+    def draw_one(self, n: int, noise_prob: float, noise_levels, rng=np.random):
+        """The reference's draws for one utterance of `n` samples, with its numpy calls in its order (data_loader.py:68-69,
+        164-165, 171): binomial(1, noise_prob), and only for a 1: choice over the clips, uniform(*noise_levels), rand().
+        `rng` is np.random (the reference's global state) or a RandomState.  Returns (add, clip, level, rand, start): clip
+        -1, level and rand NaN, start -1 without noise.
+
+        The segment start is noise_start = rand * (clip_len / sr - n / sr) seconds, in float64 as :169-172.  The reference
+        then cuts the segment with sox `trim` (utils/audio.py:21-32); that cut is not pinned here but restated as the
+        sample round(noise_start * sr), clamped so that the n samples fit in the clip; `start` is that sample's index in
+        the bank.  A clip shorter than the utterance, where the reference fails its assert (:175), raises ValueError."""
+        n = int(n)
+        if not rng.binomial(1, noise_prob):
+            return 0, -1, float("nan"), float("nan"), -1
+        c = int(rng.choice(len(self)))                # np.random.choice(paths): one randint(0, len(paths)) draw
+        level = rng.uniform(*noise_levels)
+        rand = rng.rand()
+        clip_len = int(self.lengths[c])
+        if clip_len < n:
+            raise ValueError(f"noise clip {c} has {clip_len} samples, fewer than an utterance's {n}")
+        noise_start = rand * (clip_len / self.sample_rate - n / self.sample_rate)
+        return 1, c, level, rand, int(self.offsets[c]) + min(max(round(noise_start * self.sample_rate), 0), clip_len - n)
+
+    def check(self, clip, start, lengths):
+        """ValueError unless every segment with start >= 0 lies inside its clip."""
+        clip, start, lengths = (np.asarray(a, dtype=np.int64) for a in (clip, start, lengths))
+        if not (len(clip) == len(start) == len(lengths)):
+            raise ValueError(f"{len(start)} noise draws for {len(lengths)} utterances")
+        noisy = start >= 0
+        c = clip[noisy]
+        if ((c < 0) | (c >= len(self))).any() or (start[noisy] < self.offsets[c]).any() or \
+                (start[noisy] + lengths[noisy] > self.offsets[c] + self.lengths[c]).any():
+            raise ValueError("a noise segment does not lie inside its clip")
+
+
 class NoiseBank:
     """Noise clips for `NoiseInjection` (utils/data_loader.py:147-179), back to back in one device buffer.
 
     `clips` are 1-D fp32 waveforms at `sample_rate`, in the order `librosa.util.find_files(noise_dir)` lists them (sorted
     paths): `draw` picks clips by index, so that order is what makes its choices the reference's.  Reading and resampling
-    the files is the caller's job."""
+    the files is the caller's job.  `clips` (a NoiseClips) is the host side the draws need."""
 
     def __init__(self, clips, sample_rate: int, device=None):
         arrays = [np.asarray(c.detach().cpu() if isinstance(c, torch.Tensor) else c, dtype=np.float32).reshape(-1) for c in clips]
-        if not arrays:
-            raise ValueError("NoiseBank needs at least one clip")
-        self.sample_rate = int(sample_rate)
-        self.lengths = np.array([len(a) for a in arrays], dtype=np.int64)
-        self.offsets = np.concatenate([[0], np.cumsum(self.lengths)[:-1]]).astype(np.int64)
+        self.clips = NoiseClips([len(a) for a in arrays], sample_rate)
         device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.bank = torch.from_numpy(np.concatenate(arrays)).to(device)
 
+    sample_rate = property(lambda self: self.clips.sample_rate)
+    lengths = property(lambda self: self.clips.lengths)
+    offsets = property(lambda self: self.clips.offsets)
+
     def __len__(self):
-        return len(self.lengths)
+        return len(self.clips)
 
     def draw(self, lengths, noise_prob: float, noise_levels, rng=np.random) -> NoiseDraws:
-        """The reference's draws for utterances of `lengths` samples, each in batch order, with its numpy calls in its
-        order (data_loader.py:68-69, 164-165, 171): binomial(1, noise_prob), and only for a 1: choice over the clips,
-        uniform(*noise_levels), rand().  `rng` is np.random (the reference's global state) or a RandomState.
-
-        The segment start is noise_start = rand * (clip_len / sr - L / sr) seconds, in float64 as :169-172.  The reference
-        then cuts the segment with sox `trim` (utils/audio.py:21-32); that cut is not pinned here but restated as the
-        sample round(noise_start * sr), clamped so that the L samples fit in the clip.  A clip shorter than the utterance,
-        where the reference fails its assert (:175), raises ValueError."""
-        B = len(lengths)
-        add, clip = np.zeros(B, np.int64), np.full(B, -1, np.int64)
-        level, rand = np.full(B, np.nan), np.full(B, np.nan)
-        start = np.full(B, -1, np.int64)
-        sr = self.sample_rate
-        for b, n in enumerate(lengths):
-            n = int(n)
-            add[b] = rng.binomial(1, noise_prob)
-            if not add[b]:
-                continue
-            c = int(rng.choice(len(self)))            # np.random.choice(paths): one randint(0, len(paths)) draw
-            level[b] = rng.uniform(*noise_levels)
-            rand[b] = rng.rand()
-            clip_len = int(self.lengths[c])
-            if clip_len < n:
-                raise ValueError(f"noise clip {c} has {clip_len} samples, fewer than utterance {b}'s {n}")
-            noise_start = rand[b] * (clip_len / sr - n / sr)
-            clip[b] = c
-            start[b] = self.offsets[c] + min(max(round(noise_start * sr), 0), clip_len - n)
+        """NoiseClips.draw_one for utterances of `lengths` samples, in batch order."""
+        rows = [self.clips.draw_one(n, noise_prob, noise_levels, rng) for n in lengths]
+        add, clip, level, rand, start = (np.array(col, dtype=dt).reshape(-1) for col, dt in
+                                         zip(zip(*rows) if rows else ((),) * 5,
+                                             (np.int64, np.int64, np.float64, np.float64, np.int64)))
         return NoiseDraws(self, add, clip, level, rand, start)
+
+    def device_args(self, clip, start, level, lengths, device):
+        """(bank, bank_len, start, level) for the feature calls, or None when no utterance takes noise.  clip, start and
+        lengths are host arrays (NoiseClips.check's); start and level are uploaded without a host synchronisation (pinned
+        CPU tensors, e.g. from a DataLoader's pin-memory thread, go as they are)."""
+        start_np = start.numpy() if isinstance(start, torch.Tensor) else np.asarray(start)
+        self.clips.check(clip, start_np, lengths)
+        if not (start_np >= 0).any():
+            return None
+        if self.bank.device != torch.device(device):
+            raise ValueError(f"the noise bank is on {self.bank.device}, the batch on {device}")
+        up = lambda a, dt: a.to(device, non_blocking=True) if isinstance(a, torch.Tensor) else _pinned_to(np.asarray(a, dt), device)  # noqa: E731
+        return self.bank, self.bank.numel(), up(start, np.int64), up(level, np.float32)
 
     def _device_args(self, draws: NoiseDraws, lengths, device):
         """(bank, bank_len, start, level) for b200asr_stft_features_ex, or None when no utterance takes noise."""
         if draws.bank is not self:
             raise ValueError("the draws were made by another NoiseBank")
-        if len(draws.start) != len(lengths):
-            raise ValueError(f"{len(draws.start)} noise draws for {len(lengths)} utterances")
-        noisy = draws.start >= 0
-        if not noisy.any():
-            return None
-        lengths = np.asarray(lengths, dtype=np.int64)
-        c = draws.clip[noisy]
-        if ((c < 0) | (c >= len(self))).any() or (draws.start[noisy] < self.offsets[c]).any() or \
-                (draws.start[noisy] + lengths[noisy] > self.offsets[c] + self.lengths[c]).any():
-            raise ValueError("a noise segment does not lie inside its clip")
-        if self.bank.device != torch.device(device):
-            raise ValueError(f"the noise bank is on {self.bank.device}, the batch on {device}")
-        return (self.bank, self.bank.numel(), _pinned_to(draws.start.astype(np.int64), device),
-                _pinned_to(draws.level.astype(np.float32), device))
+        return self.device_args(draws.clip, draws.start, draws.level, lengths, device)
 
 
 def _geometry(sample_rate, window_size, window_stride):
     return int(sample_rate * window_size), int(sample_rate * window_stride)
 
 
-def _features(wave, lens, t_max, n_fft, hop, normalize, reflect, precision, window, window_periodic, noise, max_frames):
-    """One b200asr_stft_features_ex call on a [B, Lmax] device batch: (inputs [B,1,F,t_max], frames [B] int32)."""
-    B, Lmax = wave.shape
+def _features(wave, lens, t_max, n_fft, hop, normalize, reflect, precision, window, window_periodic, noise, max_frames,
+              offsets=None, Lmax=None):
+    """One b200asr_stft_features_ex call on a [B, Lmax] device batch, or with `offsets` one b200asr_stft_features_packed
+    call on `wave` holding the utterances back to back (utterance b at offsets[b], Lmax >= every length):
+    (inputs [B,1,F,t_max], frames [B] int32)."""
+    if offsets is None:
+        B, Lmax = wave.shape
+    else:
+        B = offsets.numel()
     nb = n_fft // 2 + 1
     lib = ops._lib()
     ws = torch.empty(lib.b200asr_stft_features_ex_ws_bytes(B, Lmax, n_fft, hop) // 4, device=wave.device, dtype=torch.float32)
@@ -135,11 +170,28 @@ def _features(wave, lens, t_max, n_fft, hop, normalize, reflect, precision, wind
     prec = ops.config.linear if precision is None else precision
     prec = {L.PREC_BF16X3: L.PREC_TF32X3, L.PREC_BF16: L.PREC_TF32}.get(prec, prec)      # the DFT basis is an fp32 operand: tf32 grades
     bank, bank_len, start, level = noise if noise is not None else (None, 0, None, None)
-    L.check(lib.b200asr_stft_features_ex(L.ptr(wave), L.ptr(lens), L.ptr(out), L.ptr(frames), L.ptr(ws), B, Lmax, t_max, n_fft,
-                                         hop, int(reflect), int(normalize), WINDOWS.get(window, 0), int(window_periodic),
-                                         L.ptr(bank), bank_len, L.ptr(start), L.ptr(level), NO_CUT if max_frames is None else max_frames,
-                                         prec, ops._stream()), "stft_features_ex")
+    args = (L.ptr(lens), L.ptr(out), L.ptr(frames), L.ptr(ws), B, Lmax, t_max, n_fft, hop, int(reflect), int(normalize),
+            WINDOWS.get(window, 0), int(window_periodic), L.ptr(bank), bank_len, L.ptr(start), L.ptr(level),
+            NO_CUT if max_frames is None else max_frames, prec, ops._stream())
+    if offsets is None:
+        L.check(lib.b200asr_stft_features_ex(L.ptr(wave), *args), "stft_features_ex")
+    else:
+        L.check(lib.b200asr_stft_features_packed(L.ptr(wave), L.ptr(offsets), *args), "stft_features_packed")
     return out, frames
+
+
+def stft_features_packed(wave: torch.Tensor, offsets: torch.Tensor, lengths: torch.Tensor, Lmax: int, t_max: int,
+                         sample_rate: int = 16000, window_size: float = 0.02, window_stride: float = 0.01, normalize: bool = True,
+                         reflect: bool = True, precision: int | None = None, window_periodic: bool = False,
+                         window: str = "hamming", noise=None, max_frames: int | None = None):
+    """The features of a packed batch: utterance b is the lengths[b] samples of the 1-D CUDA fp32 `wave` from offsets[b]
+    (int64) on.  `Lmax` >= every length and `t_max` are host ints (no host read of the device arrays); `noise` is
+    NoiseBank.device_args' tuple or None.  Equal bit for bit to spectrogram_batch on the same utterances zero-padded to
+    [B, Lmax].  Returns (inputs [B,1,F,t_max] fp32, input_sizes [B] int32) on the device."""
+    n_fft, hop = _geometry(sample_rate, window_size, window_stride)
+    ops._need_cuda(wave, offsets, lengths)
+    return _features(ops._f32c(wave), lengths.to(torch.int32), t_max, n_fft, hop, normalize, reflect, precision, window,
+                     window_periodic, noise, max_frames, offsets=offsets.to(torch.int64), Lmax=int(Lmax))
 
 
 def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: torch.Tensor | None = None, sample_rate: int = 16000,
@@ -205,17 +257,18 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     frames = [min(1 + n // hop, src_max_len) for n in lens]
     order = sorted(range(len(batch)), key=frames.__getitem__, reverse=True)          # sorted(..., reverse=True) is stable
     B, Lmax = len(batch), max(1, max(lens))
-    host = torch.empty((B, Lmax), dtype=torch.float32, pin_memory=True)           # packed in place, uploaded without a sync
+    slens = np.array([lens[i] for i in order], dtype=np.int32)
+    offsets = np.concatenate([[0], np.cumsum(slens, dtype=np.int64)[:-1]])
+    host = torch.empty(max(1, int(slens.sum())), dtype=torch.float32, pin_memory=True)   # back to back, uploaded without a sync
     h = host.numpy()
     for r, i in enumerate(order):
-        h[r, :lens[i]] = waves[i]
-        h[r, lens[i]:] = 0.0
+        h[offsets[r]:offsets[r] + lens[i]] = waves[i]
     device = torch.device("cuda", torch.cuda.current_device())
-    slens = np.array([lens[i] for i in order], dtype=np.int32)
     dev_noise = None if draws is None else noise_bank._device_args(draws.take(order), slens, device)
     t_max = frames[order[0]]
     inputs, _ = _features(host.to(device, non_blocking=True), _pinned_to(slens, device), t_max, n_fft, hop, normalize, reflect,
-                          precision, audio_conf.get("window", "hamming"), False, dev_noise, src_max_len)
+                          precision, audio_conf.get("window", "hamming"), False, dev_noise, src_max_len,
+                          offsets=_pinned_to(offsets, device), Lmax=Lmax)
     targets_list = [batch[i][1] for i in order]
     max_tgt = max(len(t) for t in targets_list)
     targets = torch.zeros(B, max_tgt, dtype=torch.int64)

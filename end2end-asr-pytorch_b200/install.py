@@ -12,6 +12,12 @@ stay reachable through original(): LM rescoring with an LM other than an LSTM LM
 GRU / RNN LM its own RNNModel.forward, an optimizer other than a plain fp32 CUDA torch.optim.Adam its own NoamOpt.step, greedy_search with lm_rescoring=True or in training mode and evaluate in training
 mode the reference's own methods.
 
+When utils/data_loader.py is imported before install(), `AudioDataLoader.__init__` / `__iter__` are bound too
+(loader.audio_loader_init / audio_loader_iter): a loader over a SpectrogramDataset yields `_collate_fn`'s batches with
+`inputs` computed on the device, its workers only reading audio and making the reference's random draws.  A loader over
+another dataset, with the caller's own collate_fn, or with noise clips at another sample rate runs
+original(AudioDataLoader, "__iter__").
+
 Data-parallel training: when the environment of `python -m b200asr.launch` describes more than one rank (WORLD_SIZE > 1),
 or `process_group=` is passed, install() joins that process group and the bound Trainer.train trains across it
 (trainer.trainer_train, parallel.join).  Otherwise nothing about a single process changes.
@@ -21,7 +27,7 @@ from __future__ import annotations
 import importlib
 import sys
 
-from . import metrics, modules, optim, parallel, trainer
+from . import loader, metrics, modules, optim, parallel, trainer
 
 _PATCHED = {}
 
@@ -67,18 +73,25 @@ def install(reference_root: str = None, process_group=None):
     if t_mod is not None:
         targets.append((t_mod, "calculate_metrics", metrics.calculate_metrics))
         targets.append((t_mod.Trainer, "train", trainer.trainer_train))
+    dl_mod = sys.modules.get("utils.data_loader")       # AudioDataLoader: the device feature front end (loader.py)
+    if dl_mod is not None:
+        targets.append((dl_mod.AudioDataLoader, "__init__", loader.audio_loader_init))
+        targets.append((dl_mod.AudioDataLoader, "__iter__", loader.audio_loader_iter))
     for obj, name, new in targets:
         key = (id(obj), name)
-        if key not in _PATCHED:
-            _PATCHED[key] = (obj, name, getattr(obj, name))
+        if key not in _PATCHED:                         # (.., own): `name` was in obj's own dict, not inherited
+            _PATCHED[key] = (obj, name, getattr(obj, name), name in vars(obj))
         setattr(obj, name, new)
     parallel.join(process_group)
     return dict(_PATCHED)
 
 
 def uninstall():
-    for obj, name, old in _PATCHED.values():
-        setattr(obj, name, old)
+    for obj, name, old, own in _PATCHED.values():
+        if own:
+            setattr(obj, name, old)
+        else:
+            delattr(obj, name)
     _PATCHED.clear()
     parallel.leave()
 

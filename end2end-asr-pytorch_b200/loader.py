@@ -1,0 +1,215 @@
+"""The reference's AudioDataLoader (utils/data_loader.py:217-220) fed from the device feature front end.
+
+After install(), an AudioDataLoader over a SpectrogramDataset yields `_collate_fn`'s 5-tuple `(inputs, targets,
+input_percentages, input_sizes, target_sizes)` with `inputs` computed on the current CUDA device by one
+`b200asr_stft_features_packed` call per batch, and the other four host tensors equal to `_collate_fn`'s.
+
+Worker side (host, pickles): `PackedItems[i]` makes `SpectrogramDataset.__getitem__`'s calls in its order -- the manifest
+draw, the reference's own `load_audio` / `load_randomly_augmented_audio`, the noise draws, `parse_transcript` -- but
+returns the waveform and the draws instead of a spectrogram; `collate_items` sorts as `_collate_fn` does and packs the
+waveforms back to back.  Main side: `audio_loader_init` / `audio_loader_iter` (bound onto AudioDataLoader by install())
+read the noise clips once into a NoiseBank, then upload each batch without a host synchronisation and compute its
+features.
+"""
+from __future__ import annotations
+
+import importlib
+import inspect
+import random
+from typing import NamedTuple
+
+import numpy as np
+import torch
+from torch.utils.data import DataLoader, Dataset
+
+from . import features
+
+
+class Item(NamedTuple):
+    """One utterance as a worker returns it: the waveform (fp32), the noise draw as (clip index, first sample in the
+    bank, level) -- (-1, -1, NaN) without noise --, the transcript ids and the frame count after the src_max_len cut."""
+    wave: np.ndarray
+    noise_clip: int
+    noise_start: int
+    noise_level: float
+    ids: list
+    frames: int
+
+
+class PackedBatch(NamedTuple):
+    """A batch as the workers collate it, sorted as `_collate_fn` sorts (frames, longest first, stable): the waveforms
+    back to back (`wave`, at least one sample) at int64 `offsets` with int32 `lengths`; per utterance the noise clip,
+    start (int64, -1 without noise) and level (fp32); `_collate_fn`'s four host tensors; the src_max_len of the cut."""
+    wave: torch.Tensor
+    offsets: torch.Tensor
+    lengths: torch.Tensor
+    noise_clip: torch.Tensor
+    noise_start: torch.Tensor
+    noise_level: torch.Tensor
+    targets: torch.Tensor
+    input_percentages: torch.Tensor
+    input_sizes: torch.Tensor
+    target_sizes: torch.Tensor
+    src_max_len: int
+
+
+def _data_loader():
+    return importlib.import_module("utils.data_loader")
+
+
+class PackedItems(Dataset):
+    """The worker side of a SpectrogramDataset: waveforms and the reference's random draws, no spectrogram.  `clips` (a
+    features.NoiseClips) is set by the loader before its workers start when the dataset injects noise."""
+
+    def __init__(self, dataset, clips: features.NoiseClips | None = None):
+        self.dataset = dataset
+        self.clips = clips
+        self.hop = int(dataset.sample_rate * dataset.window_stride)
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def __getitem__(self, index) -> Item:
+        ds, DL = self.dataset, _data_loader()
+        ids = ds.ids_list[random.randint(0, len(ds.ids_list) - 1)]            # __getitem__ (:127-130)
+        audio_path, transcript_path = ids[index % len(ids)][:2]
+        if ds.augment:                                                        # parse_audio (:61-70)
+            y = DL.load_randomly_augmented_audio(audio_path, ds.sample_rate)
+        else:
+            y = DL.load_audio(audio_path)
+        y = np.ascontiguousarray(y, dtype=np.float32).reshape(-1)
+        clip, start, level = -1, -1, float("nan")
+        if ds.noiseInjector:
+            if self.clips is None:
+                raise RuntimeError("PackedItems: the dataset injects noise but no noise clips were given")
+            _, clip, level, _, start = self.clips.draw_one(len(y), ds.noise_prob, ds.noiseInjector.noise_levels, np.random)
+        transcript = ds.parse_transcript(transcript_path)
+        src_max_len = importlib.import_module("utils.constant").args.src_max_len      # read at call time, as :131
+        return Item(y, clip, start, level, transcript, min(1 + len(y) // self.hop, src_max_len))
+
+
+def collate_items(items) -> PackedBatch:
+    """`_collate_fn` (:182-214) over Items, without the spectrograms: the same order and the same targets, percentages,
+    sizes and target sizes (values and dtypes), the waveforms packed in that order."""
+    order = sorted(range(len(items)), key=lambda i: items[i].frames, reverse=True)   # sorted(..., reverse=True) is stable
+    items = [items[i] for i in order]
+    B, t_max = len(items), items[0].frames
+    lengths = np.array([len(it.wave) for it in items], dtype=np.int64)
+    wave = np.concatenate([it.wave for it in items] + ([np.zeros(1, np.float32)] if lengths.sum() == 0 else []))
+    max_tgt = max(len(it.ids) for it in items)
+    targets = torch.zeros(B, max_tgt, dtype=torch.int64)
+    for r, it in enumerate(items):
+        targets[r, :len(it.ids)] = torch.tensor(list(it.ids), dtype=torch.int32)
+    return PackedBatch(
+        wave=torch.from_numpy(wave),
+        offsets=torch.from_numpy(np.concatenate([[0], np.cumsum(lengths)[:-1]]).astype(np.int64)),
+        lengths=torch.from_numpy(lengths.astype(np.int32)),
+        noise_clip=torch.tensor([it.noise_clip for it in items], dtype=torch.int64),
+        noise_start=torch.tensor([it.noise_start for it in items], dtype=torch.int64),
+        noise_level=torch.tensor([it.noise_level for it in items], dtype=torch.float32),
+        targets=targets,
+        input_percentages=torch.tensor([it.frames / float(t_max) for it in items], dtype=torch.float32),
+        input_sizes=torch.tensor([it.frames for it in items], dtype=torch.int32),
+        target_sizes=torch.tensor([len(it.ids) for it in items], dtype=torch.int32),
+        src_max_len=int(importlib.import_module("utils.constant").args.src_max_len))
+
+
+def _window_name(ds, DL) -> str:
+    """The audio_conf['window'] name SpectrogramParser resolved (:52): the key of DL.windows holding ds.window."""
+    return next((k for k, v in DL.windows.items() if v is ds.window), "hamming")
+
+
+class PackedLoader:
+    """What an installed AudioDataLoader keeps: a DataLoader over PackedItems with collate_items (the caller's sampler,
+    batch sampler, workers and other arguments), the noise bank once read, and the per-batch device step."""
+
+    def __init__(self, outer, arguments: dict):
+        ds = outer.dataset
+        self.items = PackedItems(ds)
+        kwargs = dict(arguments, dataset=self.items, collate_fn=collate_items)
+        kwargs.setdefault("pin_memory", True)
+        self.inner = DataLoader(**kwargs)
+        self.bank = None
+        self.reference = False                  # set when the noise clips need the reference's own path (prepare)
+
+    def prepare(self) -> bool:
+        """Read the noise clips into a NoiseBank on the current device, once, before any worker starts.  False when the
+        reference's loader has to run: noise_dir holds no clips (the reference then fails only on a draw that adds
+        noise, never at noise_prob 0), or a clip whose duration (get_audio_length) does not give its sample count at the
+        dataset's sample rate would be resampled by sox, which is not restated here."""
+        ds = self.items.dataset
+        if self.reference or not ds.noiseInjector:
+            return not self.reference
+        if self.bank is None:
+            if not ds.noiseInjector.paths:              # no clips: the reference fails only on a draw that adds noise
+                self.reference = True
+                return False
+            DL, sr = _data_loader(), ds.sample_rate
+            clips = []
+            for path in ds.noiseInjector.paths:
+                y = np.asarray(DL.load_audio(path), dtype=np.float32).reshape(-1)
+                if round(DL.get_audio_length(path) * sr) != len(y):
+                    self.reference = True
+                    return False
+                clips.append(y)
+            self.bank = features.NoiseBank(clips, sr)
+            self.items.clips = self.bank.clips
+        device = torch.device("cuda", torch.cuda.current_device())
+        if self.bank.bank.device != device:
+            self.bank.bank = self.bank.bank.to(device)
+        return True
+
+    def batch(self, pb: PackedBatch):
+        """`_collate_fn`'s 5-tuple of one PackedBatch: the uploads and one feature call on the current stream."""
+        ds = self.items.dataset
+        device = torch.device("cuda", torch.cuda.current_device())
+        up = lambda t: t.to(device, non_blocking=True)          # noqa: E731
+        lengths = pb.lengths.numpy()
+        noise = None
+        if self.bank is not None:
+            noise = self.bank.device_args(pb.noise_clip.numpy(), pb.noise_start, pb.noise_level, lengths, device)
+        sr = ds.sample_rate
+        inputs, _ = features.stft_features_packed(
+            up(pb.wave), up(pb.offsets), up(pb.lengths), max(1, int(lengths.max())), int(pb.input_sizes[0]), sr,
+            ds.window_size, ds.window_stride, normalize=ds.normalize, window=_window_name(ds, _data_loader()), noise=noise,
+            max_frames=pb.src_max_len)
+        return inputs, pb.targets, pb.input_percentages, pb.input_sizes, pb.target_sizes
+
+
+class _Batches:
+    """Iterator over an installed loader's batches; the DataLoader iterator underneath is made at once, as iter() of the
+    reference's loader makes it (its workers' base seed is drawn then)."""
+
+    def __init__(self, packed: PackedLoader):
+        self.packed = packed
+        self.it = iter(packed.inner)
+
+    def __iter__(self):
+        return self
+
+    def __len__(self):
+        return len(self.it)
+
+    def __next__(self):
+        return self.packed.batch(next(self.it))
+
+
+def audio_loader_init(self, *args, **kwargs):
+    """AudioDataLoader.__init__ after install(): the reference's own construction (so `dataset`, `sampler`, `len()` are
+    its), plus a PackedLoader unless the dataset is not a SpectrogramDataset or the caller passed a collate_fn."""
+    from .install import original
+    original(type(self), "__init__")(self, *args, **kwargs)
+    arguments = inspect.signature(DataLoader.__init__).bind(self, *args, **kwargs).arguments
+    arguments.pop("self")
+    eligible = isinstance(self.dataset, _data_loader().SpectrogramDataset) and arguments.get("collate_fn") is None
+    self._b200asr_packed = PackedLoader(self, dict(arguments)) if eligible else None
+
+
+def audio_loader_iter(self):
+    """AudioDataLoader.__iter__ after install(): device batches from the PackedLoader, or the reference's iterator
+    (original(AudioDataLoader, "__iter__")) for a loader without one, without noise clips or with clips at another rate."""
+    packed = self.__dict__.get("_b200asr_packed")
+    if packed is None or not packed.prepare():
+        from .install import original
+        return original(type(self), "__iter__")(self)
+    return _Batches(packed)

@@ -623,6 +623,19 @@ int b200asr_stft_features_ex(const float* wave, const int* lens, float* out, int
                              int Tmax, int n_fft, int hop, int pad_reflect, int normalize, int window, int window_periodic,
                              const float* noise_bank, long long noise_bank_len, const long long* noise_start,
                              const float* noise_level, int max_frames, int precision, b200asr_stream_t stream);
+/* b200asr_stft_features_ex over a packed batch: utterance b is the lens[b] samples at wave + offsets[b] (offsets: B device
+ * int64, in any order, overlapping or not), so the caller uploads only the real samples instead of a zero-padded [B, Lmax]
+ * rectangle.  Lmax >= every lens[b] sizes the workspace (b200asr_stft_features_ex_ws_bytes(B, Lmax, n_fft, hop)) and
+ * bounds Tmax as in b200asr_stft_features_ex.  The output equals b200asr_stft_features_ex's on the same utterances laid out
+ * at b * Lmax, bit for bit, with every option.  offsets NULL: B200ASR_BAD_ARG; offsets not 8-byte or wave not 4-byte
+ * aligned: B200ASR_BAD_ALIGN.  The offsets are device data, which the library does not read on the host: an utterance
+ * with a negative offset comes back NaN, nothing before wave is read.  Other arguments, rejections and launches as
+ * b200asr_stft_features_ex. */
+int b200asr_stft_features_packed(const float* wave, const long long* offsets, const int* lens, float* out, int* frames_out,
+                                 void* ws, int B, int Lmax, int Tmax, int n_fft, int hop, int pad_reflect, int normalize,
+                                 int window, int window_periodic, const float* noise_bank, long long noise_bank_len,
+                                 const long long* noise_start, const float* noise_level, int max_frames, int precision,
+                                 b200asr_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Edit counts of the training loop's CER / WER (trainer/asr/trainer.py:60-79, 96-104 and 153-182), with no host read per
