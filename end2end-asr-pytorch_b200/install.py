@@ -20,7 +20,9 @@ original(AudioDataLoader, "__iter__").
 
 Data-parallel training: when the environment of `python -m b200asr.launch` describes more than one rank (WORLD_SIZE > 1),
 or `process_group=` is passed, install() joins that process group and the bound Trainer.train trains across it
-(trainer.trainer_train, parallel.join).  Otherwise nothing about a single process changes.
+(trainer.trainer_train, parallel.join).  The bound Transformer.evaluate in eval mode then decodes across it too: each rank
+decodes its share of the batch and every rank returns the whole batch's strings (modules.evaluate_sharded), so test.py
+runs data-parallel under the launcher.  Otherwise nothing about a single process changes.
 """
 from __future__ import annotations
 

@@ -1,6 +1,8 @@
-"""Data-parallel launcher for the reference's train.py: one process per GPU, in place of `--parallel` (nn.DataParallel).
+"""Data-parallel launcher for the reference's train.py and test.py: one process per GPU, in place of `--parallel`
+(nn.DataParallel).
 
-    python -m b200asr.launch train.py <train.py flags> [--parallel] [--device-ids 0 1 ...]
+    python -m b200asr.launch [--quiet-ranks[=DIR]] train.py <train.py flags> [--parallel] [--device-ids 0 1 ...]
+    python -m b200asr.launch [--quiet-ranks[=DIR]] test.py <test.py flags> [--device-ids 0 1 ...]
 
 One child per entry of `--device-ids` (ids of the GPUs this process sees), or one per visible GPU without the flag.  Each
 child sees only its own GPU (CUDA_VISIBLE_DEVICES), so train.py's `model.cuda(0)` and the trainer's `src.cuda()` land on
@@ -12,6 +14,10 @@ Ranks > 0 run with `--name <name>.rank<r>` (the reference's default name is `mod
 `log/<name>` in truncating mode before anything else, so ranks sharing one name would truncate and overwrite each
 other's lines.  Rank 0 keeps the name, and only rank 0 saves checkpoints (to `<save-folder>/<name>`) and writes the
 training loop's log lines; a rank > 0's own log holds what train.py itself logs before the loop.
+
+--quiet-ranks (an option of the launcher, before the script) keeps ranks > 0 off the terminal: the stdout and stderr of
+rank r > 0 go to DIR/launch.rank<r>.log (DIR defaults to the current directory), and the launcher names those files when
+it ends.  test.py prints its progress bar and results on every rank; with the flag only rank 0's reach the terminal.
 
 The launcher waits for every child.  When one fails, it terminates the others and exits with that child's code (128 + the
 signal number for a child killed by a signal); on SIGINT / SIGTERM it terminates them all.  No child outlives it.
@@ -128,6 +134,26 @@ def plan(argv, env=None):
     return [[args[0]] + rank_name_args(args[1:], r) for r in range(world)], envs
 
 
+def launcher_options(argv):
+    """(directory for the output of ranks > 0, or None to leave it on the terminal; argv from the script on).  The
+    launcher's own options come before the script: --quiet-ranks (the current directory) or --quiet-ranks=DIR."""
+    quiet, i = None, 0
+    while i < len(argv) and argv[i].startswith("-"):
+        a = argv[i]
+        if a == "--quiet-ranks":
+            quiet = "."
+        elif a.startswith("--quiet-ranks="):
+            quiet = a.split("=", 1)[1] or "."
+        else:
+            raise ValueError(f"unknown launcher option {a!r}; usage: python -m b200asr.launch [--quiet-ranks[=DIR]] SCRIPT [ARGS...]")
+        i += 1
+    return quiet, argv[i:]
+
+
+def rank_log_path(directory, rank: int) -> str:
+    return os.path.join(directory, f"launch.rank{rank}.log")
+
+
 def _exit_code(rc: int) -> int:
     return 128 - rc if rc < 0 else rc
 
@@ -147,9 +173,11 @@ def _stop(procs):
 
 
 def run(argv, env=None, poll=0.1) -> int:
-    """Start the children, wait for them; the exit code of the launcher."""
+    """Start the children, wait for them; the exit code of the launcher.  argv: the launcher's options, the script and its
+    arguments."""
+    quiet, argv = launcher_options(argv)
     args, envs = plan(argv, env)
-    procs = []
+    procs, logs = [], []
 
     def on_signal(signum, frame):
         raise KeyboardInterrupt
@@ -158,8 +186,15 @@ def run(argv, env=None, poll=0.1) -> int:
     if threading.current_thread() is threading.main_thread():
         old[signal.SIGTERM] = signal.signal(signal.SIGTERM, on_signal)
     try:
-        for a, e in zip(args, envs):
-            procs.append(subprocess.Popen([sys.executable] + a, env=e))
+        if quiet is not None and len(args) > 1:
+            os.makedirs(quiet, exist_ok=True)
+        for rank, (a, e) in enumerate(zip(args, envs)):
+            out = None
+            if quiet is not None and rank > 0:
+                out = open(rank_log_path(quiet, rank), "w")
+                logs.append(out)
+            procs.append(subprocess.Popen([sys.executable] + a, env=e, stdout=out,
+                                          stderr=subprocess.STDOUT if out is not None else None))
         while True:
             codes = [p.poll() for p in procs]
             failed = [c for c in codes if c not in (None, 0)]
@@ -174,6 +209,10 @@ def run(argv, env=None, poll=0.1) -> int:
         return 130
     finally:
         _stop(procs)
+        for f in logs:
+            f.close()
+        if logs:
+            print("b200asr.launch: the output of ranks > 0 is in " + ", ".join(f.name for f in logs), file=sys.stderr)
         for s, h in old.items():
             signal.signal(s, h)
 

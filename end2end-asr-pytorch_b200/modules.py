@@ -22,7 +22,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, parallel
 
 PAD_TOKEN, SOS_TOKEN, EOS_TOKEN = 0, 1, 2     # utils/constant.py:102-104
 
@@ -400,7 +400,13 @@ def beam_search(self, encoder_padded_outputs, beam_width=2, nbest=5, lm_rescorin
                    lm_weight=lm_weight, c_weight=c_weight, prob_weight=prob_weight)
     ids, lengths, _, _ = beam_decode(self, encoder_padded_outputs, beam_width, nbest=nbest, c_weight=c_weight, steps=300,
                                      lm=lm if lm_rescoring else None, lm_weight=lm_weight)
-    both = torch.cat([lengths.unsqueeze(-1), ids], dim=-1).cpu()
+    return beam_strings(torch.cat([lengths.unsqueeze(-1), ids], dim=-1).cpu(), self.id2label)
+
+
+def beam_strings(both, id2label):
+    """The flat yseq and string lists of Decoder.beam_search from host rows `both` [B, nbest, 1 + S + 2] int64: per
+    hypothesis its length n (0: none), then its yseq (SOS ... EOS) padded with -1.  The string of a yseq is "".join of
+    id2label over yseq[1:]; utterances and their hypotheses in order, none for an empty slot."""
     ys, strs = [], []
     for b in range(both.shape[0]):
         for i in range(both.shape[1]):
@@ -409,7 +415,7 @@ def beam_search(self, encoder_padded_outputs, beam_width=2, nbest=5, lm_rescorin
                 continue
             y = both[b, i, 1:1 + n].tolist()
             ys.append(y)
-            strs.append("".join(self.id2label[t] for t in y[1:]))
+            strs.append("".join(id2label[t] for t in y[1:]))
     return ys, strs
 
 
@@ -457,11 +463,15 @@ def greedy_search(self, encoder_padded_outputs, beam_width=2, lm_rescoring=False
         ref = _reference_method(self, "greedy_search", "with lm_rescoring=True or in training mode")
         return ref(self, encoder_padded_outputs, beam_width=beam_width, lm_rescoring=lm_rescoring, lm=lm, lm_weight=lm_weight,
                    c_weight=c_weight)
+    _check_greedy_positions(self)
+    ids = greedy_decode_cached(self, encoder_padded_outputs, steps=GREEDY_STEPS, stop_at_eos=True).cpu()
+    return greedy_strings(ids.tolist(), self.id2label)
+
+
+def _check_greedy_positions(self):
     if int(self.trg_max_length) < GREEDY_STEPS:
         raise ValueError(f"greedy search decodes {GREEDY_STEPS} positions but the decoder's positional table covers "
                          f"trg_max_length={self.trg_max_length}: build the model with tgt_max_len >= {GREEDY_STEPS}")
-    ids = greedy_decode_cached(self, encoder_padded_outputs, steps=GREEDY_STEPS, stop_at_eos=True).cpu()
-    return greedy_strings(ids.tolist(), self.id2label)
 
 
 # ------------------------------------------------------------------------------------------------ LM rescoring
@@ -645,7 +655,10 @@ def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_
     Decoder.greedy_search.  The reference's teacher-forced decoder pass and its topk (:107-108) only serve to produce `gold`
     and are skipped: gold comes from ops.preprocess_targets (raising like the reference for a target longer than
     tgt_max_len) in one device-to-host copy, and strs_gold joins id2label over all tgt_max_len entries, PAD included (:110).
-    A model in training mode runs the reference's own method."""
+    A model in training mode runs the reference's own method.
+
+    In a process that has joined a data-parallel group (parallel.join, as install() does under b200asr.launch) each rank
+    decodes its share of the batch and every rank returns the strings of the whole batch (evaluate_sharded)."""
     if self.training:
         ref = _reference_method(self, "evaluate", "in training mode")
         return ref(self, padded_input, input_lengths, padded_target, beam_search=beam_search, beam_width=beam_width,
@@ -653,11 +666,33 @@ def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_
                    verbose=verbose)
     ops._need_cuda(padded_input, padded_target)
     dec = self.decoder
+    group = parallel.joined()
+    if group is not None and not (beam_search and lm_rescoring and lstm_lm_parts(lm) is None):
+        strs_hyps, strs_gold = evaluate_sharded(self, group, padded_input, input_lengths, padded_target, beam_search,
+                                                beam_width, lm if lm_rescoring else None, lm_weight, c_weight)
+    else:
+        strs_hyps, strs_gold = _evaluate_whole(self, padded_input, input_lengths, padded_target, beam_search, beam_width, lm,
+                                               lm_rescoring, lm_weight, c_weight)
+    if verbose:
+        print("GOLD", strs_gold)
+        print("HYP", strs_hyps)
+    n = len(dec.layers)
+    return [[None] * n, [None] * n], strs_hyps, strs_gold
+
+
+def _gold_strings(self, padded_target):
+    _, gold, _, _ = ops.preprocess_targets(padded_target, int(self.decoder.trg_max_length))
+    return ["".join([self.id2label[x] for x in g]) for g in gold.cpu().tolist()]
+
+
+def _evaluate_whole(self, padded_input, input_lengths, padded_target, beam_search, beam_width, lm, lm_rescoring, lm_weight,
+                    c_weight):
+    """(strs_hyps, strs_gold) of the whole batch in this process."""
+    dec = self.decoder
     with torch.no_grad():
         feats, cf = _front_end(self, padded_input)
         enc = _encoder_body(self.encoder, feats, input_lengths, cf)
-        _, gold, _, _ = ops.preprocess_targets(padded_target, int(dec.trg_max_length))
-        strs_gold = ["".join([self.id2label[x] for x in g]) for g in gold.cpu().tolist()]
+        strs_gold = _gold_strings(self, padded_target)
         B = enc.shape[0]
         if beam_search:
             _, strs_hyps = dec.beam_search(enc, beam_width=beam_width, nbest=1, lm=lm, lm_rescoring=lm_rescoring,
@@ -667,11 +702,70 @@ def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_
                 strs_hyps = dec.greedy_search(enc)
         else:
             strs_hyps = dec.greedy_search(enc)
-    if verbose:
-        print("GOLD", strs_gold)
-        print("HYP", strs_hyps)
-    n = len(dec.layers)
-    return [[None] * n, [None] * n], strs_hyps, strs_gold
+    return strs_hyps, strs_gold
+
+
+def encoded_frames(self, T: int) -> int:
+    """Frames the front end makes of T input frames: the encoder's output length (T_e), from the shapes of the layers in
+    self.conv alone (Conv2d / MaxPool2d along the time axis, the last one)."""
+    if self.feat_extractor not in ("vgg_cnn", "emb_cnn"):
+        return int(T)
+    from torch.nn.modules.utils import _pair
+    for m in self.conv:
+        if isinstance(m, (nn.Conv2d, nn.MaxPool2d)):
+            k, s, p, d = (_pair(m.kernel_size)[1], _pair(m.stride)[1], _pair(m.padding)[1], _pair(m.dilation)[1])
+            T = (T + 2 * p - d * (k - 1) - 1) // s + 1
+    return int(T)
+
+
+def evaluate_sharded(self, group, padded_input, input_lengths, padded_target, beam_search=False, beam_width=0, lm=None,
+                     lm_weight=0.1, c_weight=1):
+    """(strs_hyps, strs_gold) of the whole batch, with this rank decoding utterances rank, rank + N, ... of it (group =
+    (process group, rank, N) as parallel.joined() returns it).  The batch is sorted by length and a shard decodes until its
+    slowest utterance ends, so a strided share gives every rank a similar mix where contiguous chunks would leave rank 0
+    the longest utterances.  The front end and the encoder run on the shard at the batch's padded T; the gold strings come
+    from the whole padded_target on every rank; the decode and the string assembly are decode_sharded's."""
+    _, rank, world = group
+    B = padded_input.shape[0]
+    with torch.no_grad():
+        strs_gold = _gold_strings(self, padded_target)
+        enc = None
+        if rank < B:
+            rows = slice(rank, B, world)
+            feats, cf = _front_end(self, padded_input[rows].contiguous())
+            enc = _encoder_body(self.encoder, feats, input_lengths[rows].contiguous(), cf)
+        Te = encoded_frames(self, padded_input.shape[-1])
+        strs_hyps = decode_sharded(self.decoder, enc, B, Te, group, beam_search, beam_width, lm, lm_weight, c_weight)
+    return strs_hyps, strs_gold
+
+
+def decode_sharded(dec, enc, B, Te, group, beam_search=False, beam_width=0, lm=None, lm_weight=0.1, c_weight=1):
+    """The strings of Transformer.evaluate's decode (transformer.py:112-118) for a batch of B utterances of which this rank
+    holds the encoder outputs of rank, rank + N, ... (`enc`, None for an empty share; T_e frames).  Every rank returns the
+    B strings in batch order.
+
+    Greedy: greedy_decode_cached(300 steps, EOS stop on the device) on the share, one all-gather of the ids
+    (parallel.gather_rows), greedy_strings.  Beam: beam_decode(nbest=1, LSTM LM rescoring when `lm` is given) on the share,
+    one all-gather of [length | yseq] rows; an utterance of any rank that ended no hypothesis makes every rank print
+    ">>>>>>> switch to greedy" and take the greedy path on its share, as one process does for the whole batch.  A rank with
+    an empty share launches no kernel and joins every collective.  The positional-table checks run on every rank before
+    the first collective, so every rank raises alike."""
+    pg = group[0]
+    if beam_search:
+        _check_beam_positions(dec, Te, GREEDY_STEPS)
+        S = min(GREEDY_STEPS, int(Te))
+        rows = None
+        if enc is not None:
+            ids, lengths, _, _ = beam_decode(dec, enc, beam_width, nbest=1, c_weight=c_weight, steps=GREEDY_STEPS, lm=lm,
+                                             lm_weight=lm_weight)
+            rows = torch.cat([lengths.unsqueeze(-1), ids], dim=-1)
+        both = parallel.gather_rows(rows, B, (1, S + 3), pg)
+        if bool((both[:, 0, 0] > 0).all()):
+            return beam_strings(both, dec.id2label)[1]
+        print(">>>>>>> switch to greedy")
+    _check_greedy_positions(dec)
+    ids = greedy_decode_cached(dec, enc, steps=GREEDY_STEPS, stop_at_eos=True) if enc is not None else None
+    return greedy_strings(parallel.gather_rows(ids, B, (GREEDY_STEPS,), pg).tolist(), dec.id2label)
 
 
 # ------------------------------------------------------------------------------------------------ mirror classes

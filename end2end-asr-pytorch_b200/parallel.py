@@ -5,6 +5,10 @@ strategy of SURVEY.md §5.8: each rank runs forward/backward on its shard of the
 UN-normalised token-loss sum, the flat gradient buffer (+ [sum-loss, n_tokens]) is all-reduced once over
 NCCL/NVLink, and the optimizer divides by the GLOBAL token count -- exactly the reference's normalisation over the
 gathered global batch (trainer.py:84 + metrics.py:127-130).
+
+Evaluation shards the same way by utterance, strided instead of chunked: each rank decodes utterances r, r + N, ... of
+the batch and one all-gather of fixed-shape id rows (gather_rows) gives every rank the whole batch's result
+(modules.evaluate_sharded).
 """
 from __future__ import annotations
 
@@ -31,7 +35,7 @@ def shard_batch(src, lengths, tgt, rank: int, world: int):
 
 
 BACKEND_ENV = "B200ASR_DIST_BACKEND"      # set by b200asr.launch: "nccl", or "gloo" when two ranks share a GPU
-_group = None                             # (process group, rank, world size) the bound Trainer.train trains across
+_group = None                             # (process group, rank, world size) the bound Trainer.train and evaluate run across
 
 
 def join(process_group=None):
@@ -58,7 +62,7 @@ def leave():
 
 
 def joined():
-    """(group, rank, world) the bound Trainer.train trains across, or None."""
+    """(group, rank, world) the bound Trainer.train trains across and the bound Transformer.evaluate decodes across, or None."""
     return _group
 
 
@@ -69,6 +73,36 @@ def shard_range(B: int, rank: int, world: int):
         raise ValueError(f"shard_range: rank {rank} of world {world}")
     n = -(-B // world)
     return min(B, rank * n), min(B, (rank + 1) * n)
+
+
+def _collective_device(process_group=None):
+    """Where a collective's tensors live: the current GPU under NCCL, the host under gloo."""
+    if dist.get_backend(process_group) == "nccl":
+        return torch.device("cuda", torch.cuda.current_device())
+    return torch.device("cpu")
+
+
+def gather_rows(rows, B: int, shape, process_group=None):
+    """Every rank's rows of a batch of B utterances, in batch order, as one host tensor [B, *shape] int64.
+
+    Rank r holds the rows of utterances r, r + N, r + 2N, ... (`rows` [len(range(r, B, N)), *shape] int64 on any device, or
+    None when it holds none).  ONE all-gather of a fixed block [ceil(B / N), *shape] per rank, padded with -1: on the device
+    under NCCL, on the host under gloo.  Row j of rank r's block is utterance j * N + r, so the gathered blocks interleave
+    into batch order."""
+    world = dist.get_world_size(process_group)
+    rank = dist.get_rank(process_group)
+    n = -(-B // world)
+    dev = _collective_device(process_group)
+    block = torch.full((n,) + tuple(shape), -1, dtype=torch.int64, device=dev)
+    mine = len(range(rank, B, world))
+    if mine:
+        if rows is None or tuple(rows.shape) != (mine,) + tuple(shape):
+            raise ValueError(f"gather_rows: rank {rank} of {world} holds {mine} of {B} rows of shape {tuple(shape)}, "
+                             f"got {None if rows is None else tuple(rows.shape)}")
+        block[:mine] = rows.to(device=dev, dtype=torch.int64)
+    parts = [torch.empty_like(block) for _ in range(world)]
+    dist.all_gather(parts, block, group=process_group)
+    return torch.stack(parts, dim=1).reshape((n * world,) + tuple(shape))[:B].cpu()
 
 
 def broadcast_params(flat, process_group=None):
@@ -101,8 +135,7 @@ def seed_host_rngs(process_group=None):
     the same seed every rank's loader yields the same global batches, of which each rank then trains its own chunk.
     Returns the seed."""
     src = dist.get_global_rank(process_group, 0) if process_group is not None else 0
-    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(process_group) == "nccl" else torch.device("cpu")
-    seed = torch.tensor([random.getrandbits(62)], dtype=torch.int64, device=dev)
+    seed = torch.tensor([random.getrandbits(62)], dtype=torch.int64, device=_collective_device(process_group))
     dist.broadcast(seed, src=src, group=process_group)
     s = int(seed.item())
     random.seed(s)
