@@ -11,11 +11,11 @@ from .install import install, original, uninstall
 from .metrics import LabelTable, calculate_loss, calculate_metrics, edit_counts, loss_and_stats
 from .modules import (LM, Decoder, DecoderLayer, Encoder, EncoderLayer, MultiHeadAttention, PositionalEncoding,
                       PositionwiseFeedForwardWithConv, RNNModel, ScaledDotProductAttention, Transformer, build_model)
-from .ops import config as precision, manual_seed
+from .ops import attention_maps, config as precision, manual_seed
 from .optim import FlatParams, FusedAdam, NoamOpt, adam_step, clip_grad_norm_
 from .parallel import DataParallelStep, HostBatchPrefetcher, shard_batch
 
 __all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "original", "calculate_loss", "calculate_metrics",
            "loss_and_stats", "LabelTable", "edit_counts","Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
            "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model", "RNNModel", "LM",
-           "precision", "manual_seed", "spectrogram_batch", "NoiseBank", "NoiseClips", "collate_waves", "stft_features_packed","FlatParams", "FusedAdam", "NoamOpt", "adam_step", "clip_grad_norm_", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]
+           "precision", "manual_seed", "attention_maps", "spectrogram_batch", "NoiseBank", "NoiseClips", "collate_waves", "stft_features_packed","FlatParams", "FusedAdam", "NoamOpt", "adam_step", "clip_grad_norm_", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]

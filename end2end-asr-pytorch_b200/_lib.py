@@ -46,6 +46,8 @@ SIGNATURES = {
                                [_f, _f, _u64, _u64, _vp]),
     "b200asr_sdpa_fused_bwd": (_i, [_vp] * 6 + [_ll] * 12 + [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp] + [_i] * 6 +
                                [_f, _f, _u64, _u64, _vp]),
+    "b200asr_sdpa_probs": (_i, [_vp, _vp] + [_ll] * 6 + [_vp, _vp, _i, _vp, _vp, _ll, _ll, _ll] + [_i] * 5 +
+                           [_f, _f, _u64, _u64, _i, _vp]),
     "b200asr_sdpa_mat_ws_bytes": (_sz, [_i, _i, _i, _i]),
     "b200asr_sdpa_mat_fwd": (_i, [_vp, _vp, _vp] + [_ll] * 9 + [_vp, _vp, _i, _vp, _ll, _ll, _ll, _vp, _vp] + [_i] * 6 +
                              [_f, _f, _u64, _u64, _i, _vp]),

@@ -26,5 +26,8 @@ int sdpa_fwd_tc(const AttnP& p, cudaStream_t st);
 int sdpa_bwd_tc(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st);
 int sdpa_fused_fwd_tc(const AttnP& p, cudaStream_t st);
 int sdpa_fused_bwd_tc(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st);
+// attention probabilities from the forward's log-sum-exp (p.lse), written through p.o / o_bs / o_hs / o_rs
+int sdpa_probs_simt(const AttnP& p, cudaStream_t st);
+int sdpa_probs_tc(const AttnP& p, int mode, cudaStream_t st);    // mode 1 = TF32, 6 = bf16x3
 
 }  // namespace b200asr

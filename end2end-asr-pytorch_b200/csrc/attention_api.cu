@@ -1,4 +1,4 @@
-// b200asr_sdpa_fwd / _bwd and b200asr_sdpa_fused_fwd / _bwd: argument checking and precision dispatch.
+// b200asr_sdpa_fwd / _bwd, b200asr_sdpa_fused_fwd / _bwd and b200asr_sdpa_probs: argument checking and precision dispatch.
 #include "../../include/b200asr.h"
 #include "attention.h"
 #include "common.cuh"
@@ -102,6 +102,32 @@ int b200asr_sdpa_fused_bwd(const float* dout, const float* q, const float* k, co
   if (rc) return rc;
   float* delta = (float*)((uint16_t*)ws_bwd + 2 * ws16_elems(B, H, Tq));
   return sdpa_fused_bwd_tc(p, dout, dq, dk_out, dv_out, delta, (cudaStream_t)stream);
+}
+
+int b200asr_sdpa_probs(const float* q, const float* k, long long q_bs, long long q_hs, long long q_rs, long long k_bs,
+                       long long k_hs, long long k_rs, const uint8_t* key_pad, const uint8_t* dense_mask, int causal,
+                       const float* lse, float* probs, long long p_bs, long long p_hs, long long p_rs, int B, int H, int Tq,
+                       int Tk, int dk, float scale, float p_drop, uint64_t seed, uint64_t offset, int precision,
+                       b200asr_stream_t stream) {
+  B200_REQUIRE(q && k && lse && probs, B200ASR_BAD_ARG, "sdpa_probs: null pointer");
+  B200_REQUIRE(B > 0 && H > 0 && Tq > 0 && Tk > 0, B200ASR_BAD_SHAPE, "sdpa_probs: empty problem B=%d H=%d Tq=%d Tk=%d", B, H, Tq, Tk);
+  B200_REQUIRE(q_rs % 4 == 0 && k_rs % 4 == 0 && q_bs % 4 == 0 && q_hs % 4 == 0 && k_bs % 4 == 0 && k_hs % 4 == 0,
+               B200ASR_BAD_ALIGN, "sdpa_probs: q/k strides must be multiples of 4 elements");
+  B200_REQUIRE(aligned16(q) && aligned16(k) && ((uintptr_t)probs & 3u) == 0, B200ASR_BAD_ALIGN, "sdpa_probs: pointer alignment");
+  B200_REQUIRE(p_drop >= 0.f && p_drop < 1.f, B200ASR_BAD_ARG, "sdpa_probs: p_drop=%f", p_drop);
+  AttnP p{};
+  p.q = q; p.k = k; p.o = probs; p.lse = const_cast<float*>(lse);
+  p.q_bs = q_bs; p.q_hs = q_hs; p.q_rs = q_rs; p.k_bs = k_bs; p.k_hs = k_hs; p.k_rs = k_rs;
+  p.o_bs = p_bs; p.o_hs = p_hs; p.o_rs = p_rs;
+  p.key_pad = key_pad; p.dense = dense_mask; p.causal = causal;
+  p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk; p.dk = dk; p.dv = 0; p.scale = scale;
+  p.thresh = p_drop > 0.f ? dropout_thresh16(p_drop) : 0u;
+  p.inv_keep = dropout_inv_keep(p_drop);
+  p.key = dropout_key(seed, offset);
+  if (precision == B200ASR_PREC_FP32) return sdpa_probs_simt(p, (cudaStream_t)stream);
+  if (precision == B200ASR_PREC_TF32 || precision == B200ASR_PREC_BF16X3) return sdpa_probs_tc(p, precision, (cudaStream_t)stream);
+  set_error("sdpa_probs: precision %d has no flash forward to match (0 = fp32, 1 = TF32, 6 = bf16x3)", precision);
+  return B200ASR_BAD_SHAPE;
 }
 
 }  // extern "C"

@@ -47,6 +47,28 @@ __device__ __forceinline__ bool is_masked(const AttnP& p, int b, int q, int key)
   return false;
 }
 
+// unscaled scores of a 64x64 tile: s[i][j] = Q row ty+16i . K row tx+16j over dk columns (the forward's and
+// sdpa_probs_simt_kernel's arithmetic, so the probabilities rebuilt from the log-sum-exp match the forward's)
+__device__ __forceinline__ void score_tile(const float* __restrict__ Qs, const float* __restrict__ Ks, int LQ, int dk, int tx,
+                                           int ty, float (&s)[4][4]) {
+#pragma unroll
+  for (int i = 0; i < 4; i++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) s[i][j] = 0.f;
+  for (int kk = 0; kk < dk; kk += 4) {
+    float4 a[4], bb[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) a[i] = *reinterpret_cast<const float4*>(Qs + (ty + 16 * i) * LQ + kk);
+#pragma unroll
+    for (int j = 0; j < 4; j++) bb[j] = *reinterpret_cast<const float4*>(Ks + (tx + 16 * j) * LQ + kk);
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+      for (int j = 0; j < 4; j++)
+        s[i][j] += a[i].x * bb[j].x + a[i].y * bb[j].y + a[i].z * bb[j].z + a[i].w * bb[j].w;
+  }
+}
+
 template <int DV>
 __global__ void __launch_bounds__(256) sdpa_fwd_simt_kernel(AttnP p) {
   extern __shared__ __align__(16) float smem[];
@@ -78,22 +100,7 @@ __global__ void __launch_bounds__(256) sdpa_fwd_simt_kernel(AttnP p) {
     load_tile(Vs, LV, vg, p.v_rs, k0, p.Tk, DV, tid);
     __syncthreads();
     float s[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-      for (int j = 0; j < 4; j++) s[i][j] = 0.f;
-    for (int kk = 0; kk < dk; kk += 4) {
-      float4 a[4], bb[4];
-#pragma unroll
-      for (int i = 0; i < 4; i++) a[i] = *reinterpret_cast<const float4*>(Qs + (ty + 16 * i) * LQ + kk);
-#pragma unroll
-      for (int j = 0; j < 4; j++) bb[j] = *reinterpret_cast<const float4*>(Ks + (tx + 16 * j) * LQ + kk);
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-          s[i][j] += a[i].x * bb[j].x + a[i].y * bb[j].y + a[i].z * bb[j].z + a[i].w * bb[j].w;
-    }
+    score_tile(Qs, Ks, LQ, dk, tx, ty, s);
 #pragma unroll
     for (int i = 0; i < 4; i++) {
       const int q = q0 + ty + 16 * i;
@@ -150,6 +157,70 @@ __global__ void __launch_bounds__(256) sdpa_fwd_simt_kernel(AttnP p) {
     // a fully masked row's log-sum-exp is NaN, as the tensor-core kernels write it; the backward reads it as "dead row"
     if (tx == 0 && p.lse) p.lse[((size_t)b * p.H + h) * p.Tq + q] = m[i] == -INFINITY ? NAN : m[i] + logf(l[i]);
   }
+}
+
+// The probabilities the forward multiplied into V, rebuilt from Q, K and its log-sum-exp: P = expf(scale * S - lse) with
+// the masks and the forward's dropout mask (times inv_keep) applied; masked keys are 0, a fully masked row (lse NaN) is
+// NaN.  Written through p.o with the strides p.o_bs / o_hs / o_rs (any row stride), staged in shared memory per 64x64
+// tile so that the stores go out as whole rows.
+__global__ void __launch_bounds__(256) sdpa_probs_simt_kernel(AttnP p) {
+  griddep_launch();      // programmatic dependent launch (common.cuh)
+  griddep_wait();
+  extern __shared__ __align__(16) float smem[];
+  const int dk = p.dk, LQ = dk + 4;
+  float* Qs = smem;
+  float* Ks = Qs + 64 * LQ;
+  float* Ps = Ks + 64 * LQ;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int q0 = blockIdx.x * TQ, h = blockIdx.y, b = blockIdx.z;
+  const float* kg = p.k + b * p.k_bs + h * p.k_hs;
+  float* og = p.o + b * p.o_bs + h * p.o_hs;
+  load_tile(Qs, LQ, p.q + b * p.q_bs + h * p.q_hs, p.q_rs, q0, p.Tq, dk, tid);
+  const size_t row_base = ((size_t)b * p.H + h) * p.Tq;
+  float lse[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) lse[i] = q0 + ty + 16 * i < p.Tq ? p.lse[row_base + q0 + ty + 16 * i] : 0.f;
+
+  for (int k0 = 0; k0 < p.Tk; k0 += TKT) {
+    const bool past = p.causal && k0 > q0 + TQ - 1;      // every key of the tile is masked for every query
+    __syncthreads();
+    if (!past) load_tile(Ks, LQ, kg, p.k_rs, k0, p.Tk, dk, tid);
+    __syncthreads();
+    float s[4][4];
+    if (!past) score_tile(Qs, Ks, LQ, dk, tx, ty, s);
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const int q = q0 + ty + 16 * i;
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int key = k0 + tx + 16 * j;
+        float pr = 0.f;
+        if (isnan(lse[i])) {
+          pr = NAN;
+        } else if (!past && !is_masked(p, b, q, key)) {
+          pr = expf(s[i][j] * p.scale - lse[i]);
+          if (p.thresh) pr = dropout_keep(p.key, (row_base + q) * p.Tk + key, p.thresh) ? pr * p.inv_keep : 0.f;
+        }
+        Ps[(ty + 16 * i) * LP + tx + 16 * j] = pr;
+      }
+    }
+    __syncthreads();
+    const int nk = min(TKT, p.Tk - k0);
+    for (int idx = tid; idx < TQ * TKT; idx += 256) {
+      const int r = idx / TKT, c = idx % TKT;
+      if (q0 + r < p.Tq && c < nk) og[(long long)(q0 + r) * p.o_rs + k0 + c] = Ps[r * LP + c];
+    }
+  }
+}
+
+int sdpa_probs_simt(const AttnP& p, cudaStream_t st) {
+  B200_REQUIRE(p.dk == 16 || p.dk == 32 || p.dk == 64 || p.dk == 128, B200ASR_BAD_SHAPE, "sdpa_probs (fp32): dk=%d unsupported (16/32/64/128)", p.dk);
+  constexpr int smem_max = (int)sizeof(float) * (64 * (128 + 4) * 2 + 64 * LP);      // dk = 128
+  const int smem = (int)sizeof(float) * (64 * (p.dk + 4) * 2 + 64 * LP);
+  static bool attr_set[kMaxDevices] = {};
+  if (int rc = ensure_dynamic_smem((const void*)sdpa_probs_simt_kernel, smem_max, attr_set, "sdpa_probs_simt")) return rc;
+  launch_pdl(sdpa_probs_simt_kernel, dim3(ceil_div(p.Tq, TQ), p.H, p.B), dim3(256), (size_t)smem, st, p);
+  return check_launch("sdpa_probs_simt");
 }
 
 // delta[b,h,q] = sum_c dO*O ; also zero dq (strided) for the atomics of the main backward kernel

@@ -140,6 +140,21 @@ __device__ __forceinline__ bool fl_masked(const AttnP& p, const uint8_t* pad, in
   return p.dense && p.dense[((size_t)b * p.Tq + qi) * p.Tk + key] != 0;
 }
 
+// unscaled scores S = Q K^T of a warp's 16 queries (A fragments qf) against the 64 keys staged in sK, as 8 C blocks of 8
+// keys: the forward's arithmetic, which flash_probs_kernel repeats so that its probabilities match the log-sum-exp
+template <int MODE, int DK>
+__device__ __forceinline__ void fl_scores(float (&s)[8][4], const typename Fl<MODE>::A (&qf)[DK / Fl<MODE>::KS], const float* sK,
+                                          int g, int q) {
+  using F = Fl<MODE>;
+  constexpr int PK = DK + 4, KS = F::KS;
+#pragma unroll
+  for (int nb = 0; nb < 8; nb++) s[nb][0] = s[nb][1] = s[nb][2] = s[nb][3] = 0.f;
+#pragma unroll
+  for (int ks = 0; ks < DK / KS; ks++)
+#pragma unroll
+    for (int nb = 0; nb < 8; nb++) F::mma(s[nb], qf[ks], F::b_feat(sK, PK, nb * 8, ks * KS, g, q));
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 template <int MODE, int DK, int DV>
 __global__ void __launch_bounds__(FL_THREADS)
@@ -177,12 +192,7 @@ flash_fwd_kernel(const AttnP p) {
     }
     __syncthreads();
     float s[8][4];
-#pragma unroll
-    for (int nb = 0; nb < 8; nb++) s[nb][0] = s[nb][1] = s[nb][2] = s[nb][3] = 0.f;
-#pragma unroll
-    for (int ks = 0; ks < DK / KS; ks++)
-#pragma unroll
-      for (int nb = 0; nb < 8; nb++) F::mma(s[nb], qf[ks], F::b_feat(sK, PK, nb * 8, ks * KS, g, q));
+    fl_scores<MODE, DK>(s, qf, sK, g, q);
     // scale + masks, block row max
     float bm0 = -INFINITY, bm1 = -INFINITY;
 #pragma unroll
@@ -233,6 +243,71 @@ flash_fwd_kernel(const AttnP p) {
   if (p.lse && q == 0) {
     if (qa < p.Tq) p.lse[bh * p.Tq + qa] = m0 == -INFINITY ? NAN : m0 + logf(l0);
     if (qb < p.Tq) p.lse[bh * p.Tq + qb] = m1 == -INFINITY ? NAN : m1 + logf(l1);
+  }
+}
+
+// The probabilities flash_fwd_kernel<MODE> multiplied into V, rebuilt from Q, K and its log-sum-exp as the backward does:
+// P = exp(scale * S - lse), masks, the forward's dropout mask (times inv_keep); masked keys 0, a fully masked row (lse NaN)
+// NaN.  CTA = (64-query tile, head, utterance) like the forward; each 64-key block is staged in shared memory and stored
+// as whole rows through p.o with the strides p.o_bs / o_hs / o_rs (any row stride).
+template <int MODE, int DK>
+__global__ void __launch_bounds__(FL_THREADS)
+flash_probs_kernel(const AttnP p) {
+  using F = Fl<MODE>;
+  constexpr int PK = DK + 4, PP = FL_ROWS + 4, KS = F::KS;
+  extern __shared__ float fl_smem[];
+  float* sQ = fl_smem;
+  float* sK = sQ + FL_ROWS * PK;
+  float* sP = sK + FL_ROWS * PK;
+  uint8_t* pad = reinterpret_cast<uint8_t*>(sP + FL_ROWS * PP);
+  griddep_launch();      // programmatic dependent launch (common.cuh)
+  griddep_wait();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const int q0 = blockIdx.x * FL_ROWS, h = blockIdx.y, b = blockIdx.z;
+  const int qa = q0 + warp * 16 + g, qb = qa + 8;
+  const size_t bh = (size_t)b * p.H + h;
+  const float lse_a = qa < p.Tq ? p.lse[bh * p.Tq + qa] : 0.f, lse_b = qb < p.Tq ? p.lse[bh * p.Tq + qb] : 0.f;
+  float* og = p.o + b * p.o_bs + h * p.o_hs;
+
+  fl_load_tile<DK>(sQ, p.q, p.q_bs, p.q_hs, p.q_rs, b, h, q0, p.Tq);
+  __syncthreads();
+  typename F::A qf[DK / KS];
+#pragma unroll
+  for (int ks = 0; ks < DK / KS; ks++) qf[ks] = F::a_feat(sQ, PK, warp * 16, ks * KS, g, q);
+
+  for (int k0 = 0; k0 < p.Tk; k0 += FL_ROWS) {
+    __syncthreads();                                       // previous block's stores are done
+    fl_load_tile<DK>(sK, p.k, p.k_bs, p.k_hs, p.k_rs, b, h, k0, p.Tk);
+    if (threadIdx.x < FL_ROWS) {
+      const int key = k0 + threadIdx.x;
+      pad[threadIdx.x] = (key >= p.Tk || (p.key_pad && p.key_pad[(size_t)b * p.Tk + key])) ? 1 : 0;
+    }
+    __syncthreads();
+    float s[8][4];
+    fl_scores<MODE, DK>(s, qf, sK, g, q);
+#pragma unroll
+    for (int nb = 0; nb < 8; nb++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) {
+        const int kl = nb * 8 + 2 * q + (e & 1), key = k0 + kl;
+        const bool r1 = (e & 2) != 0;
+        const int qi = r1 ? qb : qa;
+        const float lse = r1 ? lse_b : lse_a;
+        float pr = 0.f;
+        if (isnan(lse)) {
+          pr = NAN;
+        } else if (qi < p.Tq && !fl_masked(p, pad, b, qi, key, kl)) {
+          pr = __expf(s[nb][e] * p.scale - lse);
+          if (p.thresh) pr = dropout_keep(p.key, (bh * p.Tq + qi) * (size_t)p.Tk + key, p.thresh) ? pr * p.inv_keep : 0.f;
+        }
+        sP[(warp * 16 + g + (r1 ? 8 : 0)) * PP + kl] = pr;
+      }
+    __syncthreads();
+    const int nk = min(FL_ROWS, p.Tk - k0);
+    for (int i = threadIdx.x; i < FL_ROWS * FL_ROWS; i += FL_THREADS) {
+      const int r = i / FL_ROWS, c = i % FL_ROWS;
+      if (q0 + r < p.Tq && c < nk) og[(long long)(q0 + r) * p.o_rs + k0 + c] = sP[r * PP + c];
+    }
   }
 }
 
@@ -430,6 +505,17 @@ int flash_fwd(const AttnP& p, cudaStream_t st, const char* what) {
   return check_launch(what);
 }
 
+template <int DK> constexpr int flash_probs_smem() { return 4 * FL_ROWS * (2 * (DK + 4) + FL_ROWS + 4) + FL_ROWS; }
+
+template <int MODE, int DK>
+int flash_probs(const AttnP& p, cudaStream_t st, const char* what) {
+  auto* kern = flash_probs_kernel<MODE, DK>;
+  static bool attr_set[kMaxDevices] = {};
+  if (int rc = ensure_dynamic_smem((const void*)kern, flash_probs_smem<DK>(), attr_set, what)) return rc;
+  launch_pdl(kern, dim3(ceil_div(p.Tq, FL_ROWS), p.H, p.B), dim3(FL_THREADS), (size_t)flash_probs_smem<DK>(), st, p);
+  return check_launch(what);
+}
+
 // delta (B*H*Tq floats) is scratch
 template <int MODE, int DK, int DV>
 int flash_bwd(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st, const char* what) {
@@ -482,6 +568,18 @@ int sdpa_fused_fwd_tc(const AttnP& p, cudaStream_t st) {
   B200_REQUIRE(p.H <= 65535 && p.B <= 65535, B200ASR_BAD_SHAPE, "sdpa_fused: grid too large");
   B200_REQUIRE(p.Tk <= ATT_MAX_TK, B200ASR_BAD_SHAPE, "sdpa_fused_fwd: Tk=%d exceeds %d keys; use the materialised path", p.Tk, ATT_MAX_TK);
   return tc::flash_fwd<6, 64, 64>(p, st, "sdpa_fused_fwd");
+}
+
+// the probabilities of sdpa_fwd_tc (TF32: dk in {32, 64}) and sdpa_fused_fwd_tc (bf16x3: dk = 64), both Tk <= 448
+int sdpa_probs_tc(const AttnP& p, int mode, cudaStream_t st) {
+  using namespace tc;
+  B200_REQUIRE(p.Tk <= ATT_MAX_TK, B200ASR_BAD_SHAPE, "sdpa_probs (tensor cores): Tk=%d exceeds %d keys", p.Tk, ATT_MAX_TK);
+  B200_REQUIRE(p.H <= 65535 && p.B <= 65535, B200ASR_BAD_SHAPE, "sdpa_probs (tensor cores): grid too large");
+  if (mode == 1 && p.dk == 64) return flash_probs<1, 64>(p, st, "tc_sdpa_probs");
+  if (mode == 1 && p.dk == 32) return flash_probs<1, 32>(p, st, "tc_sdpa_probs");
+  if (mode == 6 && p.dk == 64) return flash_probs<6, 64>(p, st, "sdpa_fused_probs");
+  set_error("sdpa_probs (tensor cores): dk=%d unsupported in mode %d (TF32: dk in {32, 64}; bf16x3: dk = 64)", p.dk, mode);
+  return B200ASR_BAD_SHAPE;
 }
 
 int sdpa_fused_bwd_tc(const AttnP& p, const float* dout, float* dq, float* dk, float* dv, float* delta, cudaStream_t st) {

@@ -41,12 +41,22 @@ def _as_u8_mask(mask, B, Tq, Tk):
     return m.to(torch.uint8).contiguous()
 
 
-def _mha_core(self, query, key, value, key_pad=None, dense_mask=None, causal=False, row_scale=None):
+def _maps_sink():
+    """A list for the attention maps of a forward while ops.attention_maps is on, else None (no map is computed)."""
+    return [] if ops.attention_maps_enabled() else None
+
+
+def _first(maps):
+    return maps[0] if maps is not None else None
+
+
+def _mha_core(self, query, key, value, key_pad=None, dense_mask=None, causal=False, row_scale=None, maps=None):
     """MultiHeadAttention body (models/common_layers.py:170-200) on fused kernels.
 
     Q/K/V projections write token-major [B,T,H*d]; the attention kernel addresses heads through strides, so
     the permute/contiguous copies of :185-187 and :194-195 do not exist.  `row_scale` (the non-pad mask that the
-    layer applies right after, transformer.py:198/536/540) is folded into the LayerNorm epilogue."""
+    layer applies right after, transformer.py:198/536/540) is folded into the LayerNorm epilogue.  `maps`: a list that
+    receives the (H*B) x Tq x Tk attention map (ops.attention_probs), or None."""
     B, Tq, _ = query.shape
     Tk = key.shape[1]
     H, dk, dv = self.num_heads, self.dim_key, self.dim_value
@@ -59,12 +69,12 @@ def _mha_core(self, query, key, value, key_pad=None, dense_mask=None, causal=Fal
         # projections + attention as one autograd node: Q/K/V (or K/V) run as ONE GEMM when their weights lie back to back
         # in memory (optim.FlatParams), and the attention kernels address the packed output through strides
         o = ops.AttnProjFn.apply(query, key, ql.weight, ql.bias, kl.weight, kl.bias, vl.weight, vl.bias, H, dk, dv,
-                                 key_pad, dense_mask, causal, scale, p_attn, link)          # [B,Tq,H*dv], token-major
+                                 key_pad, dense_mask, causal, scale, p_attn, link, maps)    # [B,Tq,H*dv], token-major
     else:
         q = ops.LinearFn.apply(query, ql.weight, ql.bias).view(B, Tq, H, dk).permute(0, 2, 1, 3)
         k = ops.LinearFn.apply(key, kl.weight, kl.bias).view(B, Tk, H, dk).permute(0, 2, 1, 3)
         v = ops.LinearFn.apply(value, vl.weight, vl.bias).view(B, Tk, H, dv).permute(0, 2, 1, 3)
-        o = ops.SdpaFn.apply(q, k, v, key_pad, dense_mask, causal, scale, p_attn)         # (B,H,Tq,dv) view of [B,Tq,H,dv]
+        o = ops.SdpaFn.apply(q, k, v, key_pad, dense_mask, causal, scale, p_attn, False, maps)   # (B,H,Tq,dv) view of [B,Tq,H,dv]
         o = o.permute(0, 2, 1, 3).reshape(B, Tq, H * dv)                                  # free: memory is token-major
     o = ops.LinearFn.apply(o, self.output_linear.weight, self.output_linear.bias)
     ln = self.layer_norm
@@ -84,21 +94,24 @@ def sdpa_forward(self, q, k, v, mask=None):
     """ScaledDotProductAttention.forward(q, k, v, mask) -- models/common_layers.py:211-225.
     q,k,v are head-major (H*B) x T x d exactly as the reference passes them and `mask` is the (H*B) x Tq x Tk
     tensor MultiHeadAttention built with mask.repeat(H,1,1); each (h,b) slice is treated as its own batch entry.
-    Returns (output, None): attention probabilities are never materialised (every caller discards them)."""
+    Returns (output, attn): attn is the detached (H*B) x Tq x Tk probability map while ops.attention_maps is on, else None."""
     HB, Tq, dk = q.shape
     Tk, dv = k.shape[1], v.shape[2]
     dense = _as_u8_mask(mask, HB, Tq, Tk)
     as4 = lambda t: t.contiguous().unsqueeze(1)          # (HB,1,T,d): one "head" per batch entry
     p = float(self.dropout.p) if self.training else 0.0
-    o = ops.SdpaFn.apply(as4(q), as4(k), as4(v), None, dense, False, 1.0 / float(self.temperature), p)
-    return o.reshape(HB, Tq, dv), None
+    maps = _maps_sink()
+    o = ops.SdpaFn.apply(as4(q), as4(k), as4(v), None, dense, False, 1.0 / float(self.temperature), p, False, maps)
+    return o.reshape(HB, Tq, dv), _first(maps)
 
 
 def mha_forward(self, query, key, value, mask=None):
-    """MultiHeadAttention.forward(query, key, value, mask) -> (output, attn=None) -- common_layers.py:170-200."""
+    """MultiHeadAttention.forward(query, key, value, mask) -> (output, attn) -- common_layers.py:170-200; attn is the
+    (H*B) x Tq x Tk map while ops.attention_maps is on, else None."""
     B, Tq, _ = query.shape
     dense = _as_u8_mask(mask, B, Tq, key.shape[1])
-    return _mha_core(self, query, key, value, dense_mask=dense), None
+    maps = _maps_sink()
+    return _mha_core(self, query, key, value, dense_mask=dense, maps=maps), _first(maps)
 
 
 def ffn_forward(self, x):
@@ -107,29 +120,35 @@ def ffn_forward(self, x):
 
 
 def encoder_layer_forward(self, enc_input, non_pad_mask=None, self_attn_mask=None):
-    """EncoderLayer.forward -- models/asr/transformer.py:195-203 (dense-mask compatible signature)."""
+    """EncoderLayer.forward -- models/asr/transformer.py:195-203 (dense-mask compatible signature) -> (output, self_attn map
+    or None)."""
     B, T, _ = enc_input.shape
     rs = non_pad_mask.reshape(-1) if non_pad_mask is not None else None
-    x = _mha_core(self.self_attn, enc_input, enc_input, enc_input, dense_mask=_as_u8_mask(self_attn_mask, B, T, T), row_scale=rs)
-    return _ffn_core(self.pos_ffn, x, row_scale=rs), None
+    maps = _maps_sink()
+    x = _mha_core(self.self_attn, enc_input, enc_input, enc_input, dense_mask=_as_u8_mask(self_attn_mask, B, T, T), row_scale=rs,
+                  maps=maps)
+    return _ffn_core(self.pos_ffn, x, row_scale=rs), _first(maps)
 
 
 def decoder_layer_forward(self, decoder_input, encoder_output, non_pad_mask=None, self_attn_mask=None, dec_enc_attn_mask=None):
-    """DecoderLayer.forward -- models/asr/transformer.py:533-545 (dense-mask compatible signature)."""
+    """DecoderLayer.forward -- models/asr/transformer.py:533-545 (dense-mask compatible signature) -> (output, self_attn,
+    enc_attn), the maps None while ops.attention_maps is off."""
     B, T, _ = decoder_input.shape
     Te = encoder_output.shape[1]
     rs = non_pad_mask.reshape(-1) if non_pad_mask is not None else None
+    self_maps, cross_maps = _maps_sink(), _maps_sink()
     x = _mha_core(self.self_attn, decoder_input, decoder_input, decoder_input,
-                  dense_mask=_as_u8_mask(self_attn_mask, B, T, T), row_scale=rs)
+                  dense_mask=_as_u8_mask(self_attn_mask, B, T, T), row_scale=rs, maps=self_maps)
     x = _mha_core(self.encoder_attn, x, encoder_output, encoder_output,
-                  dense_mask=_as_u8_mask(dec_enc_attn_mask, B, T, Te), row_scale=rs)
-    return _ffn_core(self.pos_ffn, x, row_scale=rs), None, None
+                  dense_mask=_as_u8_mask(dec_enc_attn_mask, B, T, Te), row_scale=rs, maps=cross_maps)
+    return _ffn_core(self.pos_ffn, x, row_scale=rs), _first(self_maps), _first(cross_maps)
 
 
-def _encoder_body(self, feats, input_lengths, cf_order=None):
+def _encoder_body(self, feats, input_lengths, cf_order=None, maps=None):
     """Encoder.forward body (models/asr/transformer.py:157-180).  `feats` is [B,T,D]; when cf_order=(C,F) its
     feature axis is ordered f*C+c (channels-last conv output) and input_linear's columns are permuted to match.
-    Masks are a key-valid byte vector per utterance built from the RAW lengths (quirk Q1 preserved)."""
+    Masks are a key-valid byte vector per utterance built from the RAW lengths (quirk Q1 preserved).  `maps`: a list that
+    receives each layer's self-attention map, or None."""
     B, T, D = feats.shape
     key_pad, non_pad = ops.length_masks(input_lengths, B, T, feats.device)
     rs = non_pad.view(-1)
@@ -141,19 +160,32 @@ def _encoder_body(self, feats, input_lengths, cf_order=None):
     pe = self.positional_encoding.pe[0, :T]
     x = ops.AddLNFn.apply(x, None, ln.weight, ln.bias, pe, None, ln.eps, 0.0)
     for layer in self.layers:
-        x = _mha_core(layer.self_attn, x, x, x, key_pad=key_pad, row_scale=rs)
+        x = _mha_core(layer.self_attn, x, x, x, key_pad=key_pad, row_scale=rs, maps=maps)
         x = _ffn_core(layer.pos_ffn, x, row_scale=rs)
     return x
 
 
 def encoder_forward(self, padded_input, input_lengths):
-    """Encoder.forward(padded_input, input_lengths) -> (output, [None]*L)."""
-    return _encoder_body(self, padded_input, input_lengths), [None] * len(self.layers)
+    """Encoder.forward(padded_input, input_lengths) -> (output, [self_attn map per layer]); [None]*L while
+    ops.attention_maps is off."""
+    maps = _maps_sink()
+    out = _encoder_body(self, padded_input, input_lengths, maps=maps)
+    return out, maps if maps is not None else [None] * len(self.layers)
 
 
 def decoder_forward(self, padded_input, encoder_padded_outputs, encoder_input_lengths):
-    """Decoder.forward -- models/asr/transformer.py:268-305: (pred, gold, [None]*L, [None]*L).
-    Target preprocessing, masks, embedding+PE run on the device without host syncs."""
+    """Decoder.forward -- models/asr/transformer.py:268-305: (pred, gold, [self_attn map per layer], [enc_attn map per
+    layer]), [None]*L each while ops.attention_maps is off."""
+    self_maps, cross_maps = _maps_sink(), _maps_sink()
+    pred, gold = _decoder_body(self, padded_input, encoder_padded_outputs, encoder_input_lengths, self_maps, cross_maps)
+    n = len(self.layers)
+    return (pred, gold, self_maps if self_maps is not None else [None] * n,
+            cross_maps if cross_maps is not None else [None] * n)
+
+
+def _decoder_body(self, padded_input, encoder_padded_outputs, encoder_input_lengths, self_maps=None, cross_maps=None):
+    """Decoder.forward body -> (pred, gold).  Target preprocessing, masks, embedding+PE run on the device without host
+    syncs.  self_maps / cross_maps: lists that receive each layer's attention maps, or None."""
     Tt = int(self.trg_max_length)
     seq_in, seq_out, key_pad, non_pad = ops.preprocess_targets(padded_input, Tt)
     B = seq_in.shape[0]
@@ -163,12 +195,12 @@ def decoder_forward(self, padded_input, encoder_padded_outputs, encoder_input_le
     pe = self.positional_encoding.pe[0, :Tt]
     x = ops.EmbedFn.apply(seq_in, self.trg_embedding.weight, pe, float(self.x_logit_scale), _drop_p(self, self.dropout), PAD_TOKEN)
     for layer in self.layers:
-        x = _mha_core(layer.self_attn, x, x, x, key_pad=key_pad, causal=True, row_scale=rs)
-        x = _mha_core(layer.encoder_attn, x, encoder_padded_outputs, encoder_padded_outputs, key_pad=enc_key_pad, row_scale=rs)
+        x = _mha_core(layer.self_attn, x, x, x, key_pad=key_pad, causal=True, row_scale=rs, maps=self_maps)
+        x = _mha_core(layer.encoder_attn, x, encoder_padded_outputs, encoder_padded_outputs, key_pad=enc_key_pad, row_scale=rs,
+                      maps=cross_maps)
         x = _ffn_core(layer.pos_ffn, x, row_scale=rs)
     pred = ops.LinearFn.apply(x, self.output_linear.weight, None)
-    n = len(self.layers)
-    return pred, seq_out, [None] * n, [None] * n
+    return pred, seq_out
 
 
 def greedy_decode_ids(self, encoder_padded_outputs, steps=300):
@@ -637,18 +669,21 @@ def _front_end(self, padded_input):
 
 
 def transformer_forward(self, padded_input, input_lengths, padded_target, verbose=False):
-    """Transformer.forward -> (pred, gold, hyp_seq, gold_seq) -- models/asr/transformer.py:59-85."""
+    """Transformer.forward -> (pred, gold, hyp_seq, gold_seq) -- models/asr/transformer.py:59-85.  Never computes attention
+    maps: the reference discards them here."""
     ops._need_cuda(padded_input, padded_target)
     feats, cf = _front_end(self, padded_input)
     enc = _encoder_body(self.encoder, feats, input_lengths, cf)
-    pred, gold, *_ = decoder_forward(self.decoder, padded_target, enc, input_lengths)
+    pred, gold = _decoder_body(self.decoder, padded_target, enc, input_lengths)
     hyp_seq = ops.argmax_rows(pred)
     return pred, gold, hyp_seq, gold
 
 
 def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_search=False, beam_width=0, beam_nbest=0, lm=None,
                          lm_rescoring=False, lm_weight=0.1, c_weight=1, verbose=False):
-    """Transformer.evaluate (models/asr/transformer.py:87-124) -> ([[None] * L, [None] * L], strs_hyps, strs_gold).
+    """Transformer.evaluate (models/asr/transformer.py:87-124) -> ([[None] * L, [None] * L], strs_hyps, strs_gold); while
+    ops.attention_maps is on, the first value is [decoder self-attention maps, decoder encoder-attention maps] of the
+    reference's teacher-forced decoder pass, which then runs (teacher_forced_maps) -- its topk still does not.
 
     The front end (_front_end: emb_cnn normalises with BatchNorm's running statistics in eval mode) and the encoder run on the
     device, then Decoder.beam_search (nbest=1; greedy_search when fewer than B strings come back, :112-118) or
@@ -658,7 +693,8 @@ def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_
     A model in training mode runs the reference's own method.
 
     In a process that has joined a data-parallel group (parallel.join, as install() does under b200asr.launch) each rank
-    decodes its share of the batch and every rank returns the strings of the whole batch (evaluate_sharded)."""
+    decodes its share of the batch and every rank returns the strings of the whole batch (evaluate_sharded); the attention
+    maps, when on, are of the whole batch on every rank, without a collective."""
     if self.training:
         ref = _reference_method(self, "evaluate", "in training mode")
         return ref(self, padded_input, input_lengths, padded_target, beam_search=beam_search, beam_width=beam_width,
@@ -667,17 +703,35 @@ def transformer_evaluate(self, padded_input, input_lengths, padded_target, beam_
     ops._need_cuda(padded_input, padded_target)
     dec = self.decoder
     group = parallel.joined()
+    n = len(dec.layers)
+    maps = [[None] * n, [None] * n]
     if group is not None and not (beam_search and lm_rescoring and lstm_lm_parts(lm) is None):
         strs_hyps, strs_gold = evaluate_sharded(self, group, padded_input, input_lengths, padded_target, beam_search,
                                                 beam_width, lm if lm_rescoring else None, lm_weight, c_weight)
+        if ops.attention_maps_enabled():
+            maps = teacher_forced_maps(self, padded_input, input_lengths, padded_target)
     else:
-        strs_hyps, strs_gold = _evaluate_whole(self, padded_input, input_lengths, padded_target, beam_search, beam_width, lm,
-                                               lm_rescoring, lm_weight, c_weight)
+        strs_hyps, strs_gold, enc = _evaluate_whole(self, padded_input, input_lengths, padded_target, beam_search, beam_width,
+                                                    lm, lm_rescoring, lm_weight, c_weight)
+        if ops.attention_maps_enabled():
+            maps = teacher_forced_maps(self, padded_input, input_lengths, padded_target, enc)
     if verbose:
         print("GOLD", strs_gold)
         print("HYP", strs_hyps)
-    n = len(dec.layers)
-    return [[None] * n, [None] * n], strs_hyps, strs_gold
+    return maps, strs_hyps, strs_gold
+
+
+def teacher_forced_maps(self, padded_input, input_lengths, padded_target, enc=None):
+    """[decoder self-attention maps, decoder encoder-attention maps] of Transformer.evaluate's teacher-forced decoder pass
+    (models/asr/transformer.py:106: `hyp, gold, *_ = self.decoder(...)` leaves them in `_`), over the whole batch; `enc` is
+    the encoder output when the caller has it."""
+    with torch.no_grad():
+        if enc is None:
+            feats, cf = _front_end(self, padded_input)
+            enc = _encoder_body(self.encoder, feats, input_lengths, cf)
+        self_maps, cross_maps = [], []
+        _decoder_body(self.decoder, padded_target, enc, input_lengths, self_maps, cross_maps)
+    return [self_maps, cross_maps]
 
 
 def _gold_strings(self, padded_target):
@@ -687,7 +741,7 @@ def _gold_strings(self, padded_target):
 
 def _evaluate_whole(self, padded_input, input_lengths, padded_target, beam_search, beam_width, lm, lm_rescoring, lm_weight,
                     c_weight):
-    """(strs_hyps, strs_gold) of the whole batch in this process."""
+    """(strs_hyps, strs_gold, encoder output) of the whole batch in this process."""
     dec = self.decoder
     with torch.no_grad():
         feats, cf = _front_end(self, padded_input)
@@ -702,7 +756,7 @@ def _evaluate_whole(self, padded_input, input_lengths, padded_target, beam_searc
                 strs_hyps = dec.greedy_search(enc)
         else:
             strs_hyps = dec.greedy_search(enc)
-    return strs_hyps, strs_gold
+    return strs_hyps, strs_gold, enc
 
 
 def encoded_frames(self, T: int) -> int:

@@ -488,6 +488,66 @@ class AddLNFn(torch.autograd.Function):
 
 
 # ----------------------------------------------------------------------------------------------- attention
+_maps_enabled = False
+
+
+class attention_maps:
+    """Whether the attention forwards return their probability maps, as ScaledDotProductAttention.forward and everything
+    above it do in the reference (models/common_layers.py:211-225).  Off by default: the forwards then return None in their
+    place and launch or allocate nothing for them.  Like torch.set_grad_enabled, calling it sets the state and using it as a
+    `with` block restores the previous state on exit (exceptions and nesting included).
+
+    A map is an fp32 (H*B) x Tq x Tk tensor in the reference's order (maps_layout): the matrix the kernel multiplied into V,
+    i.e. softmax(scale * Q K^T, masks) with the forward's own dropout mask and 1 / (1 - p) applied in training.  Masked keys
+    are 0, a fully masked row is NaN.  Maps are detached (requires_grad=False): no gradient flows through them."""
+
+    def __init__(self, enabled: bool):
+        global _maps_enabled
+        self.prev = _maps_enabled
+        _maps_enabled = bool(enabled)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        global _maps_enabled
+        _maps_enabled = self.prev
+        return False
+
+
+def attention_maps_enabled() -> bool:
+    return _maps_enabled
+
+
+def maps_layout(B, H, Tq, Tk):
+    """(shape, (bs, hs, rs)) of an attention map: (H*B) x Tq x Tk with row block h*B + b -- the order of the reference's
+    mask.repeat(H, 1, 1) (models/common_layers.py:189) -- so probability (b, h, t, j) lives at b*bs + h*hs + t*rs + j."""
+    return (H * B, Tq, Tk), (Tq * Tk, B * Tq * Tk, Tk)
+
+
+def attention_probs(state):
+    """The attention map of the forward that produced `state` (_sdpa_forward_impl), in maps_layout.  The materialised
+    path copies the probabilities it kept for the backward (after dropout when p > 0, without the pad columns); the flash
+    paths rebuild them with b200asr_sdpa_probs from Q, K and the forward's log-sum-exp at the forward's precision, with the
+    forward's (seed, offset), so nothing is drawn from `rng`."""
+    q, k = state["tensors"][:2]
+    B, H, Tq, dk = q.shape
+    Tk = k.shape[2]
+    causal, scale, p_drop, seed, off, _ = state["meta"]
+    shape, (bs, hs, rs) = maps_layout(B, H, Tq, Tk)
+    maps = torch.empty(shape, device=q.device, dtype=torch.float32)
+    if state["mat"]:
+        probs, probs_drop = state["tensors"][4:6]
+        src = (probs_drop if p_drop > 0.0 else probs).view(B, H, Tq, -1)[..., :Tk]
+        maps.view(H, B, Tq, Tk).copy_(src.permute(1, 0, 2, 3))
+        return maps
+    lse, key_pad, dense_mask = state["tensors"][4:7]
+    L.check(_lib().b200asr_sdpa_probs(L.ptr(q), L.ptr(k), *_bhtd_strides(q), *_bhtd_strides(k), L.ptr(key_pad), L.ptr(dense_mask),
+                                      causal, L.ptr(lse), L.ptr(maps), bs, hs, rs, B, H, Tq, Tk, dk, scale, p_drop, seed, off,
+                                      state["fwd_prec"], _stream()), "sdpa_probs")
+    return maps
+
+
 def _bhtd_strides(t):
     """(batch, head, row) element strides of a 4-D (B,H,T,d) view whose last dim is contiguous."""
     if t.dim() != 4 or t.stride(3) != 1:
@@ -524,7 +584,7 @@ def _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop, head
                                            L.ptr(out), *os_, L.ptr(lse), L.ptr(ws16), B, H, Tq, Tk, dk, dv, float(scale), float(p_drop),
                                            seed, off, _stream()), "sdpa_fused_fwd")
         return out, dict(mat=False, fused=True, tensors=(q, k, v, out, lse, key_pad, dense_mask, ws16),
-                         meta=(int(causal), float(scale), float(p_drop), seed, off, prec))
+                         meta=(int(causal), float(scale), float(p_drop), seed, off, prec), fwd_prec=prec)
     if prec == L.PREC_TF32X3 and not (dk % 32 == 0 and dv % 32 == 0 and dk <= 256 and dv <= 256 and Tk <= 2048):
         prec = L.PREC_FP32
     if prec == L.PREC_TF32 and not (Tk <= 448 and dk in (32, 64) and dv in (32, 64)):
@@ -549,7 +609,7 @@ def _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop, head
     if bwd_prec == L.PREC_TF32X3:
         bwd_prec = L.PREC_FP32       # the flash-style backward exists as fp32 (CUDA cores) and TF32 (tensor cores) only
     return out, dict(mat=False, tensors=(q, k, v, out, lse, key_pad, dense_mask),
-                     meta=(int(causal), float(scale), float(p_drop), seed, off, bwd_prec))
+                     meta=(int(causal), float(scale), float(p_drop), seed, off, bwd_prec), fwd_prec=prec)
 
 
 def _sdpa_backward_impl(state, dout, dq=None, dkk=None, dvv=None):
@@ -595,11 +655,14 @@ def _sdpa_backward_impl(state, dout, dq=None, dkk=None, dvv=None):
 
 
 class SdpaFn(torch.autograd.Function):
-    """Fused softmax(q k^T * scale, masks) v over (B,H,T,d) *views* (any batch/head/row strides)."""
+    """Fused softmax(q k^T * scale, masks) v over (B,H,T,d) *views* (any batch/head/row strides).  When `maps` is a list,
+    the forward appends its attention map (attention_probs) to it."""
 
     @staticmethod
-    def forward(ctx, q, k, v, key_pad, dense_mask, causal, scale, p_drop, head_major_out=False):
+    def forward(ctx, q, k, v, key_pad, dense_mask, causal, scale, p_drop, head_major_out=False, maps=None):
         out, state = _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop, head_major_out)
+        if maps is not None:
+            maps.append(attention_probs(state))
         ctx.state = state        # tensors are kept alive by the dict (no in-place ops touch them afterwards)
         return out
 
@@ -607,7 +670,7 @@ class SdpaFn(torch.autograd.Function):
     def backward(ctx, dout):
         dq, dkk, dvv = _sdpa_backward_impl(ctx.state, dout)
         ctx.state = None
-        return dq, dkk, dvv, None, None, None, None, None, None
+        return dq, dkk, dvv, None, None, None, None, None, None, None
 
 
 def _adjacent(*ts):
@@ -640,10 +703,11 @@ class AttnProjFn(torch.autograd.Function):
     V of encoder-decoder attention): 200-tile problems on 132 SMs become 600-tile ones, the three data gradients become one
     GEMM with K = 3*H*d (no gradient-accumulation adds), the three weight gradients one split-K GEMM.  The attention kernels
     read Q/K/V as column slices of the packed projection output and write dQ/dK/dV into column slices of one packed
-    buffer, all through strides.  Any other memory arrangement runs the same arithmetic as three GEMMs."""
+    buffer, all through strides.  Any other memory arrangement runs the same arithmetic as three GEMMs.  When `maps` is a
+    list, the forward appends the attention map (attention_probs) to it."""
 
     @staticmethod
-    def forward(ctx, xq, xkv, wq, bq, wk, bk, wv, bv, H, dk, dv, key_pad, dense_mask, causal, scale, p_drop, link=None):
+    def forward(ctx, xq, xkv, wq, bq, wk, bk, wv, bv, H, dk, dv, key_pad, dense_mask, causal, scale, p_drop, link=None, maps=None):
         _need_cuda(xq, xkv, wq, wk, wv)
         ctx.link = link
         if link is not None:
@@ -684,6 +748,8 @@ class AttnProjFn(torch.autograd.Function):
         else:
             q = head_view(packed[0], 0, Tq, dk); k = head_view(packed[1], 0, Tk, dk); v = head_view(packed[2], 0, Tk, dv)
         out, state = _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop)
+        if maps is not None:
+            maps.append(attention_probs(state))
         ctx.state, ctx.saved, ctx.has_bias = state, saved, has_bias
         ctx.params = (wq, bq, wk, bk, wv, bv)
         ctx.shapes = (xq.shape, xkv.shape, same, fuse3, fuse2, (n_q, n_k, n_v), H, dk, dv)
@@ -746,7 +812,7 @@ class AttnProjFn(torch.autograd.Function):
         dxq = dxq.view(xq_shape) if dxq is not None else None
         dxkv = dxkv.view(xkv_shape) if dxkv is not None else None
         return (dxq, dxkv, grads_w[0], grads_b[0], grads_w[1], grads_b[1], grads_w[2], grads_b[2],
-                None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None)
 
 
 def _dense_like(t):

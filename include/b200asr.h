@@ -204,6 +204,20 @@ int b200asr_sdpa_mat_bwd(const float* dout, const float* q, const float* k, cons
                          float* dv_out, float* dp_ws, int B, int H, int Tq, int Tk, int dk, int dv, float scale,
                          float p_drop, uint64_t seed, uint64_t offset, int precision, b200asr_stream_t stream);
 
+/* Attention probabilities of a flash forward (b200asr_sdpa_fwd at precision 0 or 1, b200asr_sdpa_fused_fwd = precision 6),
+ * which keeps only the log-sum-exp: ScaledDotProductAttention.forward's `attn` (models/common_layers.py:217-221).  From the
+ * forward's q, k, masks, lse, scale and (p_drop, seed, offset), recomputes the scores at that forward's precision and writes
+ * P[b,h,t,j] = exp(scale * S - lse[b,h,t]), times the forward's dropout keep / (1 - p) when p_drop > 0, to
+ * probs[b*p_bs + h*p_hs + t*p_rs + j] for j < Tk (any strides; nothing else is written).  Masked keys are 0 and a fully
+ * masked row (lse NaN) is NaN.  Shapes: precision 0 dk in {16,32,64,128}, any Tk; precision 1 dk in {32,64}, Tk <= 448;
+ * precision 6 dk = 64, Tk <= 448.  Any other (shape, precision) pair returns B200ASR_BAD_SHAPE and launches nothing.
+ * q / k strides and alignment as b200asr_sdpa_fwd; probs 4-byte aligned. */
+int b200asr_sdpa_probs(const float* q, const float* k, long long q_bs, long long q_hs, long long q_rs, long long k_bs,
+                       long long k_hs, long long k_rs, const uint8_t* key_pad, const uint8_t* dense_mask, int causal,
+                       const float* lse, float* probs, long long p_bs, long long p_hs, long long p_rs, int B, int H, int Tq,
+                       int Tk, int dk, float scale, float p_drop, uint64_t seed, uint64_t offset, int precision,
+                       b200asr_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * VGG front end (models/asr/transformer.py:42-53).  Activations are kept channels-last with time as the
  * outer spatial axis, [B,T,F,C], so the flatten/transpose of :74-76 becomes a free view [B*T, F*C]
