@@ -4,7 +4,7 @@ Everything computes in hand-written sm_90a CUDA kernels behind the C ABI of incl
 (libb200asr.so, built in-tree).  There is no CPU or stock-PyTorch fallback: importing is fine anywhere, running
 needs the built library and an H100.
 """
-from . import _lib
+from . import _lib, lm_train
 from .config import ASRConfig, BASELINE_CONFIGS
 from .features import NoiseBank, NoiseClips, collate_waves, spectrogram_batch, stft_features_packed
 from .install import install, original, uninstall
@@ -18,4 +18,4 @@ from .parallel import DataParallelStep, HostBatchPrefetcher, shard_batch
 __all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "original", "calculate_loss", "calculate_metrics",
            "loss_and_stats", "LabelTable", "edit_counts","Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
            "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model", "RNNModel", "LM",
-           "precision", "manual_seed", "attention_maps", "spectrogram_batch", "NoiseBank", "NoiseClips", "collate_waves", "stft_features_packed","FlatParams", "FusedAdam", "NoamOpt", "adam_step", "clip_grad_norm_", "DataParallelStep", "HostBatchPrefetcher", "shard_batch"]
+           "precision", "manual_seed", "attention_maps", "spectrogram_batch", "NoiseBank", "NoiseClips", "collate_waves", "stft_features_packed","FlatParams", "FusedAdam", "NoamOpt", "adam_step", "clip_grad_norm_", "DataParallelStep", "HostBatchPrefetcher", "shard_batch", "lm_train"]

@@ -110,6 +110,8 @@ SIGNATURES = {
     "b200asr_lstm_grad_unprepare": (_i, [_vp] * 3 + [_i, _i] + [_vp] * 5),
     "b200asr_lm_nll": (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp]),
     "b200asr_lm_seq_sum": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
+    "b200asr_xent_fwd": (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "b200asr_xent_bwd": (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b200asr_ce_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "b200asr_ce_finalize": (_i, [_vp, _vp, _i, _vp]),
     "b200asr_ce_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _f, _vp, _vp, _vp]),
@@ -124,6 +126,7 @@ SIGNATURES = {
     "b200asr_norm_multi": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b200asr_clip_coef": (_i, [_vp, _i, _f, _vp, _vp]),
     "b200asr_scale_multi": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "b200asr_sgd_multi": (_i, [_vp, _vp, _i, _f, _vp]),
     "b200asr_permute_cols_cf":(_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "b200asr_edit_counts_ws_bytes": (_sz, [_i, _i, _i, _i]),
     "b200asr_edit_counts": (_i, [_vp, _i, _ll, _i, _vp, _i, _ll, _i, _i] + [_vp] * 5 + [_i, _i, _ll, _vp, _vp, _vp, _vp]),

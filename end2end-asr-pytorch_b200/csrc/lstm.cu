@@ -2,7 +2,8 @@
 // (lstm_prepare) and its inverse for gradients (lstm_grad_unprepare), the recurrence as one tile-engine launch per (layer,
 // step) whose epilogue is the LSTM cell (LstmCellPolicyT: rescoring, and training with the gates and cell states saved),
 // the backward recurrence with the cell backward in the epilogue (LstmCellBwdPolicy), the dropout between layers
-// (lstm_dropout), the exact-fp32 token NLL of the logits rows (lm_nll) and the per-sequence sums (lm_seq_sum).
+// (lstm_dropout), the exact-fp32 token NLL of the logits rows (lm_nll) and the per-sequence sums (lm_seq_sum), and the
+// training loss on the same row code (xent_fwd / xent_bwd: nn.CrossEntropyLoss with its defaults).
 //
 // Layout.  H = nhid and I = ninp rounded up to multiples of 8 (16-byte bf16 row pitches for TMA).  The gate rows of W_ih / W_hh
 // are interleaved -- prepared row 4u + g holds gate g (PyTorch order i, f, g, o) of unit u -- so that every 32 consecutive
@@ -330,15 +331,73 @@ __global__ void lstm_prepare_kernel(const float* __restrict__ w_ih, const float*
 }
 
 // One CTA per row: nll = logsumexp(x) - x[target] in exact fp32 (expf / logf); block reductions in a fixed order.
+// row_nll is the row code of both lm_nll and xent_fwd, so a row gets the same bits from either.
 constexpr int NLL_THREADS = 256;
+__device__ __forceinline__ float row_nll(const RowLse& st, const float* __restrict__ x, int V, int64_t tg) {
+  return (tg >= 0 && tg < V) ? (st.mx + logf(st.sumexp)) - x[tg] : NAN;
+}
+
 __global__ void __launch_bounds__(NLL_THREADS) lm_nll_kernel(const float* __restrict__ logits, long long ld,
                                                              const int64_t* __restrict__ targets, float* __restrict__ nll, int V) {
   const int row = blockIdx.x;
   const float* x = logits + (size_t)row * ld;
   const RowLse st = block_row_lse<NLL_THREADS, false>(x, V);
+  if (threadIdx.x == 0) nll[row] = row_nll(st, x, V, targets[row]);
+}
+
+// nn.CrossEntropyLoss() (mean over rows, nothing ignored): the row losses of lm_nll, plus each row's max and log of its
+// exp-sum for the backward.
+__global__ void __launch_bounds__(NLL_THREADS) xent_rows_kernel(const float* __restrict__ logits, long long ld,
+                                                                const int64_t* __restrict__ targets, float* __restrict__ nll,
+                                                                float* __restrict__ stats, int V) {
+  const int row = blockIdx.x;
+  const float* x = logits + (size_t)row * ld;
+  const RowLse st = block_row_lse<NLL_THREADS, false>(x, V);
   if (threadIdx.x == 0) {
-    const int64_t tg = targets[row];
-    nll[row] = (tg >= 0 && tg < V) ? (st.mx + logf(st.sumexp)) - x[tg] : NAN;
+    nll[row] = row_nll(st, x, V, targets[row]);
+    stats[2 * (size_t)row] = st.mx;
+    stats[2 * (size_t)row + 1] = logf(st.sumexp);
+  }
+}
+
+// loss[0] = (sum of nll[0 .. rows-1]) / rows, one CTA: thread i adds rows i, i + 1024, ... in order, then the warp tree,
+// then the 32 warp sums in order -- the same bits on every call.
+constexpr int XENT_MEAN_THREADS = 1024;
+__global__ void __launch_bounds__(XENT_MEAN_THREADS) xent_mean_kernel(const float* __restrict__ nll, int rows,
+                                                                      float* __restrict__ loss) {
+  __shared__ float red[XENT_MEAN_THREADS / 32];
+  float s = 0.f;
+  for (int r = threadIdx.x; r < rows; r += XENT_MEAN_THREADS) s = __fadd_rn(s, nll[r]);
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < XENT_MEAN_THREADS / 32; w++) t = __fadd_rn(t, red[w]);
+    loss[0] = __fdiv_rn(t, (float)rows);
+  }
+}
+
+// dlogits[r, v] = (softmax(x_r)[v] - [v == t_r]) * (*dloss / rows), softmax formed as expf((x - max) - log(sum)) from the
+// forward's stats; a row whose target is outside [0, V) gets NaN, as its loss did.
+__global__ void __launch_bounds__(NLL_THREADS) xent_bwd_kernel(const float* __restrict__ logits, long long ld,
+                                                               const int64_t* __restrict__ targets, const float* __restrict__ stats,
+                                                               const float* __restrict__ dloss, float* __restrict__ dlogits, int rows,
+                                                               int V) {
+  const int row = blockIdx.x;
+  const float* x = logits + (size_t)row * ld;
+  float* dx = dlogits + (size_t)row * ld;
+  const int64_t tg = targets[row];
+  if (tg < 0 || tg >= V) {
+    for (int c = threadIdx.x; c < V; c += NLL_THREADS) dx[c] = NAN;
+    return;
+  }
+  const float s = __fdiv_rn(*dloss, (float)rows);
+  const float mx = stats[2 * (size_t)row], ls = stats[2 * (size_t)row + 1];
+  for (int c = threadIdx.x; c < V; c += NLL_THREADS) {
+    const float p = expf((x[c] - mx) - ls);
+    dx[c] = (c == (int)tg ? p - 1.f : p) * s;
   }
 }
 
@@ -461,6 +520,27 @@ int b200asr_lm_nll(const float* logits, long long ld, const int64_t* targets, fl
   if (rows == 0) return B200ASR_OK;
   lm_nll_kernel<<<rows, NLL_THREADS, 0, (cudaStream_t)stream>>>(logits, ld, targets, nll, V);
   return check_launch("lm_nll");
+}
+
+int b200asr_xent_fwd(const float* logits, long long ld, const int64_t* targets, float* nll, float* stats, float* loss, int rows, int V,
+                     b200asr_stream_t stream) {
+  B200_REQUIRE(logits && targets && nll && stats && loss, B200ASR_BAD_ARG, "xent_fwd: null pointer");
+  B200_REQUIRE(V >= 1 && ld >= V && rows >= 1, B200ASR_BAD_SHAPE, "xent_fwd: rows=%d V=%d ld=%lld (need rows >= 1, V >= 1, ld >= V)",
+               rows, V, ld);
+  cudaStream_t st = (cudaStream_t)stream;
+  xent_rows_kernel<<<rows, NLL_THREADS, 0, st>>>(logits, ld, targets, nll, stats, V);
+  if (int rc = check_launch("xent_fwd")) return rc;
+  xent_mean_kernel<<<1, XENT_MEAN_THREADS, 0, st>>>(nll, rows, loss);
+  return check_launch("xent_fwd");
+}
+
+int b200asr_xent_bwd(const float* logits, long long ld, const int64_t* targets, const float* stats, const float* dloss, float* dlogits,
+                     int rows, int V, b200asr_stream_t stream) {
+  B200_REQUIRE(logits && targets && stats && dloss && dlogits, B200ASR_BAD_ARG, "xent_bwd: null pointer");
+  B200_REQUIRE(V >= 1 && ld >= V && rows >= 1, B200ASR_BAD_SHAPE, "xent_bwd: rows=%d V=%d ld=%lld (need rows >= 1, V >= 1, ld >= V)",
+               rows, V, ld);
+  xent_bwd_kernel<<<rows, NLL_THREADS, 0, (cudaStream_t)stream>>>(logits, ld, targets, stats, dloss, dlogits, rows, V);
+  return check_launch("xent_bwd");
 }
 
 int b200asr_lm_seq_sum(const float* nll, const int64_t* offsets, const int64_t* lengths, int nseq, float* sums,

@@ -1,5 +1,6 @@
 // Step tail over a LIST of separate tensors, the way torch.optim.Adam holds them (no flat buffer): Adam with the arithmetic of
-// torch's foreach implementation, and the gradient-norm clip of torch.nn.utils.clip_grad_norm_ (norm_type 2).
+// torch's foreach implementation, the gradient-norm clip of torch.nn.utils.clip_grad_norm_ (norm_type 2), and the plain SGD
+// update p.data.add_(p.grad, alpha=-lr) of the word-language-model loop.
 //
 // Every kernel takes its per-tensor table by value in the kernel parameters (__grid_constant__, up to 32 KB on sm_90), so a
 // step needs no host-to-device copy, no allocation and no synchronisation.  A table holds at most OPT_TABLE tensors; a longer
@@ -43,7 +44,17 @@ struct GradTable {
   int count;
 };
 
+struct SgdTable {
+  float* p[OPT_TABLE];
+  const float* g[OPT_TABLE];
+  Span s[OPT_TABLE];
+  int block_end[OPT_TABLE];
+  int count;
+  float alpha;
+};
+
 static_assert(sizeof(AdamTable) <= 32764, "Adam table exceeds the kernel parameter limit");
+static_assert(sizeof(SgdTable) <= 32764, "SGD table exceeds the kernel parameter limit");
 
 __device__ __forceinline__ int table_entry(const int* block_end, int count) {
   int lo = 0, hi = count - 1;
@@ -189,6 +200,24 @@ __global__ void __launch_bounds__(OPT_THREADS) scale_multi_kernel(const __grid_c
       });
 }
 
+// p += alpha * g for every element, as one fma: ATen's add_(g, alpha=alpha) computes self + alpha * other in fp32 opmath,
+// which the compiler contracts to fma(alpha, other, self)
+__global__ void __launch_bounds__(OPT_THREADS) sgd_multi_kernel(const __grid_constant__ SgdTable t) {
+  const int k = table_entry(t.block_end, t.count);
+  const long long c = (long long)blockIdx.x - (k ? t.block_end[k - 1] : 0);
+  float* __restrict__ p = t.p[k];
+  const float* __restrict__ g = t.g[k];
+  const float a = t.alpha;
+  visit_chunk(
+      t.s[k], c, [&](long long i) { p[i] = __fmaf_rn(a, g[i], p[i]); },
+      [&](long long i) {
+        float4 P = *reinterpret_cast<const float4*>(p + i);
+        const float4 G = *reinterpret_cast<const float4*>(g + i);
+        P.x = __fmaf_rn(a, G.x, P.x); P.y = __fmaf_rn(a, G.y, P.y); P.z = __fmaf_rn(a, G.z, P.z); P.w = __fmaf_rn(a, G.w, P.w);
+        *reinterpret_cast<float4*>(p + i) = P;
+      });
+}
+
 // Span and chunk count of a tensor whose pointers are ptrs[0 .. nptr-1] (an empty tensor gets no chunk)
 static long long plan_span(const uint64_t* ptrs, int nptr, long long n, Span& s) {
   const uint64_t phase = ptrs[0] & 15u;
@@ -266,6 +295,20 @@ int b200asr_adam_multi(const uint64_t* tensors, const long long* numel, const fl
   t.lerp_w = lerp_weight; t.beta2 = beta2; t.one_minus_beta2 = one_minus_beta2; t.eps = eps;
   adam_multi_kernel<<<(unsigned)blocks, OPT_THREADS, 0, (cudaStream_t)stream>>>(t);
   return check_launch("adam_multi");
+}
+
+int b200asr_sgd_multi(const uint64_t* tensors, const long long* numel, int count, float alpha, b200asr_stream_t stream) {
+  SgdTable t;
+  const long long blocks = plan_table(tensors, 2, numel, count, t.s, t.block_end, "sgd_multi");
+  if (blocks <= 0) return (int)blocks;
+  t.count = count;
+  for (int k = 0; k < count; k++) {
+    t.p[k] = reinterpret_cast<float*>(tensors[2 * (size_t)k]);
+    t.g[k] = reinterpret_cast<const float*>(tensors[2 * (size_t)k + 1]);
+  }
+  t.alpha = alpha;
+  sgd_multi_kernel<<<(unsigned)blocks, OPT_THREADS, 0, (cudaStream_t)stream>>>(t);
+  return check_launch("sgd_multi");
 }
 
 int b200asr_norm_multi(const uint64_t* tensors, const long long* numel, int count, float* norms, b200asr_stream_t stream) {

@@ -1676,6 +1676,49 @@ class CrossEntropyFn(torch.autograd.Function):
         return dx.view(shape), None, None, None
 
 
+class XentFn(torch.autograd.Function):
+    """nn.CrossEntropyLoss() with its defaults -- the mean over rows of logsumexp(row) - row[target], nothing ignored -- the
+    loss of the LSTM LM's training loop (utils/lstm_utils.py:69), on b200asr_xent_fwd / _bwd.
+
+    logits: CUDA fp32 [N, V] with unit column stride (any row pitch); targets: int64 [N] on the same device.  Returns the
+    0-dim mean loss (NaN if a target lies outside [0, V): no host check, as that would need a sync).  The backward reads the
+    upstream gradient on the device, so neither direction synchronises the host."""
+
+    @staticmethod
+    def forward(ctx, logits, targets):
+        if not (torch.is_tensor(logits) and logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 2
+                and logits.shape[0] >= 1 and logits.shape[1] >= 1 and logits.stride(1) == 1):
+            raise ValueError("XentFn: logits must be a CUDA float32 [N, V] tensor (N, V >= 1) with unit column stride, got "
+                             f"{getattr(logits, 'dtype', type(logits))} {tuple(getattr(logits, 'shape', ()))} on "
+                             f"{getattr(logits, 'device', None)}")
+        if not (torch.is_tensor(targets) and targets.dtype == torch.int64 and targets.dim() == 1
+                and targets.shape[0] == logits.shape[0] and targets.device == logits.device):
+            raise ValueError(f"XentFn: targets must be int64 [{logits.shape[0]}] on {logits.device}, got "
+                             f"{getattr(targets, 'dtype', type(targets))} {tuple(getattr(targets, 'shape', ()))} on "
+                             f"{getattr(targets, 'device', None)}")
+        rows, V = logits.shape
+        ld = max(logits.stride(0), V) if rows == 1 else logits.stride(0)
+        tg = targets.contiguous()
+        dev = logits.device
+        nll = torch.empty(rows, device=dev, dtype=torch.float32)
+        stats = torch.empty((rows, 2), device=dev, dtype=torch.float32)
+        loss = torch.empty((), device=dev, dtype=torch.float32)
+        L.check(_lib().b200asr_xent_fwd(L.ptr(logits), ld, L.ptr(tg), L.ptr(nll), L.ptr(stats), L.ptr(loss), rows, V, _stream()),
+                "xent_fwd")
+        ctx.save_for_backward(logits, tg, stats)
+        ctx.ld = ld
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        logits, tg, stats = ctx.saved_tensors
+        rows, V = logits.shape
+        dx = torch.empty((rows, ctx.ld), device=logits.device, dtype=torch.float32)[:, :V]
+        L.check(_lib().b200asr_xent_bwd(L.ptr(logits), ctx.ld, L.ptr(tg), L.ptr(stats), L.ptr(_f32c(dloss)), L.ptr(dx), rows, V,
+                                        _stream()), "xent_bwd")
+        return dx, None
+
+
 def _ctc_host_lengths(lengths, B, limit, what):
     """The lengths of one ctc_loss argument as host ints, checked as torch's ctc_loss checks them: B values in [0, limit].
     CPU tensors (the reference's `sizes` and loader `tgt_lengths`) need no device sync; device tensors are read back."""

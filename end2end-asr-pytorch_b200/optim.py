@@ -324,6 +324,31 @@ def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=Fals
     return out[0]
 
 
+def sgd_step(parameters, lr) -> None:
+    """`for p in parameters: p.data.add_(p.grad, alpha=-lr)`, the update of the word-language-model loop that trains the LSTM
+    LM, as b200asr_sgd_multi launches (one per table of tensors): bit-identical to ATen's add_, no copy, no allocation, no
+    host synchronisation.  Parameters without a gradient are skipped.  Every parameter and gradient must be a dense
+    contiguous fp32 tensor on one CUDA device (ValueError otherwise).  The parameters' version counters advance, as an
+    in-place update of the parameter itself would advance them, so caches keyed on them see the new weights."""
+    import numpy as np
+    params = [parameters] if torch.is_tensor(parameters) else list(parameters)
+    params = [p for p in params if p.grad is not None]
+    if not params:
+        return
+    dev = params[0].device
+    if dev.type != _DEVICE or not all(_plain_cuda_fp32(p, dev) and _plain_cuda_fp32(p.grad, dev) and p.grad.shape == p.shape
+                                      for p in params):
+        raise ValueError("b200asr.sgd_step: every parameter and gradient must be a dense contiguous fp32 tensor on one CUDA device")
+    ptrs = np.array([[p.data_ptr(), p.grad.data_ptr()] for p in params], dtype=np.uint64)
+    numel = np.array([p.numel() for p in params], dtype=np.int64)
+    lib = L.load()
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        for i, j in _tables(len(params)):
+            L.check(lib.b200asr_sgd_multi(ptrs[i:j].ctypes.data, numel[i:j].ctypes.data, j - i, -float(lr), stream), "sgd_multi")
+    torch._C._increment_version(params)
+
+
 def clip_grads(parameters, max_norm):
     """clip_grad_norm_ on the device where clip_eligible takes the gradients, torch.nn.utils.clip_grad_norm_ otherwise."""
     parameters = [parameters] if torch.is_tensor(parameters) else list(parameters)

@@ -518,6 +518,21 @@ int b200asr_lstm_grad_unprepare(const float* dw_ih_p, const float* dw_hh_p, cons
 int b200asr_lm_nll(const float* logits, long long ld, const int64_t* targets, float* nll, int rows, int V, b200asr_stream_t stream);
 int b200asr_lm_seq_sum(const float* nll, const int64_t* offsets, const int64_t* lengths, int nseq, float* sums,
                        b200asr_stream_t stream);
+/* LSTM LM training loss: nn.CrossEntropyLoss() with its defaults (mean over rows, nothing ignored), the criterion of
+ * LM.__init__ (utils/lstm_utils.py:69) and of the word-language-model loop that trains RNNModel.  b200asr_ce_* cannot
+ * serve: they drop every row whose target is 0 (PAD), and in an LM vocabulary 0 is '<eos>'.
+ *   xent_fwd: nll [rows] = the row code of lm_nll (the same bits: logsumexp(logits[r, :V]) - logits[r, targets[r]] in exact
+ *     fp32, row pitch ld, NaN for a target outside [0, V)); stats [rows][2] = (row max, logf(sum of exp(x - max))), read by
+ *     xent_bwd; loss [1] = (sum of nll) / rows, summed in a fixed order by one CTA.  Two launches.
+ *   xent_bwd: dlogits[r, v] = (exp(logits[r, v] - lse_r) - [v == targets[r]]) * (*dloss) / rows, formed as
+ *     expf((x - max) - log-sum) from stats; dlogits has the row pitch ld too (columns V .. ld-1 untouched); a row whose
+ *     target is outside [0, V) gets NaN.  dloss is a device scalar (the upstream gradient).  One launch.
+ * rows >= 1, V >= 1, ld >= V (B200ASR_BAD_SHAPE), no NULL pointer (B200ASR_BAD_ARG); a rejected call launches nothing.  No
+ * host synchronisation, no atomics: repeated calls give identical bits. */
+int b200asr_xent_fwd(const float* logits, long long ld, const int64_t* targets, float* nll, float* stats, float* loss, int rows, int V,
+                     b200asr_stream_t stream);
+int b200asr_xent_bwd(const float* logits, long long ld, const int64_t* targets, const float* stats, const float* dloss, float* dlogits,
+                     int rows, int V, b200asr_stream_t stream);
 int b200asr_ce_fwd(const float* logits, const int64_t* gold, float* row_lse, float* stats, int rows, int V,
                    float smoothing, b200asr_stream_t stream);
 /* stats[3] = stats[0] / stats[1] (the reference's mean loss), stats[4] = 1 / stats[1];
@@ -591,6 +606,10 @@ int b200asr_norm_multi(const uint64_t* tensors, const long long* numel, int coun
 int b200asr_clip_coef(const float* norms, int count, float max_norm, float* out, b200asr_stream_t stream);
 /* tensors[k] *= *coef (device scalar) for every element, in place. */
 int b200asr_scale_multi(const uint64_t* tensors, const long long* numel, int count, const float* coef, b200asr_stream_t stream);
+/* The word-language-model loop's update `for p in model.parameters(): p.data.add_(p.grad, alpha=-lr)` (the loop that trains
+ * utils/lstm_utils.RNNModel): tensors [count][2] = param, grad; param = fma(alpha, grad, param) per element with
+ * alpha = (float)(-lr), which is what ATen's add_ computes -- bit-identical to it on the same device. */
+int b200asr_sgd_multi(const uint64_t* tensors, const long long* numel, int count, float alpha, b200asr_stream_t stream);
 
 /* dst = src permuted: dst[r, f*C + c] = src[r, c*F + f] (input_linear column order, see VGG note);
  * inverse != 0 applies the inverse permutation. */
