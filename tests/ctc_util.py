@@ -53,6 +53,118 @@ def ctc_float64(pred, gold, input_lengths, target_lengths):
     return nll, loss, grad
 
 
+def _log_softmax64(x):
+    x = np.asarray(x, dtype=np.float64)
+    m = x.max(axis=-1, keepdims=True)
+    return (x - m) - np.log(np.exp(x - m).sum(axis=-1, keepdims=True))
+
+
+def _shift(a, k):
+    """a[s - k] (k > 0) or a[s + |k|] (k < 0), -inf where that index is outside a."""
+    out = np.full_like(a, -np.inf)
+    if k > 0:
+        out[k:] = a[:-k]
+    else:
+        out[:k] = a[-k:]
+    return out
+
+
+def ctc_float64_fb(pred, gold, input_lengths, target_lengths, dloss=1.0):
+    """(nll [B], mean loss, d loss / d pred [B, T, V]) in float64, the same quantities and conventions as `ctc_float64`
+    (infeasible: nll +inf and NaN rows t < T_b; rows t >= T_b are 0), from the forward-backward recursions in log space,
+    vectorised over the states of each step: alpha and beta over the extended labels l', gamma_t(s) = exp(alpha_t(s) +
+    beta_t(s) - lp'_t(s) + nll_b), and dz_t = g_b (softmax_t - sum over s with l'(s) = v of gamma_t(s)) with g_b = dloss /
+    (B max(L_b, 1)).  Memory is one [T_b, 2 L_b + 1] float64 array per utterance, so 4095 labels over 8200 frames take
+    about 0.5 GB and a few seconds."""
+    x = pred.detach().cpu().double().numpy() if torch.is_tensor(pred) else np.asarray(pred, dtype=np.float64)
+    gold = np.asarray(gold.cpu() if torch.is_tensor(gold) else gold)
+    il = [int(v) for v in np.asarray(input_lengths).reshape(-1)]
+    tl = [int(v) for v in np.asarray(target_lengths).reshape(-1)]
+    B, T, V = x.shape
+    nll = np.zeros(B)
+    grad = np.zeros((B, T, V))
+    for b in range(B):
+        Tb, Lb = il[b], tl[b]
+        if Tb == 0:
+            nll[b] = 0.0 if Lb == 0 else np.inf
+            continue
+        lab = np.zeros(2 * Lb + 1, dtype=np.int64)
+        lab[1::2] = gold[b, :Lb]
+        Sb = lab.size
+        ls = _log_softmax64(x[b, :Tb])                                        # [Tb, V]
+        rep = np.zeros(Sb, dtype=bool)                                        # l'(s) == l'(s - 2) for odd s >= 3
+        rep[3::2] = lab[3::2] == lab[1:-2:2]
+        skip_a = np.zeros(Sb, dtype=bool)
+        skip_a[3::2] = ~rep[3::2]                                             # the skip into s
+        skip_b = np.zeros(Sb, dtype=bool)
+        skip_b[1:-2:2] = ~rep[3::2]                                           # the skip out of s
+        alpha = np.empty((Tb, Sb))
+        a = np.full(Sb, -np.inf)
+        a[:2] = ls[0, lab[:2]]
+        alpha[0] = a
+        for t in range(1, Tb):
+            a = np.logaddexp(np.logaddexp(a, _shift(a, 1)), np.where(skip_a, _shift(a, 2), -np.inf)) + ls[t, lab]
+            alpha[t] = a
+        lp_end = np.logaddexp(a[-1], a[-2]) if Sb >= 2 else a[-1]
+        if not np.isfinite(lp_end):
+            nll[b] = np.inf
+            grad[b, :Tb] = np.nan
+            continue
+        nll[b] = -lp_end
+        # beta from the last frame down; alpha[t] becomes log gamma_t in place (beta_t is not kept)
+        bt = np.full(Sb, -np.inf)
+        bt[-2:] = ls[Tb - 1, lab[-2:]] if Sb >= 2 else ls[Tb - 1, lab]
+        alpha[Tb - 1] += bt - ls[Tb - 1, lab] + nll[b]
+        for t in range(Tb - 2, -1, -1):
+            lpt = ls[t, lab]
+            bt = np.logaddexp(np.logaddexp(bt, _shift(bt, -1)), np.where(skip_b, _shift(bt, -2), -np.inf)) + lpt
+            alpha[t] += bt - lpt + nll[b]
+        g = dloss / (B * max(Lb, 1))
+        onehot = np.zeros((Sb, V))                                            # state -> symbol
+        onehot[np.arange(Sb), lab] = 1.0
+        for c0 in range(0, Tb, 1024):                                         # gamma summed per symbol, 1024 rows at a time
+            c1 = min(Tb, c0 + 1024)
+            grad[b, c0:c1] = g * (np.exp(ls[c0:c1]) - np.exp(alpha[c0:c1]) @ onehot)
+    loss = float(np.mean(nll / np.maximum(np.asarray(tl, dtype=np.float64), 1.0)))
+    return torch.from_numpy(nll), torch.tensor(loss, dtype=torch.float64), torch.from_numpy(grad)
+
+
+def repeats(y):
+    """r: the number of adjacent equal labels of target y, so that L + r is the fewest frames that align y."""
+    return sum(int(y[i]) == int(y[i + 1]) for i in range(len(y) - 1))
+
+
+def ctc_unique_path(pred, gold, input_lengths, target_lengths, dloss=1.0):
+    """(nll [B], mean loss, d loss / d pred [B, T, V]) in float64 for batches where every utterance has exactly one
+    alignment: a target without the label 0 and T_b = L_b + r_b frames (r_b = repeats(target)).  The alignment emits
+    each label once and a blank between equal neighbours, so nll_b = -sum_t log softmax_t(pi_t) and dz_t = g_b (softmax_t -
+    onehot(pi_t)) -- no recursion at all."""
+    x = pred.detach().cpu().double().numpy() if torch.is_tensor(pred) else np.asarray(pred, dtype=np.float64)
+    il = [int(v) for v in np.asarray(input_lengths).reshape(-1)]
+    tl = [int(v) for v in np.asarray(target_lengths).reshape(-1)]
+    B, T, V = x.shape
+    nll = np.zeros(B)
+    grad = np.zeros((B, T, V))
+    for b in range(B):
+        y = [int(v) for v in gold[b, :tl[b]]]
+        assert 0 not in y and il[b] == len(y) + repeats(y), "not a single-alignment utterance"
+        path = []
+        for i, v in enumerate(y):
+            if i and v == y[i - 1]:
+                path.append(0)
+            path.append(v)
+        Tb = il[b]
+        if Tb == 0:
+            continue
+        ls = _log_softmax64(x[b, :Tb])
+        nll[b] = -ls[np.arange(Tb), path].sum()
+        d = np.exp(ls)
+        d[np.arange(Tb), path] -= 1.0
+        grad[b, :Tb] = dloss / (B * max(tl[b], 1)) * d
+    loss = float(np.mean(nll / np.maximum(np.asarray(tl, dtype=np.float64), 1.0)))
+    return torch.from_numpy(nll), torch.tensor(loss, dtype=torch.float64), torch.from_numpy(grad)
+
+
 def cpu_backward_differs(gold, input_lengths, target_lengths):
     """[(b, t)]: the rows where torch's CPU ctc_loss backward is not the derivative.  When an utterance's last label is the
     blank 0, at its last frame t = T_b - 1 torch's CPU kernel assigns the blank's occupation from state 2 L_b - 1 over the

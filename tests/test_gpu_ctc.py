@@ -12,6 +12,13 @@
   * calculate_loss + backward with CPU int32 lengths under torch.cuda.set_sync_debug_mode("error").
   * Rejections: lengths > T, target lengths > S, negative lengths, CPU logits.
   * The reference's Trainer.train with --loss ctc for one epoch, eager and installed, with an infeasible training batch.
+
+tests/test_gpu_ctc_widths.py covers the rest of the kernels, on guarded buffers against the float64 forward-backward of
+tests/ctc_util.py: every recursion width K = 1 .. 32 (targets up to 4095 labels, the shared-memory opt-in at K = 32) on both
+sides of each boundary, trained-model logits (sigma up to 30, forced alignments +80 over the rest) at T up to 8200, the
+feasibility boundary T_b = L_b + r_b against the closed-form single alignment, all-empty batches and V = 1, bitwise
+independence of the utterances at B = 257, dloss != 1 through ops, the 4095-label limit, and NaN results for lengths that
+break the contract on the device.
 """
 import copy
 import importlib
