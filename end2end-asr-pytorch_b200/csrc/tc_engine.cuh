@@ -15,7 +15,8 @@
 //                        pipelined (mma_pipeline): k-block kb + 1 is prepared -- B made ready, A fragments built into a
 //                        second register buffer -- while kb's MMAs run, and kb's stage is released one k-block late;
 //                        after the last k-block they stage the accumulators through shared memory and hand 32-column row
-//                        pieces to Policy::store, a warp covering 32 consecutive rows.
+//                        pieces to Policy::store, a warp covering 32 consecutive rows -- or, where the policy offers it
+//                        (Policy::kStoreVec4), 4-column groups to Policy::load4 / store4, a warp covering whole rows.
 // The producer warpgroup gives registers to the consumers (setmaxnreg: 40 / 232 per thread).  The kernel must contain no
 // function call anywhere (no printf, no 64-bit division helper in a Policy): ptxas then serializes every wgmma (C7510).
 //
@@ -28,6 +29,8 @@
 //                              // (fixed tx bytes, issued by the leader lane only); every lane advances the k cursor in Tile
 //   static __device__ void load16(..., halves);               // the same for the bf16 modes with a pre-converted B
 //   static __device__ void store(p, const Tile&, row, col0, const float (&v)[32]);     // 32 accumulator columns of one row
+//   static constexpr bool kStoreVec4 (optional);  struct Epi4;  bool vec4_ok(p);  Epi4 load4(p, Tile, row, col);
+//       void store4(p, Tile, row, col, float4 v, const Epi4&);     // coalesced epilogue (epilogue_vec4), 4 columns of one row
 //   static constexpr bool kSumA, kSumB;   // fused reductions over the contraction index, taken from the fp32 operand tiles
 //       the consumers read anyway: kSumA = row sums of A, kSumB = column sums of an MN-major B tile (bias gradients of the
 //       weight-gradient GEMMs -- a separate column-sum pass would re-read the operand from HBM)
@@ -256,6 +259,49 @@ __device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], float*
         v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
       }
       out(row, cc * EC + piece * 32, v);
+    }
+  }
+}
+
+// Policy::kStoreVec4 (optional, default false): the policy also offers a coalesced epilogue -- vec4_ok(p) says whether a
+// launch may use it, load4 / store4 handle 4 consecutive columns of one row (loads first, so that a thread's loads of
+// several groups are in flight together)
+template <class P, class = void> struct policy_store_vec4 : std::false_type {};
+template <class P> struct policy_store_vec4<P, std::void_t<decltype(P::kStoreVec4)>> : std::bool_constant<P::kStoreVec4> {};
+
+// The accumulators staged as in epilogue_rows, but handed out as 4-column groups: EC / 4 consecutive lanes cover one row
+// of the chunk, so every global access of a warp is a contiguous run of its rows (a 32-column row piece per thread puts
+// each of a warp's 16-byte accesses in a different cache line).  All ENG_CONSUMERS threads call it.
+template <class Policy, int BN>
+__device__ __forceinline__ void epilogue_vec4(const typename Policy::Params& p, const typename Policy::Tile& tc,
+                                              const float (&acc)[BN / 2], float* epi, int ctid, int r0, int r1, int q) {
+  constexpr int EC = BN < 64 ? BN : 64, EP = EC + 4;
+  constexpr int LPR = EC / 4, RPP = ENG_CONSUMERS / LPR, NIT = 128 / RPP, U = 2;   // lanes per row, rows per pass, passes
+  static_assert(NIT % U == 0, "passes");
+  const int cl = ctid % LPR, rl = ctid / LPR;
+#pragma unroll
+  for (int cc = 0; cc < BN / EC; cc++) {
+    named_bar_sync(ENG_BAR, ENG_CONSUMERS);           // the previous chunk's readers are done with the buffer
+#pragma unroll
+    for (int j = 0; j < EC / 8; j++) {
+      const int jj = cc * (EC / 8) + j, col = j * 8 + 2 * q;
+      *reinterpret_cast<float2*>(epi + r0 * EP + col) = make_float2(acc[4 * jj], acc[4 * jj + 1]);
+      *reinterpret_cast<float2*>(epi + r1 * EP + col) = make_float2(acc[4 * jj + 2], acc[4 * jj + 3]);
+    }
+    named_bar_sync(ENG_BAR, ENG_CONSUMERS);
+    const int col = cc * EC + cl * 4;
+#pragma unroll
+    for (int i0 = 0; i0 < NIT; i0 += U) {
+      float4 v[U];
+      typename Policy::Epi4 x[U];
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const int row = (i0 + u) * RPP + rl;
+        v[u] = *reinterpret_cast<const float4*>(epi + row * EP + cl * 4);
+        x[u] = Policy::load4(p, tc, row, col);
+      }
+#pragma unroll
+      for (int u = 0; u < U; u++) Policy::store4(p, tc, (i0 + u) * RPP + rl, col, v[u], x[u]);
     }
   }
 }
@@ -537,7 +583,15 @@ tc_engine_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     }
 
     // ---- epilogue
-    epilogue_rows<BN>(acc, epi, ctid, r0, r1, q, [&](int row, int col0, const float (&v)[32]) { Policy::store(p, tc, row, col0, v); });
+    // (not with B_T32: its consumers hold the transposed B tile and are close to kConsumerRegs already)
+    constexpr bool kVec4 = policy_store_vec4<Policy>::value && Cfg::kBMode != B_T32;
+    bool vec4 = false;
+    if constexpr (kVec4) vec4 = Policy::vec4_ok(p);
+    if constexpr (kVec4) {
+      if (vec4) epilogue_vec4<Policy, BN>(p, tc, acc, epi, ctid, r0, r1, q);
+    }
+    if (!vec4)
+      epilogue_rows<BN>(acc, epi, ctid, r0, r1, q, [&](int row, int col0, const float (&v)[32]) { Policy::store(p, tc, row, col0, v); });
   }
 }
 

@@ -148,6 +148,41 @@ struct GemmPolicy {
     if (p.e.splits > 1) p.e.rowpart[(size_t)t.z * p.e.M + t.m0 + r] = v;
     else p.e.rowsum[t.m0 + r] += v;                      // one tile per row when K is not split
   }
+  // Coalesced epilogue (tc_engine.cuh: epilogue_vec4) for the launches whose store takes the fast path below; the same
+  // arithmetic per element (bias 0, mask 1, old C 0 where absent), so the results are those of store.
+  static constexpr bool kStoreVec4 = true;
+  struct Epi4 { float4 b, m, c; };
+  static __device__ __forceinline__ bool vec4_ok(const Params& p) {
+    const EpiP& e = p.e;
+    if ((e.N & 3) != 0) return false;
+    if (e.splits > 1) return true;
+    return (e.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(e.C) & 15) == 0 && (reinterpret_cast<uintptr_t>(e.bias) & 15) == 0 &&
+           (reinterpret_cast<uintptr_t>(e.relu_mask) & 15) == 0;
+  }
+  static __device__ __forceinline__ Epi4 load4(const Params& p, const Tile& t, int r, int c) {
+    const EpiP& e = p.e;
+    Epi4 x{make_float4(0.f, 0.f, 0.f, 0.f), make_float4(1.f, 1.f, 1.f, 1.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+    const int row = t.m0 + r, col = t.n0 + c;
+    if (e.splits > 1 || row >= e.M || col >= e.N) return x;
+    if (e.bias) x.b = __ldg(reinterpret_cast<const float4*>(e.bias + col));
+    if (e.relu_mask) x.m = __ldg(reinterpret_cast<const float4*>(e.relu_mask + (size_t)row * e.ldc + col));
+    if (e.accumulate) x.c = *reinterpret_cast<const float4*>(e.C + (size_t)row * e.ldc + col);
+    return x;
+  }
+  static __device__ __forceinline__ void store4(const Params& p, const Tile& t, int r, int c, float4 v, const Epi4& x) {
+    const EpiP& e = p.e;
+    const int row = t.m0 + r, col = t.n0 + c;
+    if (row >= e.M || col >= e.N) return;
+    if (e.splits > 1) {                                   // this split's partial tile
+      *reinterpret_cast<float4*>(e.part + ((size_t)t.z * e.M + row) * e.N + col) = v;
+      return;
+    }
+    float o[4] = {v.x + x.b.x, v.y + x.b.y, v.z + x.b.z, v.w + x.b.w};
+    if (e.relu) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); o[2] = fmaxf(o[2], 0.f); o[3] = fmaxf(o[3], 0.f); }
+    o[0] = x.m.x > 0.f ? o[0] : 0.f; o[1] = x.m.y > 0.f ? o[1] : 0.f;
+    o[2] = x.m.z > 0.f ? o[2] : 0.f; o[3] = x.m.w > 0.f ? o[3] : 0.f;
+    *reinterpret_cast<float4*>(e.C + (size_t)row * e.ldc + col) = make_float4(o[0] + x.c.x, o[1] + x.c.y, o[2] + x.c.z, o[3] + x.c.w);
+  }
   static __device__ __forceinline__ void store(const Params& p, const Tile& t, int r, int c0, const float (&v)[32]) {
     const EpiP& e = p.e;
     const int m0 = t.m0, n0 = t.n0, z = t.z;
