@@ -212,7 +212,14 @@ def test_step_needs_no_sync_and_few_launches(clip):
     tables = -(-n_grads // cap)
     torch.cuda.synchronize()
     launches0 = L.load().b200asr_launch_count()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]) as prof:
+    # a warm-up step whose events are discarded first: kernels launched while CUPTI starts tracing can go unrecorded
+    seen = []
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA],
+                                schedule=torch.profiler.schedule(wait=0, warmup=1, active=1, repeat=1),
+                                on_trace_ready=lambda p: seen.append(count_cuda(p))) as prof:
+        torch.cuda._sleep(1000)
+        torch.cuda.synchronize()
+        prof.step()
         torch.cuda._sleep(1000)                                 # marks where the step's work begins
         torch.cuda.set_sync_debug_mode("error")
         try:
@@ -223,7 +230,9 @@ def test_step_needs_no_sync_and_few_launches(clip):
         finally:
             torch.cuda.set_sync_debug_mode(0)
         torch.cuda.synchronize()
-    kernels, copies = count_cuda(prof)
+        prof.step()
+    assert len(seen) == 1
+    kernels, copies = seen[0]
     # per table: Adam 1 launch; clip 3 (sum of squares, per-tensor norms, scale); plus the clip coefficient once
     want = tables * (4 if clip else 1) + (1 if clip else 0)
     print(f"clip={clip}: {n_grads} tensors, {tables} tables, {len(kernels)} kernels, {len(copies)} copies")
