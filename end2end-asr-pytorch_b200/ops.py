@@ -5,11 +5,13 @@ kernel of libb200asr.so.  All functions require CUDA tensors; there is no CPU im
 """
 from __future__ import annotations
 
+import functools
 import os
 from typing import Optional
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib as L
 
@@ -300,17 +302,64 @@ class ResidualLink:
         return dz
 
 
-def _grad_sink(param):
-    """The parameter's existing .grad if a kernel can accumulate straight into it (the flat gradient buffer of
-    optim.FlatParams), else None.  Writing there removes autograd's AccumulateGrad add kernel and a temporary per weight."""
+def _engine_accumulates(param, node):
+    """True if the running backward will execute `node`, the parameter's AccumulateGrad node (the node's edge to it,
+    ctx.next_functions[i][0]), i.e. autograd itself would add a gradient into .grad: plain .backward(), or
+    backward(inputs=...) naming the parameter.  False for a frozen parameter, under autograd.grad (the engine raises for a
+    leaf among its inputs and must leave .grad alone), for a parameter backward(inputs=...) does not name, and outside a
+    backward."""
+    if not param.requires_grad:
+        return False          # frozen (also after the forward): autograd adds nothing, neither may a kernel
+    try:
+        return bool(torch._C._will_engine_execute_node(node))
+    except RuntimeError:      # a leaf among autograd.grad's inputs, or no backward running
+        return False
+
+
+def _sink_candidate(param, node):
+    """The device-independent part of _grad_sink: the parameter's .grad if the sink rule allows writing into it, else None."""
     if param is None or not param.is_leaf or not getattr(param, "_b200_flat_grad", False):
         return None          # opt-in: only parameters re-homed by optim.FlatParams (it owns their .grad views)
     if getattr(param, "_backward_hooks", None) or getattr(param, "_post_accumulate_grad_hooks", None):
         return None          # tensor hooks (DDP, clipping hooks ...) must see the gradient: let autograd deliver it
     g = param.grad
-    if g is None or not g.is_cuda or g.dtype != torch.float32 or not g.is_contiguous() or g.shape != param.shape:
+    if g is None or g.shape != param.shape or not _engine_accumulates(param, node):
+        return None          # frozen, or the engine was not asked for this parameter's .grad: return the gradient instead
+    return g
+
+
+def _edge_map(*args):
+    """Argument position -> index into the node's next_functions: autograd keeps an edge for each tensor argument only."""
+    out, n = [], 0
+    for a in args:
+        out.append(n if torch.is_tensor(a) else None)
+        n += torch.is_tensor(a)
+    return out
+
+
+def _grad_sink(ctx, i, param):
+    """The existing .grad of `param`, argument i of the node `ctx` (ctx.edges = _edge_map of the forward's arguments), if a
+    kernel can accumulate straight into it (the flat gradient buffer of optim.FlatParams), else None.  Writing there removes
+    autograd's AccumulateGrad add kernel and a temporary per weight."""
+    g = _sink_candidate(param, ctx.next_functions[ctx.edges[i]][0])
+    if g is None or not g.is_cuda or g.dtype != torch.float32 or not g.is_contiguous():
         return None
     return g
+
+
+def _backward(fn):
+    """Decorator of every backward in this module.  The backwards launch kernels that record no graph, so a double backward
+    (create_graph=True) is refused here instead of returning gradients without a grad_fn that differentiate to zero."""
+    inner = once_differentiable(fn)
+
+    @functools.wraps(fn)
+    def backward(ctx, *grads):
+        if torch.is_grad_enabled():
+            raise RuntimeError(f"{fn.__qualname__.split('.')[0]}: the b200asr backward kernels are not differentiable "
+                               "(create_graph=True is not supported)")
+        return inner(ctx, *grads)
+
+    return backward
 
 
 def linear_bwd_weight(dy2, x2, want_bias, prec, w_sink=None, b_sink=None):
@@ -366,24 +415,26 @@ class LinearFn(torch.autograd.Function):
         ctx.prec = _linear_prec(w2.shape[0], w2.shape[1])
         ws = split_weight(w2, ctx.prec, need_bwd=ctx.needs_input_grad[0])
         y = linear_fwd(x2, w2, b, False, ctx.prec, ws)
-        ctx.save_for_backward(x2, w2)
-        ctx.ws = ws
+        ctx.save_for_backward(x2, w2, ws.bwd if ws is not None else None)       # (kept under retain_graph, freed after backward)
         ctx.xshape, ctx.wshape, ctx.has_bias = x.shape, w.shape, b is not None
-        ctx.params = (w, b)
+        ctx.params, ctx.edges = (w, b), _edge_map(x, w, b)
         return y.view(*x.shape[:-1], w2.shape[0])
 
     @staticmethod
+    @_backward
     def backward(ctx, dy):
-        x2, w2 = ctx.saved_tensors
-        ws, ctx.ws = ctx.ws, None
+        x2, w2, ws_bwd = ctx.saved_tensors
         dy2 = _f32c(dy).reshape(-1, w2.shape[0])
+        need = ctx.needs_input_grad
         dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            dx = linear_bwd_data(dy2, w2, None, ctx.prec, ws).view(ctx.xshape)
-        if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):
+        if need[0]:
+            dx = linear_bwd_data(dy2, w2, None, ctx.prec, WSplit(None, ws_bwd)).view(ctx.xshape)
+        want_b = ctx.has_bias and need[2]
+        if need[1] or want_b:
             w, b = ctx.params
-            dw, db = linear_bwd_weight(dy2, x2, ctx.has_bias, ctx.prec, _grad_sink(w), _grad_sink(b))
-            dw = dw.view(ctx.wshape) if dw is not None else None
+            dw, db = linear_bwd_weight(dy2, x2, want_b, ctx.prec, _grad_sink(ctx, 1, w) if need[1] else None,
+                                       _grad_sink(ctx, 2, b) if want_b else None)
+            dw = dw.view(ctx.wshape) if (dw is not None and need[1]) else None
         return dx, dw, db
 
 
@@ -405,30 +456,34 @@ class FFNFn(torch.autograd.Function):
         if decision_capture is not None:
             decision_capture.append(("relu", h.view(*x.shape[:-1], w1m.shape[0])))
         y = linear_fwd(h, w2m, b2, False, ctx.prec, ws2)
-        ctx.save_for_backward(x2, h, w1m, w2m)
-        ctx.ws = (ws1, ws2)
+        ctx.save_for_backward(x2, h, w1m, w2m, ws1.bwd if ws1 is not None else None, ws2.bwd if ws2 is not None else None)
         ctx.shapes = (x.shape, w1.shape, w2.shape)
-        ctx.params = (w1, b1, w2, b2)
+        ctx.params, ctx.edges = (w1, b1, w2, b2), _edge_map(x, w1, b1, w2, b2)
         return y.view(*x.shape[:-1], w2m.shape[0])
 
     @staticmethod
+    @_backward
     def backward(ctx, dy):
-        x2, h, w1m, w2m = ctx.saved_tensors
-        (ws1, ws2), ctx.ws = ctx.ws, None
+        x2, h, w1m, w2m, ws1_bwd, ws2_bwd = ctx.saved_tensors
         xs, w1s, w2s = ctx.shapes
         dy2 = _f32c(dy).reshape(-1, w2m.shape[0])
         w1, b1, w2, b2 = ctx.params
         need = ctx.needs_input_grad                          # (x, w1, b1, w2, b2): frozen weights get no wgrad GEMM
-        dw1 = db1 = dw2 = db2 = None
-        if need[3] or need[4]:
-            dw2, db2 = linear_bwd_weight(dy2, h, True, ctx.prec, _grad_sink(w2), _grad_sink(b2))
-        dh = linear_bwd_data(dy2, w2m, h, ctx.prec, ws2) if (need[0] or need[1] or need[2]) else None     # masked by relu'(h)
-        if need[1] or need[2]:
-            dw1, db1 = linear_bwd_weight(dh, x2, True, ctx.prec, _grad_sink(w1), _grad_sink(b1))
+
+        def wgrad(dyi, xi, i, w, b, wshape):           # w, b: inputs i, i + 1
+            need_w, need_b = need[i], need[i + 1]
+            if not (need_w or need_b):
+                return None, None
+            dw, db = linear_bwd_weight(dyi, xi, need_b, ctx.prec, _grad_sink(ctx, i, w) if need_w else None,
+                                       _grad_sink(ctx, i + 1, b) if need_b else None)
+            return (dw.view(wshape) if (dw is not None and need_w) else None), db
+
+        dw2, db2 = wgrad(dy2, h, 3, w2, b2, w2s)
+        dh = linear_bwd_data(dy2, w2m, h, ctx.prec, WSplit(None, ws2_bwd)) if (need[0] or need[1] or need[2]) else None  # relu'(h)
+        dw1, db1 = wgrad(dh, x2, 1, w1, b1, w1s) if dh is not None else (None, None)
         res = ctx.link.take() if ctx.link is not None else None          # residual-branch gradient of x, if AddLNFn handed it over
-        dx = linear_bwd_data(dh, w1m, None, ctx.prec, ws1, accumulate_into=res) if need[0] else None
-        return ((dx.view(xs) if dx is not None else None), (dw1.view(w1s) if dw1 is not None else None), db1,
-                (dw2.view(w2s) if dw2 is not None else None), db2, None)
+        dx = linear_bwd_data(dh, w1m, None, ctx.prec, WSplit(None, ws1_bwd), accumulate_into=res) if need[0] else None
+        return (dx.view(xs) if dx is not None else None), dw1, db1, dw2, db2, None
 
 
 # ----------------------------------------------------------------------------------------------- residual + LN
@@ -458,21 +513,25 @@ class AddLNFn(torch.autograd.Function):
                                           float(p_drop), seed, off, _stream()), "add_ln_fwd")
         ctx.save_for_backward(z if need_z else x2, gamma, mean, rstd, rs)
         ctx.meta = (x.shape, residual is not None, float(p_drop), seed, off, rows, d)
-        ctx.params = (gamma, beta)
+        ctx.params, ctx.edges = (gamma, beta), _edge_map(x, residual, gamma, beta)
         return y.view(x.shape)
 
     @staticmethod
+    @_backward
     def backward(ctx, dy):
         z, gamma, mean, rstd, rs = ctx.saved_tensors
         xshape, has_res, p_drop, seed, off, rows, d = ctx.meta
         dy2 = _f32c(dy).reshape(-1, d)
         lib = _lib()
+        need = ctx.needs_input_grad
         dz = torch.empty_like(dy2)
         # with a link, dz is later added to in place by the consumer of the residual: keep it distinct from dx
         dx = torch.empty_like(dy2) if (p_drop > 0.0 or ctx.link is not None) else dz
         # gamma / beta gradients go straight into the parameters' .grad (flat gradient buffer) when that exists: no
-        # zero-fill, no AccumulateGrad add -- four tiny launches less per LayerNorm
-        g_sink, b_sink = _grad_sink(ctx.params[0]), _grad_sink(ctx.params[1])
+        # zero-fill, no AccumulateGrad add -- four tiny launches less per LayerNorm.  The kernel writes both, so it
+        # accumulates only when both may be sunk; otherwise it writes temporaries and autograd gets what it asked for.
+        g_sink = _grad_sink(ctx, 2, ctx.params[0]) if need[2] else None
+        b_sink = _grad_sink(ctx, 3, ctx.params[1]) if need[3] else None
         direct = g_sink is not None and b_sink is not None
         dgamma = g_sink if direct else torch.empty(d, device=dy.device, dtype=torch.float32)
         dbeta = b_sink if direct else torch.empty(d, device=dy.device, dtype=torch.float32)
@@ -483,8 +542,8 @@ class AddLNFn(torch.autograd.Function):
         if ctx.link is not None:
             ctx.link.dz = dz                       # summed into the data gradient of the node that consumes the residual
             has_res = False
-        return (dx.view(xshape), (dz.view(xshape) if has_res else None), None if direct else dgamma, None if direct else dbeta,
-                None, None, None, None, None)
+        return (dx.view(xshape) if need[0] else None, (dz.view(xshape) if has_res and need[1] else None),
+                None if direct or not need[2] else dgamma, None if direct or not need[3] else dbeta, None, None, None, None, None)
 
 
 # ----------------------------------------------------------------------------------------------- attention
@@ -663,14 +722,25 @@ class SdpaFn(torch.autograd.Function):
         out, state = _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop, head_major_out)
         if maps is not None:
             maps.append(attention_probs(state))
-        ctx.state = state        # tensors are kept alive by the dict (no in-place ops touch them afterwards)
+        ctx.save_for_backward(*_state_tensors(ctx, state))
         return out
 
     @staticmethod
+    @_backward
     def backward(ctx, dout):
-        dq, dkk, dvv = _sdpa_backward_impl(ctx.state, dout)
-        ctx.state = None
+        dq, dkk, dvv = _sdpa_backward_impl(_restore_state(ctx, ctx.saved_tensors), dout)
         return dq, dkk, dvv, None, None, None, None, None, None, None
+
+
+def _state_tensors(ctx, state):
+    """Splits an attention state (_sdpa_forward_impl) for a ctx: its tensors are returned for ctx.save_for_backward (kept
+    under retain_graph, freed after the backward otherwise), the rest stays on ctx."""
+    ctx.state_meta = {key: val for key, val in state.items() if key != "tensors"}
+    return state["tensors"]
+
+
+def _restore_state(ctx, tensors):
+    return dict(ctx.state_meta, tensors=tuple(tensors))
 
 
 def _adjacent(*ts):
@@ -750,15 +820,21 @@ class AttnProjFn(torch.autograd.Function):
         out, state = _sdpa_forward_impl(q, k, v, key_pad, dense_mask, causal, scale, p_drop)
         if maps is not None:
             maps.append(attention_probs(state))
-        ctx.state, ctx.saved, ctx.has_bias = state, saved, has_bias
-        ctx.params = (wq, bq, wk, bk, wv, bv)
+        st = _state_tensors(ctx, state)
+        ctx.save_for_backward(*st, *[t for _, x2, W, wsplit, _ in saved for t in (x2, W, wsplit.bwd if wsplit is not None else None)])
+        ctx.n_state, ctx.groups, ctx.has_bias = len(st), [(idx, prec) for idx, _, _, _, prec in saved], has_bias
+        ctx.params, ctx.edges = (wq, bq, wk, bk, wv, bv), _edge_map(xq, xkv, wq, bq, wk, bk, wv, bv)
         ctx.shapes = (xq.shape, xkv.shape, same, fuse3, fuse2, (n_q, n_k, n_v), H, dk, dv)
         return out.permute(0, 2, 1, 3).reshape(B, Tq, H * dv)          # free: memory is token-major
 
     @staticmethod
+    @_backward
     def backward(ctx, dout):
         xq_shape, xkv_shape, same, fuse3, fuse2, (n_q, n_k, n_v), H, dk, dv = ctx.shapes
-        q, k, v = ctx.state["tensors"][:3]
+        saved_t = ctx.saved_tensors
+        state = _restore_state(ctx, saved_t[:ctx.n_state])
+        groups = [(idx, *saved_t[ctx.n_state + 3 * j:ctx.n_state + 3 * j + 3], prec) for j, (idx, prec) in enumerate(ctx.groups)]
+        q, k, v = state["tensors"][:3]
         B, Tq, Tk = q.shape[0], q.shape[2], k.shape[2]
         dev = q.device
         new = lambda m, n: torch.empty((m, n), device=dev, dtype=torch.float32)
@@ -774,40 +850,44 @@ class AttnProjFn(torch.autograd.Function):
             dys = [new(B * Tq, n_q), new(B * Tk, n_k), new(B * Tk, n_v)]
             dq, dkk, dvv = head_view(dys[0], 0, Tq, dk), head_view(dys[1], 0, Tk, dk), head_view(dys[2], 0, Tk, dv)
         dout4 = dout.reshape(B, Tq, H, dv).permute(0, 2, 1, 3)
-        _sdpa_backward_impl(ctx.state, dout4, dq, dkk, dvv)
-        ctx.state = None
+        _sdpa_backward_impl(state, dout4, dq, dkk, dvv)
         params = ctx.params
+        need = ctx.needs_input_grad
         grads_w, grads_b = [None] * 3, [None] * 3
         dxkv = None
-        need_xq, need_xkv = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_xq, need_xkv = need[0], need[1]
         # running sums: every further contribution is added in its GEMM's epilogue; dxq starts from the residual-branch
         # gradient of the query input when AddLNFn handed it over (ResidualLink)
         dxq = ctx.link.take() if ctx.link is not None else None
         if dxq is not None and not need_xq:
             dxq = None
-        for (idx, x2, W, wsplit, prec), dy in zip(ctx.saved, dys):
+        for (idx, x2, W, wsplit_bwd, prec), dy in zip(groups, dys):
             feeds_q = 0 in idx
             if (feeds_q and need_xq) or (not feeds_q and (need_xkv or (same and need_xq))):
                 if feeds_q or same:
-                    dxq = linear_bwd_data(dy, W, None, prec, wsplit, accumulate_into=dxq)
+                    dxq = linear_bwd_data(dy, W, None, prec, WSplit(None, wsplit_bwd), accumulate_into=dxq)
                 else:
-                    dxkv = linear_bwd_data(dy, W, None, prec, wsplit, accumulate_into=dxkv)
-            ws_ = [params[2 * i] for i in idx]
-            bs_ = [params[2 * i + 1] for i in idx]
-            sinks_w = [_grad_sink(w) for w in ws_]
-            sinks_b = [_grad_sink(b) for b in bs_] if ctx.has_bias else []
+                    dxkv = linear_bwd_data(dy, W, None, prec, WSplit(None, wsplit_bwd), accumulate_into=dxkv)
+            need_w = [need[2 + 2 * i] for i in idx]
+            need_b = [ctx.has_bias and need[3 + 2 * i] for i in idx]
+            if not (any(need_w) or any(need_b)):
+                continue                # the whole group is frozen: no weight-gradient GEMM
+            # a stacked sink only when every member of the group can be sunk (each one needs its gradient)
+            sinks_w = [_grad_sink(ctx, 2 + 2 * i, params[2 * i]) if nw else None for i, nw in zip(idx, need_w)]
+            want_b = any(need_b)
+            sinks_b = [_grad_sink(ctx, 3 + 2 * i, params[2 * i + 1]) if nb else None for i, nb in zip(idx, need_b)] if want_b else []
             w_sink = b_sink = None
             if all(g is not None for g in sinks_w) and _adjacent(*[g.reshape(g.shape[0], -1) for g in sinks_w]):
                 w_sink = _stacked(*[g.reshape(g.shape[0], -1) for g in sinks_w])
-            if ctx.has_bias and all(g is not None for g in sinks_b) and _adjacent(*sinks_b):
+            if want_b and all(g is not None for g in sinks_b) and _adjacent(*sinks_b):
                 b_sink = _stacked(*sinks_b)
-            dw, db = linear_bwd_weight(dy, x2, ctx.has_bias, prec, w_sink, b_sink)
-            if dw is not None:          # no direct accumulation: hand the slices to autograd
+            dw, db = linear_bwd_weight(dy, x2, want_b, prec, w_sink, b_sink)
+            if dw is not None:          # no direct accumulation: hand the slices autograd asked for to it
                 r0 = 0
-                for i in idx:
+                for i, nw, nb in zip(idx, need_w, need_b):
                     n_i = (n_q, n_k, n_v)[i]
-                    grads_w[i] = dw[r0:r0 + n_i].view(params[2 * i].shape)
-                    grads_b[i] = db[r0:r0 + n_i] if db is not None else None
+                    grads_w[i] = dw[r0:r0 + n_i].view(params[2 * i].shape) if nw else None
+                    grads_b[i] = db[r0:r0 + n_i] if nb else None
                     r0 += n_i
         dxq = dxq.view(xq_shape) if dxq is not None else None
         dxkv = dxkv.view(xkv_shape) if dxkv is not None else None
@@ -880,6 +960,7 @@ class VggFrontendFn(torch.autograd.Function):
         return p2
 
     @staticmethod
+    @_backward
     def backward(ctx, dp2):
         if frontend_backward_hook is not None:
             frontend_backward_hook()
@@ -940,6 +1021,7 @@ class PermuteColsFn(torch.autograd.Function):
         return out
 
     @staticmethod
+    @_backward
     def backward(ctx, dw):
         C, F = ctx.cf
         dw = _f32c(dw)
@@ -1024,6 +1106,7 @@ class EmbFrontendFn(torch.autograd.Function):
         return out
 
     @staticmethod
+    @_backward
     def backward(ctx, dout):
         if frontend_backward_hook is not None:
             frontend_backward_hook()
@@ -1081,6 +1164,7 @@ class FlattenFn(torch.autograd.Function):
         return out
 
     @staticmethod
+    @_backward
     def backward(ctx, dout):
         B, C, F, T = ctx.shape
         dout = _f32c(dout)
@@ -1169,6 +1253,7 @@ class EmbedFn(torch.autograd.Function):
         return out
 
     @staticmethod
+    @_backward
     def backward(ctx, dout):
         (tokens,) = ctx.saved_tensors
         V, d, scale, p_drop, seed, off, pad_idx = ctx.meta
@@ -1568,6 +1653,7 @@ class LstmStackFn(torch.autograd.Function):
         return out, h_n, c_n
 
     @staticmethod
+    @_backward
     def backward(ctx, d_out, d_hn, d_cn):
         inp, c0p, *saved = ctx.saved_tensors
         op, (T, B) = ctx.op, ctx.TB
@@ -1664,6 +1750,7 @@ class CrossEntropyFn(torch.autograd.Function):
         return loss, stats
 
     @staticmethod
+    @_backward
     def backward(ctx, dloss, _dstats):
         x, g, lse, stats = ctx.saved_tensors
         shape, smoothing, mean = ctx.meta
@@ -1710,6 +1797,7 @@ class XentFn(torch.autograd.Function):
         return loss
 
     @staticmethod
+    @_backward
     def backward(ctx, dloss):
         logits, tg, stats = ctx.saved_tensors
         rows, V = logits.shape
@@ -1770,6 +1858,7 @@ class CtcLossFn(torch.autograd.Function):
         return loss
 
     @staticmethod
+    @_backward
     def backward(ctx, dloss):
         x, tg, lens, nll, ws = ctx.saved_tensors
         (B, T, V), lmax = ctx.meta

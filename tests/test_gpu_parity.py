@@ -44,6 +44,17 @@ def _ops(b200):
     return importlib.import_module(b200.__name__ + ".ops")
 
 
+def _cases(*rows):
+    """Parametrize rows whose last value is emb_trg_sharing (the decoder's output projection tied to its embedding, one
+    parameter with a sunk GEMM gradient plus the embedding's returned one); untied rows keep their plain ids."""
+    return [pytest.param(*r, id="-".join(str(v) for v in r[:-1]) + ("-tied" if r[-1] else "")) for r in rows]
+
+
+def _untie(grads_o, grads):
+    """The oracle's gradient dict lists a tied weight under both names; the model's named_parameters() under one."""
+    return {k: v for k, v in grads_o.items() if k in grads}
+
+
 # ------------------------------------------------------------------------------------------------ end to end
 @pytest.mark.parametrize("case", GOLDEN_CASES)
 def test_golden_forward_loss_backward(b200, case):
@@ -61,16 +72,18 @@ def test_golden_forward_loss_backward(b200, case):
     assert_grads_close(grads, G, TOL, exact_kernels=b200.k == 1.0)
 
 
-@pytest.mark.parametrize("feat,L,H,d,dk,dv,di,B,T,Tt,V,freq", [
-    ("vgg_cnn", 2, 4, 128, 32, 32, 256, 2, 20, 9, 77, 41),
-    ("", 2, 2, 64, 16, 32, 128, 4, 70, 13, 33, 161),
-    ("emb_cnn", 1, 2, 64, 32, 32, 64, 2, 36, 6, 20, 161),
-    ("vgg_cnn", 1, 8, 512, 64, 64, 2048, 2, 16, 12, 4364, 41),        # cfg2 architecture, 1 layer, small spectrogram
-])
-def test_oracle_forward_loss_backward(b200, feat, L, H, d, dk, dv, di, B, T, Tt, V, freq):
+@pytest.mark.parametrize("feat,L,H,d,dk,dv,di,B,T,Tt,V,freq,tied", _cases(
+    ("vgg_cnn", 2, 4, 128, 32, 32, 256, 2, 20, 9, 77, 41, False),
+    ("", 2, 2, 64, 16, 32, 128, 4, 70, 13, 33, 161, False),
+    ("emb_cnn", 1, 2, 64, 32, 32, 64, 2, 36, 6, 20, 161, False),
+    ("vgg_cnn", 1, 8, 512, 64, 64, 2048, 2, 16, 12, 4364, 41, False),        # cfg2 architecture, 1 layer, small spectrogram
+    ("vgg_cnn", 2, 4, 128, 32, 32, 256, 2, 20, 9, 77, 41, True),
+    ("", 2, 2, 64, 16, 32, 128, 4, 70, 13, 33, 161, True),
+))
+def test_oracle_forward_loss_backward(b200, feat, L, H, d, dk, dv, di, B, T, Tt, V, freq, tied):
     from tests.gpu_util import TOL, cuda_model, cuda_step
     cfg = O.OracleConfig(num_layers=L, num_heads=H, dim_model=d, dim_key=dk, dim_value=dv, dim_inner=di, vocab=V,
-                         feat_extractor=feat, tgt_max_len=Tt, freq=freq)
+                         feat_extractor=feat, tgt_max_len=Tt, freq=freq, emb_trg_sharing=tied)
     P = O.init_params(cfg, seed=3)
     g = torch.Generator().manual_seed(17)
     for k in sorted(P):             # move norm scales / biases off (1, 0)
@@ -97,7 +110,7 @@ def test_oracle_forward_loss_backward(b200, feat, L, H, d, dk, dv, di, B, T, Tt,
     assert torch.equal(hyp[clear], hyp_o[clear])
     assert abs(loss.item() - loss_o.item()) < TOL * abs(loss_o.item())
     assert int(stats[1].item()) == n_word
-    assert_grads_close(grads, grads_o, TOL, exact_kernels=b200.k == 1.0)
+    assert_grads_close(grads, _untie(grads_o, grads), TOL, exact_kernels=b200.k == 1.0)
 
 
 # ------------------------------------------------------------------------------------------------ kernel families
@@ -171,18 +184,20 @@ def test_add_layernorm_fwd_bwd(b200, rows, T, d, with_res, with_pe, with_scale):
     assert rel_err(bc.grad, beta.grad) < 1e-4
 
 
-@pytest.mark.parametrize("feat,L,H,d,dk,dv,di,B,T,Tt,V,freq", [
-    ("vgg_cnn", 2, 4, 128, 32, 32, 256, 2, 20, 9, 77, 41),
-    ("", 2, 2, 64, 32, 64, 128, 3, 50, 11, 33, 161),                  # dk != dv: the stacked Q|K|V rows differ in width
-])
-def test_flat_params_stack_qkv_projections(b200, feat, L, H, d, dk, dv, di, B, T, Tt, V, freq):
+@pytest.mark.parametrize("feat,L,H,d,dk,dv,di,B,T,Tt,V,freq,tied", _cases(
+    ("vgg_cnn", 2, 4, 128, 32, 32, 256, 2, 20, 9, 77, 41, False),
+    ("", 2, 2, 64, 32, 64, 128, 3, 50, 11, 33, 161, False),           # dk != dv: the stacked Q|K|V rows differ in width
+    ("vgg_cnn", 2, 4, 128, 32, 32, 256, 2, 20, 9, 77, 41, True),
+    ("", 2, 2, 64, 32, 64, 128, 3, 50, 11, 33, 161, True),
+))
+def test_flat_params_stack_qkv_projections(b200, feat, L, H, d, dk, dv, di, B, T, Tt, V, freq, tied):
     """optim.FlatParams lays W_q|W_k|W_v (and biases, and their gradients) back to back, which makes ops.AttnProjFn run
     the projections as one stacked GEMM with the weight / bias gradients accumulated straight into the flat buffer
     (self-attention: Q|K|V, encoder-decoder attention: K|V).  Same oracle, same tolerance as the separate-GEMM path."""
     from tests.gpu_util import TOL, cuda_model, cuda_step
     ops = _ops(b200)
     cfg = O.OracleConfig(num_layers=L, num_heads=H, dim_model=d, dim_key=dk, dim_value=dv, dim_inner=di, vocab=V,
-                         feat_extractor=feat, tgt_max_len=Tt, freq=freq)
+                         feat_extractor=feat, tgt_max_len=Tt, freq=freq, emb_trg_sharing=tied)
     P = O.init_params(cfg, seed=5)
     for seed in range(1, 200):
         src, lens, tgt = O.synthetic_batch(cfg, B, T, seed=seed, ragged=True)
@@ -205,7 +220,7 @@ def test_flat_params_stack_qkv_projections(b200, feat, L, H, d, dk, dv, di, B, T
     grads = {n: p.grad.detach().cpu() for n, p in model.named_parameters()}
     assert rel_err(pred.cpu(), pred_o.float()) < TOL
     assert abs(loss.item() - loss_o.item()) < TOL * abs(loss_o.item())
-    assert_grads_close(grads, {k: v.float() for k, v in grads_o.items()}, TOL, exact_kernels=b200.k == 1.0)
+    assert_grads_close(grads, {k: v.float() for k, v in _untie(grads_o, grads).items()}, TOL, exact_kernels=b200.k == 1.0)
 
 
 def _attention_case(ops, B, H, Tq, Tk, dk, dv, mode, seed=0):
@@ -461,18 +476,29 @@ def test_fused_adam_matches_torch(b200):
 
 
 def test_greedy_decode_token_ids_match_oracle(b200):
+    _greedy_decode_matches_oracle(b200, tied=False)
+
+
+def test_greedy_decode_token_ids_match_oracle_tied(b200):
+    """The same with emb_trg_sharing: the logits come from the embedding table itself."""
+    _greedy_decode_matches_oracle(b200, tied=True)
+
+
+def _greedy_decode_matches_oracle(b200, tied):
     """SURVEY.md §8 A18: greedy decode (full-prefix re-decode, argmax per step) gives the oracle's token ids bit-exactly.
     Decoding is compared up to the first step whose oracle top-2 logit margin is inside the rounding band (a near-tie may
     legitimately resolve either way and then changes the rest of the sequence)."""
     from tests.gpu_util import cuda_model
     cfg = O.OracleConfig(num_layers=2, num_heads=4, dim_model=128, dim_key=32, dim_value=32, dim_inner=256, vocab=60,
-                         feat_extractor="", tgt_max_len=40, freq=161)
+                         feat_extractor="", tgt_max_len=40, freq=161, emb_trg_sharing=tied)
     P = O.init_params(cfg, seed=21)
     g = torch.Generator().manual_seed(3)
     for k in P:
         if P[k].dim() == 1:
             P[k] = P[k] + 0.1 * torch.randn(P[k].shape, generator=g)
     P["decoder.output_linear.weight"] = P["decoder.output_linear.weight"] * 4.0       # spread the logits
+    if tied:
+        P["decoder.trg_embedding.weight"] = P["decoder.output_linear.weight"]
     src, lens, _ = O.synthetic_batch(cfg, 3, 30, seed=5, ragged=False)
     enc = O.encoder_forward(O.flatten_features(src), lens, P, cfg)
     ids_o, margins = O.greedy_decode(P, cfg, enc, steps=16)
