@@ -11,7 +11,8 @@ whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
 `spectrogram_batch` returns the device triple `(inputs, input_percentages, input_sizes)`; `collate_waves` returns
 `_collate_fn`'s 5-tuple, sorted, with everything but `inputs` on the host.  `NoiseClips` holds the noise clips' lengths
 and makes the reference's random draws (host data: DataLoader workers draw with it); `NoiseBank` adds the clips on the
-device.  loader.py feeds the reference's AudioDataLoader from here.
+device.  `SpecAugment` is an opt-in augmentation policy both helpers (and loader.py) apply to their output on the device.
+loader.py feeds the reference's AudioDataLoader from here.
 """
 from __future__ import annotations
 
@@ -149,6 +150,77 @@ class NoiseBank:
         return self.device_args(draws.clip, draws.start, draws.level, lengths, device)
 
 
+class SpecAugment:
+    """SpecAugment (Park et al. 2019) for the device front end's batches: a time warp of parameter `W` frames,
+    `n_freq_masks` frequency masks of up to `Fp` bins and `n_time_masks` time masks of up to min(`Tp`, floor(`p` * T_b))
+    frames, applied in that order by one `b200asr_spec_augment` launch per batch (include/b200asr.h states the draws and
+    the fp32 formulas).  Masked bins and frames become 0, the utterance mean of normalised features.
+
+    The paper's policies for LibriSpeech are LB (W=80, Fp=27, n_freq_masks=1, Tp=100, p=1.0, n_time_masks=1) and LD (the
+    same with two masks of each kind); its Switchboard ones are SM (W=40, Fp=15, 2, Tp=70, p=0.2, 2) and SS (W=40, Fp=27, 2,
+    Tp=70, p=0.2, 2).  They were tuned on 80 mel bins every 10 ms; the reference's features are n_fft/2 + 1 = 161
+    linear bins at the same frame rate, so Fp is worth scaling.  Nothing here has a default.
+
+    The draws come from the counter-based generator of dropout keyed by (`seed`, batch counter, utterance, slot): no host
+    draw, no host synchronisation, nothing taken from numpy's, `random`'s or torch's generators.  `counter` counts the
+    batches `apply` has augmented; the same (seed, counter) gives the same augmentation on any device and any rank.  A
+    SpecAugment holds plain numbers, so it pickles (DataLoader workers receive it with the dataset it is attached to)."""
+
+    MAX_MASKS = 64
+
+    def __init__(self, W: int, Fp: int, n_freq_masks: int, Tp: int, p: float, n_time_masks: int, seed: int):
+        ints = dict(W=W, Fp=Fp, n_freq_masks=n_freq_masks, Tp=Tp, n_time_masks=n_time_masks)
+        for name, v in ints.items():
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 0 or v > 2 ** 31 - 1:
+                raise ValueError(f"SpecAugment: {name}={v!r} must be an integer in [0, 2^31 - 1]")
+        for name in ("n_freq_masks", "n_time_masks"):
+            if ints[name] > self.MAX_MASKS:
+                raise ValueError(f"SpecAugment: {name}={ints[name]} exceeds {self.MAX_MASKS}")
+        if isinstance(p, bool) or not isinstance(p, (int, float, np.floating, np.integer)) or not 0.0 <= float(np.float32(p)) <= 1.0:
+            raise ValueError(f"SpecAugment: p={p!r} must lie in [0, 1]")
+        if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
+            raise ValueError(f"SpecAugment: seed={seed!r} must be an integer in [0, 2^64)")
+        self.W, self.Fp, self.n_freq_masks, self.Tp, self.n_time_masks = (int(ints[k]) for k in ints)
+        self.p = float(p)
+        self.seed = int(seed)
+        self.counter = 0
+
+    def __repr__(self):
+        return (f"SpecAugment(W={self.W}, Fp={self.Fp}, n_freq_masks={self.n_freq_masks}, Tp={self.Tp}, p={self.p}, "
+                f"n_time_masks={self.n_time_masks}, seed={self.seed})")
+
+    @property
+    def draws_per_utterance(self) -> int:
+        """c, w, then (f, f0) per frequency mask and (t, t0) per time mask."""
+        return 2 + 2 * self.n_freq_masks + 2 * self.n_time_masks
+
+    def apply(self, inputs: torch.Tensor, input_sizes: torch.Tensor):
+        """Augment `inputs` [B,1,F,T] (CUDA fp32, the front end's layout) whose utterance b has `input_sizes[b]` frames
+        (int, on the host or the device; a host tensor is uploaded without a host synchronisation) with batch counter
+        `self.counter`, which then advances by one.  Returns (augmented [B,1,F,T], draws [B, draws_per_utterance]
+        int32), both new device tensors; `inputs` is left as it is."""
+        ops._need_cuda(inputs)
+        if inputs.dim() != 4 or inputs.shape[1] != 1:
+            raise ValueError(f"SpecAugment.apply: inputs of shape {tuple(inputs.shape)}, not [B, 1, F, T]")
+        B, _, F, T = inputs.shape
+        if self.Fp > F:
+            raise ValueError(f"SpecAugment: Fp={self.Fp} exceeds the {F} frequency bins")
+        if input_sizes.numel() != B:
+            raise ValueError(f"SpecAugment.apply: {input_sizes.numel()} sizes for {B} utterances")
+        x = ops._f32c(inputs)
+        if input_sizes.is_cuda:
+            frames = input_sizes.to(device=x.device, dtype=torch.int32).contiguous()
+        else:
+            frames = _pinned_to(input_sizes.numpy().astype(np.int32), x.device)
+        out = torch.empty_like(x)
+        draws = torch.empty((B, self.draws_per_utterance), device=x.device, dtype=torch.int32)
+        counter, self.counter = self.counter, self.counter + 1
+        L.check(ops._lib().b200asr_spec_augment(L.ptr(x), L.ptr(out), L.ptr(draws), L.ptr(frames), B, F, T, self.W, self.Fp,
+                                                self.n_freq_masks, self.Tp, self.p, self.n_time_masks, self.seed,
+                                                int(counter) & (2 ** 64 - 1), ops._stream()), "spec_augment")
+        return out, draws
+
+
 def _geometry(sample_rate, window_size, window_stride):
     return int(sample_rate * window_size), int(sample_rate * window_stride)
 
@@ -197,11 +269,12 @@ def stft_features_packed(wave: torch.Tensor, offsets: torch.Tensor, lengths: tor
 def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: torch.Tensor | None = None, sample_rate: int = 16000,
                       window_size: float = 0.02, window_stride: float = 0.01, normalize: bool = True, reflect: bool = True,
                       precision: int | None = None, window_periodic: bool = False, window: str = "hamming",
-                      noise: NoiseDraws | None = None, max_frames: int | None = None):
+                      noise: NoiseDraws | None = None, max_frames: int | None = None, spec_augment: SpecAugment | None = None):
     """waves: list of 1-D CUDA float tensors, or a zero-padded [B, L_max] CUDA tensor with `lengths` (int32 samples).
     `window`: "hamming", "hann", "blackman" or "bartlett" (any other name: Hamming, as the reference).  `noise`: draws of
     `NoiseBank.draw` for these utterances, in this order.  `max_frames`: keep at most this many frames of each utterance
-    after normalising over all of them (the reference's src_max_len cut).
+    after normalising over all of them (the reference's src_max_len cut).  `spec_augment`: a SpecAugment applied to the
+    batch after the cut (SpecAugment.apply, which advances its counter); None leaves the features as they are.
     Returns (inputs [B,1,F,T_max] fp32, input_percentages [B] fp32, input_sizes [B] int32), all on the device."""
     n_fft, hop = _geometry(sample_rate, window_size, window_stride)
     if isinstance(waves, torch.Tensor):
@@ -225,11 +298,13 @@ def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: tor
     dev_noise = None if noise is None else noise.bank._device_args(noise, lens.cpu().numpy(), wave.device)
     out, frames = _features(wave, lens, t_max, n_fft, hop, normalize, reflect, precision, window, window_periodic, dev_noise,
                             max_frames)
+    if spec_augment is not None:
+        out, _ = spec_augment.apply(out, frames)
     return out, frames.float() / float(t_max), frames
 
 
 def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBank | None = None, normalize: bool = True,
-                  rng=np.random, precision: int | None = None, reflect: bool = True):
+                  rng=np.random, precision: int | None = None, reflect: bool = True, spec_augment: SpecAugment | None = None):
     """`_collate_fn` (utils/data_loader.py:182-214) over waveforms: what a DataLoader over the reference's
     `SpectrogramDataset` yields, computed on the device.
 
@@ -237,7 +312,8 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     dict train.py builds (sample_rate, window_size, window_stride, window, noise_dir, noise_prob, noise_levels).  With
     audio_conf["noise_dir"] set, noise is drawn from `noise_bank` (ValueError without one) in batch order, before
     sorting, as `__getitem__` draws it.  Each spectrogram is normalised over the whole utterance, then cut to
-    `src_max_len` frames (:131).
+    `src_max_len` frames (:131).  `spec_augment`: a SpecAugment applied to the sorted batch after the cut
+    (SpecAugment.apply, which advances its counter); None leaves the features as they are.
 
     Returns (inputs [B,1,F,T] fp32 on the current CUDA device, targets [B,max_tgt] int64, input_percentages [B] fp32,
     input_sizes [B] int32, target_sizes [B] int32), the last four on the host, sorted by frame count, longest first
@@ -275,6 +351,8 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     for r, t in enumerate(targets_list):
         targets[r, :len(t)] = torch.tensor(list(t), dtype=torch.int32)
     input_sizes = torch.tensor([frames[i] for i in order], dtype=torch.int32)
+    if spec_augment is not None:
+        inputs, _ = spec_augment.apply(inputs, input_sizes)
     input_percentages = torch.tensor([frames[i] / float(t_max) for i in order], dtype=torch.float32)
     target_sizes = torch.tensor([len(t) for t in targets_list], dtype=torch.int32)
     return inputs, targets, input_percentages, input_sizes, target_sizes

@@ -10,6 +10,11 @@ returns the waveform and the draws instead of a spectrogram; `collate_items` sor
 waveforms back to back.  Main side: `audio_loader_init` / `audio_loader_iter` (bound onto AudioDataLoader by install())
 read the noise clips once into a NoiseBank, then upload each batch without a host synchronisation and compute its
 features.
+
+SpecAugment is opt-in per dataset: a SpectrogramDataset with a `spec_augment` attribute (a features.SpecAugment) has it
+applied to every batch after the features, on the device.  Building the loader restarts the policy's batch counter at
+0; the counter then advances once per batch, across epochs.  A dataset without the attribute yields exactly what it
+yields without this feature, and the reference's random draws are untouched either way.
 """
 from __future__ import annotations
 
@@ -131,6 +136,9 @@ class PackedLoader:
         self.inner = DataLoader(**kwargs)
         self.bank = None
         self.reference = False                  # set when the noise clips need the reference's own path (prepare)
+        augment = getattr(ds, "spec_augment", None)
+        if augment is not None:
+            augment.counter = 0
 
     def prepare(self) -> bool:
         """Read the noise clips into a NoiseBank on the current device, once, before any worker starts.  False when the
@@ -173,6 +181,9 @@ class PackedLoader:
             up(pb.wave), up(pb.offsets), up(pb.lengths), max(1, int(lengths.max())), int(pb.input_sizes[0]), sr,
             ds.window_size, ds.window_stride, normalize=ds.normalize, window=_window_name(ds, _data_loader()), noise=noise,
             max_frames=pb.src_max_len)
+        augment = getattr(ds, "spec_augment", None)
+        if augment is not None:
+            inputs, _ = augment.apply(inputs, pb.input_sizes)
         return inputs, pb.targets, pb.input_percentages, pb.input_sizes, pb.target_sizes
 
 
@@ -210,6 +221,9 @@ def audio_loader_iter(self):
     (original(AudioDataLoader, "__iter__")) for a loader without one, without noise clips or with clips at another rate."""
     packed = self.__dict__.get("_b200asr_packed")
     if packed is None or not packed.prepare():
+        if getattr(self.dataset, "spec_augment", None) is not None:     # the reference's iterator would drop it silently
+            raise RuntimeError("the dataset carries spec_augment, which only the device front end applies; this loader "
+                               "runs the reference's own iterator (a collate_fn was given, or the noise clips need sox)")
         from .install import original
         return original(type(self), "__iter__")(self)
     return _Batches(packed)

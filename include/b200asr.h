@@ -670,6 +670,44 @@ int b200asr_stft_features_packed(const float* wave, const long long* offsets, co
                                  const long long* noise_start, const float* noise_level, int max_frames, int precision,
                                  b200asr_stream_t stream);
 
+/* SpecAugment (Park et al. 2019, "SpecAugment: A Simple Data Augmentation Method for Automatic Speech Recognition") over a
+ * batch of the front end's output: in, out [B,1,F,T] fp32 (the layout above), frames [B] int32 (device) = each
+ * utterance's frame count after the src_max_len cut (input_sizes), read as T_b = min(max(frames[b], 0), T).  Applied in
+ * this order over frames [0, T_b) of each utterance; frames t >= T_b of out are 0.
+ *
+ * Draws.  Integer j of utterance b is uniform in [lo, hi]:  lo + ((r >> 32) * (hi - lo + 1)) >> 32  with
+ * r = splitmix64(key + (b << 16 | j) * 0x9E3779B97F4A7C15) and key = splitmix64(seed ^ (counter * 0xD1342543DE82EF95 +
+ * 0x2545F4914F6CDD1D)) -- the counter stream of dropout (common.cuh: dropout_key, dropout_bits4), 64-bit unsigned
+ * arithmetic throughout.  No host draw and no host synchronisation.  draws [B][n] int32 (n =
+ * b200asr_spec_augment_draws_ints(n_freq_masks, n_time_masks) = 2 + 2 n_freq_masks + 2 n_time_masks) receives the
+ * integers used, at their slot j: c, w, then (f, f0) per frequency mask, then (t, t0) per time mask.
+ *
+ * Time warp.  If T_b > 2W + 1: c uniform in [W, T_b - W - 1] (slot 0), w uniform in [-W, W] (slot 1); otherwise no draw
+ *   is made, c = w = 0 and the utterance is not warped (nor is it when w = 0).  With d = c + w, output frame t reads the
+ *   source position s(t) = num / den of the piecewise linear map 0 -> 0, d -> c, T_b - 1 -> T_b - 1 (integers):
+ *     t = 0 or t = T_b - 1:  s = t (the end frames stay put)
+ *     0 < t <= d:            num = t * c,                   den = d,              i0 = num / den
+ *     d < t < T_b - 1:       num = (t - d) * (T_b - 1 - c), den = T_b - 1 - d,    i0 = c + num / den
+ *   rem = num % den; out = x[i0] when rem == 0, else fmaf((float)rem / (float)den, x[i0 + 1] - x[i0], x[i0]) in fp32 --
+ *   linear interpolation between the two neighbouring source frames, x[i0 + 1] read only then (i0 + 1 <= T_b - 1).
+ *   Degenerate segments: with d = 0 (c = W, w = -W) frame 0 still reads frame 0 and frames 1 .. T_b - 2 the second piece,
+ *   which starts from c; with d = T_b - 1 (c = T_b - W - 1, w = W) frame T_b - 1 still reads itself and frames 1 .. T_b - 2
+ *   the first piece, which ends at c.  Integer parts and remainders are exact; the weight is exact for T_b < 2^24.
+ * Frequency masks.  For each of n_freq_masks: f uniform in [0, Fp], f0 uniform in [0, F - f]; bins [f0, f0 + f) become 0.
+ * Time masks.  For each of n_time_masks: t uniform in [0, min(Tp, floor(p * T_b))] (p * T_b in double), t0 uniform in
+ *   [0, T_b - t]; frames [t0, t0 + t) become 0.
+ * 0 is the utterance mean of normalised features.  Masked elements and padding are written as exact zeros.
+ *
+ * One launch; each element is read once (twice where the warp interpolates) and written once.  Rejections, which launch and
+ * write nothing: a NULL pointer (B200ASR_BAD_ARG); a pointer that is not 4-byte aligned (B200ASR_BAD_ALIGN); B, F or T < 1,
+ * B > 65535, F > 1048560 or F * T > 2^31 - 1 (B200ASR_BAD_SHAPE); W < 0, Fp < 0, Fp > F, Tp < 0, p outside [0, 1] or NaN, a mask
+ * count outside [0, 64], or out overlapping in (the warp reads other frames than it writes) (B200ASR_BAD_ARG).
+ * b200asr_spec_augment_draws_ints returns 0 for a mask count outside [0, 64]. */
+size_t b200asr_spec_augment_draws_ints(int n_freq_masks, int n_time_masks);
+int b200asr_spec_augment(const float* in, float* out, int* draws, const int* frames, int B, int F, int T, int W, int Fp,
+                         int n_freq_masks, int Tp, float p, int n_time_masks, unsigned long long seed,
+                         unsigned long long counter, b200asr_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Edit counts of the training loop's CER / WER (trainer/asr/trainer.py:60-79, 96-104 and 153-182), with no host read per
  * token.  Per utterance b the strings h (from hyp row b) and g (from gold row b) are built as the trainer builds them: the
