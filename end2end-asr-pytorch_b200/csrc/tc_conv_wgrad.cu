@@ -10,19 +10,22 @@
 // the dy tile once, converts dy once for all nine taps, and the taps are nine shifted row mappings of the patch, exactly
 // as in the halo forward convolution (tc_conv_halo.cu).
 //
-// Roles (512 threads, 1 CTA / SM, one tile per CTA):
+// Roles (384 threads, 1 CTA / SM, one tile per CTA):
 //   warpgroup 0            producer: warp 0 issues the TMA of the x patch + dy tile of each pixel block into a ring of
 //                          stages; warps 0-3 convert dy -- raw MN-major tile -> K-major hi | lo in the same stage, once for
 //                          all nine taps, with the bias-gradient column sums on the way -- and signal the consumers through
 //                          an mbarrier.
-//   warpgroups 1, 2, 3     consumers: warpgroup w owns taps 3 (w - 1) .. 3 (w - 1) + 2 (df = w - 2, dt = -1 .. 1), i.e. three
-//                          m64n64 accumulator blocks.  Per (tap, 8-pixel k-step) a thread reads its four patch elements
-//                          while the previous k-step's MMAs run, waits for them (wgmma.wait_group 0), splits the elements
-//                          into tf32 hi | lo fragments and issues the MMAs asynchronously.  One fragment buffer: the three
-//                          warpgroups keep the tensor cores fed between each other's waits.
-// The producer warpgroup gives registers to the consumers (setmaxnreg), which need 96 for the accumulators alone.  Even so
-// ptxas (CUDA 12.9) allocates the consumers barely past 128 registers at 512 threads: it spills a few registers once per
-// pixel block and reports C7512 (serialized wgmma) for this kernel.  A second fragment buffer spills more.
+//   warpgroups 1, 2        consumers: warpgroup 1 owns taps 0-4, warpgroup 2 taps 5-8 (tap = 3 (df + 1) + dt + 1), i.e. five
+//                          / four m64n64 accumulator blocks.  A pipeline unit is one (tap, 8-pixel k-step); there are two
+//                          fragment buffers.  While unit u's MMAs run, a thread reads unit u + 1's four patch elements,
+//                          waits for unit u - 1 (wgmma.wait_group 1), splits the elements into the freed buffer's tf32
+//                          hi | lo and issues unit u + 1.  A stage is released one unit late: once the wait in its
+//                          successor's first unit has retired the MMAs of its last unit.
+// Registers (setmaxnreg): the producer warpgroup drops to 40 per thread and the consumers rise to 232, room for 160
+// accumulators, two fragment buffers and the next unit's patch elements.  ptxas (CUDA 12.9) grants the consumers those
+// registers only with one code path for both consumer warpgroups, a warp index it knows to be warp-uniform and a branch
+// between setmaxnreg.inc and the accumulators' zeroing (see the consumer code); then it spills nothing and serializes no
+// wgmma (no C7512, which the 512-thread form with three consumer warpgroups at 152 registers reported).
 //
 // Contraction order inside a k-step: MMA k position j of step ks is pixel (time ks, freq 2j) for j < 4 and (ks, 2j - 7)
 // for j >= 4, so the four lanes q of a quad read patch columns 2q (+1): distinct 128-byte swizzle phases, no bank conflicts.
@@ -45,14 +48,15 @@ constexpr int WH_PATCH_BOX = WH_PT * WH_PF * 128;        // 7,680 B per 32-chann
 constexpr int WH_PATCH_CHUNK = 8192;                     // boxes on 1024-byte boundaries (128B swizzle phase = row & 7)
 constexpr int WH_N = 64;                                 // output channels per tile
 constexpr int WH_PRODUCER = 128;                         // warpgroup 0: TMA (warp 0) and dy conversion (warps 0-3)
-constexpr int WH_CONSUMERS = 384;                        // warpgroups 1-3
+constexpr int WH_CONSUMERS = 256;                        // warpgroups 1, 2
 constexpr int WH_THREADS = WH_PRODUCER + WH_CONSUMERS;
 constexpr int WH_CONVERTERS = WH_PRODUCER / 32;
-// Register split (setmaxnreg): __launch_bounds__(512, 1) allots 128 per thread.  One SM sub-partition holds one producer
-// and three consumer warps, 40 + 3 * 152 = 496 <= 512 registers per lane: room for a consumer's three m64n64 accumulator
-// blocks (96) next to its hi | lo fragments and the next k-step's patch elements.
-constexpr int WH_PRODUCER_REGS = 40, WH_CONSUMER_REGS = 152;
-static_assert(WH_PRODUCER * WH_PRODUCER_REGS + WH_CONSUMERS * WH_CONSUMER_REGS <= WH_THREADS * 128, "register split");
+constexpr int WH_TAPS0 = 5;                              // accumulator blocks per consumer (warpgroup 2 uses four)
+// Register split (setmaxnreg): __launch_bounds__(384, 1) allots 168 per thread; 128 * 40 + 256 * 232 = 384 * 168.  The
+// busier consumer holds five m64n64 accumulator blocks (160) next to two hi | lo fragment buffers (16) and the next unit's
+// patch elements.
+constexpr int WH_PRODUCER_REGS = 40, WH_CONSUMER_REGS = 232;
+static_assert(WH_PRODUCER * WH_PRODUCER_REGS + WH_CONSUMERS * WH_CONSUMER_REGS <= WH_THREADS * 168, "register split");
 constexpr int WH_BAR_CONV = 1;                           // named barrier of the producer warpgroup (bias partials)
 
 struct WgHaloP {
@@ -92,13 +96,18 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   auto ready_bar = [&](int s) { return bar_base + 8u * (S + s); };       // dy hi | lo of stage s written
   auto empty_bar = [&](int s) { return bar_base + 8u * (2 * S + s); };   // the MMAs of stage s completed
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // tile = split z, then (input-channel slice, output-channel slice): the tiles of one split are adjacent CTAs (shared L2)
-  const int groups = p.ncs * p.ncn;
-  const int z = blockIdx.x / groups, grp = blockIdx.x % groups;
-  const int ci0 = (grp / p.ncn) * 64, co0 = (grp % p.ncn) * WH_N;
-  const int blk0 = z * p.blocks_per_cta;
-  const int nkb = max(0, min(p.blocks_per_cta, p.total_blocks - blk0));
+  // the warp index through a shuffle, so that ptxas knows the role branches are warp-uniform (with threadIdx.x >> 5 it
+  // spills in the consumers)
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+  // tile = split z, then (input-channel slice, output-channel slice): the tiles of one split are adjacent CTAs (shared L2).
+  // Each role computes these after setmaxnreg, so that nothing is live across it.
+  struct Tile { int z, ci0, co0, blk0, nkb; };
+  auto tile_of = [&]() {
+    const int groups = p.ncs * p.ncn;
+    const int z = blockIdx.x / groups, grp = blockIdx.x % groups;
+    const int blk0 = z * p.blocks_per_cta;
+    return Tile{z, (grp / p.ncn) * 64, (grp % p.ncn) * WH_N, blk0, max(0, min(p.blocks_per_cta, p.total_blocks - blk0))};
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; s++) {
@@ -117,6 +126,8 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   if (warp < WH_CONVERTERS) {
     // ------------------------------------------------------------------ producer: TMA (warp 0) + dy conversion (warps 0-3)
     setmaxnreg_dec<WH_PRODUCER_REGS>();
+    const Tile t = tile_of();
+    const int z = t.z, ci0 = t.ci0, co0 = t.co0, blk0 = t.blk0, nkb = t.nkb;
     // The loads run S - 1 pixel blocks ahead of warp 0's conversion.  (Not S: the stage of block kb + S is free only once
     // the consumers have moved on to block kb + 1, which waits for this warpgroup's conversion of it.)
     const bool leader = elect_one() && warp == 0;
@@ -189,76 +200,137 @@ tc_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_c
   setmaxnreg_inc<WH_CONSUMER_REGS>();
 
   // -------------------------------------------------------------------- consumers
-  const int wg = (threadIdx.x - WH_PRODUCER) >> 7, cw = warp & 3;
-  const int g = lane >> 2, q = lane & 3;
+  // Every tile the host launches has at least one pixel block.  This check also starts a basic block after
+  // setmaxnreg.inc: with the accumulators zeroed in the block of the setmaxnreg itself, ptxas (CUDA 12.9) spills them and
+  // serializes the wgmma.
+  const Tile t = tile_of();
+  if (t.nkb <= 0) return;
+  // Taps and slots.  Tap (dt, df) reads patch row R = (ks + dt + 1) * WH_PF + df + 1 + 2q + h for pixel (ks, 2q + h) of
+  // k-step ks.  Both warpgroups run one code path (a second inlined path for the second tap set also makes ptxas serialize
+  // and spill).  Relative to patch column 2 wg (wg = 0 / 1: warpgroup 1 / 2), slots 0-2 are rows + 0, 10, 20 (taps 0-2, or
+  // 6-8 for wg = 1), slot 3 is + X with X = 1 (tap 3) or 19 (tap 5), and slot 4, wg = 0 only, + 11 (tap 4).  Slot j
+  // accumulates into block j.
+  const int wg = (warp - WH_CONVERTERS) >> 2, cw = warp & 3, g = lane >> 2, q = lane & 3;
   // A rows of this thread in each tap block: input channels cw * 16 + g and + 8 (same 32-channel box, swizzle chunks cch
-  // and cch + 2); tap 3 * wg + j reads patch row R + pcol, R = (t + j) * WH_PF + h, for pixel (t, 2q + h).  Its 128B
-  // swizzle term depends on (R + pcol) & 7; byte m of sw[m / 4] holds it for R & 7 = m, so that with R known at compile
-  // time a load is a byte extract, an xor and an immediate offset.  (Offsets hoisted per row, or an 8-register table,
-  // would not fit in the register budget next to the accumulators.)
+  // and cch + 2).  A row's 128B swizzle term depends on (R + pcol) & 7; byte m of sw[m / 4] holds it for R & 7 = m, so that
+  // with R known at compile time a load is a byte extract, an xor and an immediate offset.  Slot 3 reads through its own
+  // base (X rows further) and table.
   const int cch = ((cw * 16 + g) & 31) >> 2;
-  const int pcol = wg + 2 * q;
+  const int pcol = 2 * wg + 2 * q, x3 = wg ? 19 : 1;
   const int aoff = (cw >> 1) * WH_PATCH_CHUNK + (g & 3) * 4 + pcol * 128;
-  uint32_t sw[2] = {0u, 0u};
+  uint32_t sw[2] = {0u, 0u}, sw3[2] = {0u, 0u};
 #pragma unroll
-  for (int m = 0; m < 8; m++) sw[m >> 2] |= ((cch ^ ((m + pcol) & 7)) << 4) << (8 * (m & 3));
-  float acc[3][WH_N / 2];
+  for (int m = 0; m < 8; m++) {
+    sw[m >> 2] |= ((cch ^ ((m + pcol) & 7)) << 4) << (8 * (m & 3));
+    sw3[m >> 2] |= ((cch ^ ((m + pcol + x3) & 7)) << 4) << (8 * (m & 3));
+  }
+  float acc[WH_TAPS0][WH_N / 2];
 #pragma unroll
-  for (int j = 0; j < 3; j++)
+  for (int j = 0; j < WH_TAPS0; j++)
 #pragma unroll
     for (int i = 0; i < WH_N / 2; i++) acc[j][i] = 0.f;
-  uint32_t ah[4], al[4];
+  uint32_t ah[2][4], al[2][4];                         // fragment buffer ks % 2 holds k-step ks of a slot
   uint32_t s = 0, ph = 0;
-  for (int kb = 0; kb < nkb; kb++) {
+  const uint8_t* patch = gen_base;
+  uint32_t bhi = 0;
+  auto enter = [&]() {                                 // wait for stage s: x patch landed, dy hi | lo written
     mbar_wait(full_bar(s), ph);
     mbar_wait(ready_bar(s), ph);
-    const uint8_t* patch = gen_base + s * Cfg::kStageBytes + aoff;
-    const uint32_t bhi = smem_base + s * Cfg::kStageBytes + Cfg::kOffHi, blo = bhi + (Cfg::kOffLo - Cfg::kOffHi);
-    asm volatile("" : "+r"(sw[0]), "+r"(sw[1]));     // keeps the extracts below in the loop (see sw)
-    auto ld = [&](int r, int c2) {
-      const uint32_t x = (sw[(r >> 2) & 1] >> (8 * (r & 3))) & 0xFFu;
-      return *reinterpret_cast<const float*>(patch + r * 128 + (x ^ (c2 ? 32 : 0)));
+    patch = gen_base + s * Cfg::kStageBytes + aoff;
+    bhi = smem_base + s * Cfg::kStageBytes + Cfg::kOffHi;
+    asm volatile("" : "+r"(sw[0]), "+r"(sw[1]), "+r"(sw3[0]), "+r"(sw3[1]));   // keeps the extracts in the loop (see sw)
+  };
+  // fragment of (slot sl, k-step ks): a0 = (row g, pixel 2q), a1 = (g + 8, 2q), a2 = (g, 2q + 1), a3 = (g + 8, 2q + 1) of
+  // time row ks
+  auto load = [&](int sl, int ks, float (&x)[4]) {
+    const int r = ks * WH_PF + (sl < 3 ? sl * WH_PF : sl == 4 ? WH_PF + 1 : 0);
+    const uint8_t* base = sl == 3 ? patch + x3 * 128 : patch;
+    const uint32_t* tab = sl == 3 ? sw3 : sw;
+    auto ld = [&](int rr, int c2) {
+      const uint32_t sx = (tab[(rr >> 2) & 1] >> (8 * (rr & 3))) & 0xFFu;
+      return *reinterpret_cast<const float*>(base + rr * 128 + (sx ^ (c2 ? 32 : 0)));
     };
+    x[0] = ld(r, 0);
+    x[1] = ld(r, 1);
+    x[2] = ld(r + 1, 0);
+    x[3] = ld(r + 1, 1);
+  };
+  auto split = [&](int b, const float (&x)[4]) {
 #pragma unroll
-    for (int j = 0; j < 3; j++) {
-#pragma unroll
-      for (int ks = 0; ks < 4; ks++) {
-        const int r = (ks + j) * WH_PF;
-        // fragment: a0 = (row g, pixel 2q), a1 = (g + 8, 2q), a2 = (g, 2q + 1), a3 = (g + 8, 2q + 1) of time row ks;
-        // loaded while the previous k-step's MMAs run
-        const float x[4] = {ld(r, 0), ld(r, 1), ld(r + 1, 0), ld(r + 1, 1)};
-        wgmma_wait<0>();                        // the previous k-step's MMAs are done: the fragment registers are free
-        keep_live(ah);                          // (so far: the compiler must not reuse those registers while they run)
-        if constexpr (NSPLIT == 3) keep_live(al);
-        if (j == 0 && ks == 0 && kb > 0) {      // ... and they were the last ones to read the previous stage
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar(s == 0 ? S - 1 : s - 1));
-        }
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const float h = tf32_rn(x[i]);
-          ah[i] = __float_as_uint(h);
-          if constexpr (NSPLIT == 3) al[i] = __float_as_uint(x[i] - h);
-        }
-        wgmma_fence();
-        if constexpr (NSPLIT == 3) {            // small products first: lo*hi + hi*lo + hi*hi
-          wgmma_tf32<WH_N>(acc[j], al, kmajor_desc_tf32(bhi + ks * 32));
-          wgmma_tf32<WH_N>(acc[j], ah, kmajor_desc_tf32(blo + ks * 32));
-        }
-        wgmma_tf32<WH_N>(acc[j], ah, kmajor_desc_tf32(bhi + ks * 32));
-        wgmma_commit();
-      }
+    for (int i = 0; i < 4; i++) {
+      const float h = tf32_rn(x[i]);
+      ah[b][i] = __float_as_uint(h);
+      if constexpr (NSPLIT == 3) al[b][i] = __float_as_uint(x[i] - h);
     }
-    if (++s == S) { s = 0; ph ^= 1; }
+  };
+  {
+    enter();
+    float x[4];
+    load(0, 0, x);
+    split(0, x);
+  }
+  // Pipeline unit = (slot, k-step), in order slot 0 .. 3 (.. 4), k-steps 0-3 within a slot.  While unit u's MMAs run, unit
+  // u + 1's patch elements are read; the wait then leaves only u in flight, so u - 1's fragment buffer takes u + 1's split.
+  // A stage is released one unit late: the wait in the next pixel block's first unit retires the MMAs of its last unit.
+  int kb = 0;
+  auto unit = [&](int sl, int ks, float (&a)[WH_N / 2], uint32_t bh) {
+    const int b = ks & 1;
+    const uint32_t bl = bh + (Cfg::kOffLo - Cfg::kOffHi);
+    wgmma_fence();
+    if constexpr (NSPLIT == 3) {                       // small products first: lo*hi + hi*lo + hi*hi
+      wgmma_tf32<WH_N>(a, al[b], kmajor_desc_tf32(bh + ks * 32));
+      wgmma_tf32<WH_N>(a, ah[b], kmajor_desc_tf32(bl + ks * 32));
+    }
+    wgmma_tf32<WH_N>(a, ah[b], kmajor_desc_tf32(bh + ks * 32));
+    wgmma_commit();
+    const bool last = ks == 3 && (sl == 4 || (sl == 3 && wg != 0));   // the pixel block's last unit
+    const bool next = !last || kb + 1 < t.nkb;
+    float x[4];
+    if (ks < 3) {
+      load(sl, ks + 1, x);
+    } else if (!last) {
+      load(sl + 1, 0, x);
+    } else if (next) {                                 // the next pixel block's first unit, once its stage is ready
+      if (++s == S) { s = 0; ph ^= 1; }
+      enter();
+      load(0, 0, x);
+    }
+    wgmma_wait<1>();                                   // unit u - 1 is done: its fragment buffer is free
+    keep_live(ah[b ^ 1]);                              // (so far: the compiler must not reuse those registers while it runs)
+    if constexpr (NSPLIT == 3) keep_live(al[b ^ 1]);
+    if (sl == 0 && ks == 0 && kb > 0) {                // ... and it was the last unit of the previous stage
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s == 0 ? S - 1 : s - 1));
+    }
+    if (next) split(b ^ 1, x);
+  };
+  for (; kb < t.nkb; kb++) {
+    const uint32_t bh = bhi;
+#pragma unroll
+    for (int sl = 0; sl < 4; sl++)
+#pragma unroll
+      for (int ks = 0; ks < 4; ks++) unit(sl, ks, acc[sl], bh);
+    if (wg == 0) {
+#pragma unroll
+      for (int ks = 0; ks < 4; ks++) unit(4, ks, acc[4], bh);
+    }
   }
   wgmma_wait<0>();
+  keep_live(ah[0]);
+  keep_live(ah[1]);
+  if constexpr (NSPLIT == 3) {
+    keep_live(al[0]);
+    keep_live(al[1]);
+  }
 #pragma unroll
-  for (int j = 0; j < 3; j++) acc_fence(acc[j]);
+  for (int j = 0; j < WH_TAPS0; j++) acc_fence(acc[j]);
 
   // ---- partials: accumulator (row g (+8), col 8 jj + 2q (+1)) -> [z][tap][ci][co]; a warp stores full 32-byte sectors
 #pragma unroll
-  for (int j = 0; j < 3; j++) {
-    float* o = p.part + (((size_t)z * 9 + 3 * wg + j) * p.Ci + ci0 + cw * 16 + g) * p.Co + co0 + 2 * q;
+  for (int j = 0; j < WH_TAPS0; j++) {
+    if (j == 4 && wg != 0) continue;
+    const int tap = wg == 0 ? j : j < 3 ? 6 + j : 5;
+    float* o = p.part + (((size_t)t.z * 9 + tap) * p.Ci + t.ci0 + cw * 16 + g) * p.Co + t.co0 + 2 * q;
 #pragma unroll
     for (int jj = 0; jj < WH_N / 8; jj++) {
       *reinterpret_cast<float2*>(o + 8 * jj) = make_float2(acc[j][4 * jj], acc[j][4 * jj + 1]);
