@@ -11,8 +11,9 @@ whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
 `spectrogram_batch` returns the device triple `(inputs, input_percentages, input_sizes)`; `collate_waves` returns
 `_collate_fn`'s 5-tuple, sorted, with everything but `inputs` on the host.  `NoiseClips` holds the noise clips' lengths
 and makes the reference's random draws (host data: DataLoader workers draw with it); `NoiseBank` adds the clips on the
-device.  `SpecAugment` is an opt-in augmentation policy both helpers (and loader.py) apply to their output on the device.
-loader.py feeds the reference's AudioDataLoader from here.
+device.  `SpecAugment` is an opt-in augmentation policy both helpers (and loader.py) apply to their output on the device;
+`TempoGain` (with `tempo_gain`) is the reference's tempo and gain perturbation, which collate_waves (and loader.py) apply to
+the waveforms before the features.  loader.py feeds the reference's AudioDataLoader from here.
 """
 from __future__ import annotations
 
@@ -124,7 +125,10 @@ class NoiseBank:
 
     def draw(self, lengths, noise_prob: float, noise_levels, rng=np.random) -> NoiseDraws:
         """NoiseClips.draw_one for utterances of `lengths` samples, in batch order."""
-        rows = [self.clips.draw_one(n, noise_prob, noise_levels, rng) for n in lengths]
+        return self._draws([self.clips.draw_one(n, noise_prob, noise_levels, rng) for n in lengths])
+
+    def _draws(self, rows) -> NoiseDraws:
+        """NoiseDraws from NoiseClips.draw_one's rows, in batch order."""
         add, clip, level, rand, start = (np.array(col, dtype=dt).reshape(-1) for col, dt in
                                          zip(zip(*rows) if rows else ((),) * 5,
                                              (np.int64, np.int64, np.float64, np.float64, np.int64)))
@@ -221,6 +225,135 @@ class SpecAugment:
         return out, draws
 
 
+class TempoGain:
+    """The reference's `--augment` (`load_randomly_augmented_audio`, utils/audio.py:50-61) on the device: per utterance a
+    tempo uniform in `tempo_range` and a gain uniform in `gain_range` dB, applied by `tempo_gain` (WSOLA modelled on sox's
+    `tempo` effect, then `gain` and a 16-bit output; include/b200asr.h states the algorithm).  The defaults are the
+    reference's ranges.  Parity with sox itself is not pinned: the restated algorithm is the contract.
+
+    A TempoGain holds plain numbers, so it pickles (DataLoader workers receive it with the dataset it is attached to)."""
+
+    TEMPO_LIMITS = (0.25, 4.0)
+
+    def __init__(self, tempo_range=(0.85, 1.15), gain_range=(-6, 8)):
+        self.tempo_range = self._range("tempo_range", tempo_range)
+        self.gain_range = self._range("gain_range", gain_range)
+        lo, hi = self.TEMPO_LIMITS
+        if not (lo <= self.tempo_range[0] and self.tempo_range[1] <= hi):
+            raise ValueError(f"TempoGain: tempo_range={tempo_range!r} must lie in [{lo}, {hi}]")
+
+    @staticmethod
+    def _range(name, r):
+        try:
+            a, b = r
+        except (TypeError, ValueError):
+            raise ValueError(f"TempoGain: {name}={r!r} is not a (low, high) pair") from None
+        for v in (a, b):
+            if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)) or not np.isfinite(v):
+                raise ValueError(f"TempoGain: {name}={r!r} needs two finite numbers")
+        if a > b:
+            raise ValueError(f"TempoGain: {name}={r!r} has low > high")
+        return float(a), float(b)
+
+    def __repr__(self):
+        return f"TempoGain(tempo_range={self.tempo_range}, gain_range={self.gain_range})"
+
+    def draw_one(self, rng=np.random):
+        """load_randomly_augmented_audio's draws for one utterance, with its numpy calls in its order: uniform over the
+        tempo range, then over the gain range; each rounded as the sox command line writes it ("{:.3f}").  `rng` is
+        np.random (the reference's global state) or a RandomState.  Returns (tempo, gain_db)."""
+        tempo = rng.uniform(low=self.tempo_range[0], high=self.tempo_range[1])
+        gain = rng.uniform(low=self.gain_range[0], high=self.gain_range[1])
+        return float(f"{tempo:.3f}"), float(f"{gain:.3f}")
+
+    @staticmethod
+    def geometry(sample_rate) -> tuple[int, int, int]:
+        """(segment, search, overlap) in samples of sox's default tempo profile at `sample_rate`, in float64: (1312, 235,
+        192) at 16 kHz.  ValueError for a rate too low to give a valid geometry."""
+        sr = float(sample_rate)
+        segment = int(np.floor(sr * 82 / 1000 + 0.5))
+        search = int(np.floor(sr * (82 / 5.587) / 1000 + 0.5))
+        overlap = int(np.floor(max(sr * (82 / 6.833) / 1000 + 4.5, 16)))
+        overlap -= overlap % 8
+        if 2 * overlap > segment:
+            overlap -= 8
+        if not (np.isfinite(sr) and search >= 1 and overlap >= 8 and 2 * overlap <= segment):
+            raise ValueError(f"TempoGain: sample_rate={sample_rate!r} gives no valid geometry ({segment}, {search}, {overlap})")
+        return segment, search, overlap
+
+    @staticmethod
+    def out_length(n: int, tempo: float) -> int:
+        """Samples of the output for `n` input samples: floor(n / tempo + 0.5) in float64."""
+        return int(np.floor(int(n) / float(tempo) + 0.5))
+
+    @staticmethod
+    def linear_gain(gain_db: float) -> np.float32:
+        """fp32(10^(gain_db / 20)), computed in float64."""
+        return np.float32(10.0 ** (float(gain_db) / 20.0))
+
+
+def _tempo_gain(wave, offsets, lengths, tempo, g, out_lengths, sample_rate, picks=False):
+    """One b200asr_tempo_gain launch.  wave, offsets, lengths on the device; tempo (float64), g (fp32) and out_lengths
+    (int) host arrays, or pinned CPU tensors; the outputs back to back in batch order."""
+    segment, search, overlap = TempoGain.geometry(sample_rate)
+    device = wave.device
+    up = lambda a, dt: a.to(device, non_blocking=True) if isinstance(a, torch.Tensor) else _pinned_to(np.asarray(a, dt), device)  # noqa: E731
+    out_np = np.asarray(out_lengths.numpy() if isinstance(out_lengths, torch.Tensor) else out_lengths, dtype=np.int64).reshape(-1)
+    B = len(out_np)
+    out_offsets = np.concatenate([[0], np.cumsum(out_np)[:-1]]).astype(np.int64)
+    out = torch.empty(max(1, int(out_np.sum())), device=device, dtype=torch.float32)
+    out_off_d, out_len_d = _pinned_to(out_offsets, device), up(out_lengths, np.int32)
+    pk = pk_off = pk_off_d = None
+    if picks:
+        K = -(-out_np // (segment - overlap))
+        pk_off = np.concatenate([[0], np.cumsum(K)[:-1]]).astype(np.int64)
+        pk = torch.empty(max(1, int(K.sum())), device=device, dtype=torch.int32)
+        pk_off_d = _pinned_to(pk_off, device)
+    tempo_d, g_d = up(tempo, np.float64), up(g, np.float32)      # held until the launch: a freed block would be reused
+    L.check(ops._lib().b200asr_tempo_gain(
+        L.ptr(wave), L.ptr(offsets), L.ptr(lengths), L.ptr(tempo_d), L.ptr(g_d), L.ptr(out), L.ptr(out_off_d),
+        L.ptr(out_len_d), L.ptr(pk), L.ptr(pk_off_d), B, segment, search, overlap, ops._stream()), "tempo_gain")
+    return out, out_off_d, out_len_d, pk, pk_off
+
+
+def tempo_gain(wave: torch.Tensor, offsets, lengths, tempo, gain_db, sample_rate: int, picks: bool = False):
+    """Tempo and gain perturbation of a packed batch (`TempoGain`'s algorithm, include/b200asr.h): utterance b is the
+    lengths[b] samples of the 1-D CUDA fp32 `wave` from offsets[b] on (int64; a CUDA tensor, or host data uploaded).
+    `lengths` (int32), `tempo` and `gain_db` (one per utterance) are host data: the output lengths are computed from them
+    on the host, so there is no host synchronisation; they are uploaded through pinned memory.  One launch.
+
+    Per utterance: out_length = floor(n / tempo + 0.5) samples of WSOLA at sox's default geometry for `sample_rate`
+    (TempoGain.geometry), scaled by fp32(10^(gain_db / 20)) and quantised to 16 bits (clamp(rint(32768 v), -32768,
+    32767) / 32768, so gains above 0 dB clip loud utterances).  Segment k starts at input sample floor(tempo * k * step +
+    0.5) plus its pick p_k, the smallest offset in [0, search) minimising the float64 sum of squared differences to the
+    overlap that follows the previous segment (p_0 = search // 2); segments crossfade linearly over `overlap` samples.
+
+    Returns (out, out_offsets, out_lengths): the outputs back to back in batch order (a 1-D CUDA fp32 tensor, at least
+    one element), their int64 offsets and int32 lengths on the device.  With picks=True also (picks, pick_offsets): every
+    utterance's ceil(out_length / step) picks (int32, device) from its host int64 offset on."""
+    ops._need_cuda(wave)
+    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
+        raise ValueError("tempo_gain: lengths must be host data (the output lengths are computed on the host)")
+    lens = np.asarray(lengths.numpy() if isinstance(lengths, torch.Tensor) else lengths, dtype=np.int64).reshape(-1)
+    tempo = np.asarray(tempo, dtype=np.float64).reshape(-1)
+    gain_db = np.asarray(gain_db, dtype=np.float64).reshape(-1)
+    B = len(lens)
+    if not B or len(tempo) != B or len(gain_db) != B:
+        raise ValueError(f"tempo_gain: {B} lengths, {len(tempo)} tempos and {len(gain_db)} gains")
+    if not (np.isfinite(tempo).all() and (tempo > 0).all()):
+        raise ValueError("tempo_gain: every tempo must be finite and positive")
+    device = wave.device
+    offs = offsets.to(device, torch.int64, non_blocking=True) if isinstance(offsets, torch.Tensor) else \
+        _pinned_to(np.asarray(offsets, np.int64), device)
+    if offs.numel() != B:
+        raise ValueError(f"tempo_gain: {offs.numel()} offsets for {B} utterances")
+    out_lengths = np.array([TempoGain.out_length(n, t) for n, t in zip(lens, tempo)], dtype=np.int32)
+    g = np.array([TempoGain.linear_gain(d) for d in gain_db], dtype=np.float32)
+    out, out_off, out_len, pk, pk_off = _tempo_gain(ops._f32c(wave), offs, _pinned_to(lens.astype(np.int32), device), tempo,
+                                                    g, out_lengths, sample_rate, picks)
+    return (out, out_off, out_len, pk, pk_off) if picks else (out, out_off, out_len)
+
+
 def _geometry(sample_rate, window_size, window_stride):
     return int(sample_rate * window_size), int(sample_rate * window_stride)
 
@@ -304,7 +437,8 @@ def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: tor
 
 
 def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBank | None = None, normalize: bool = True,
-                  rng=np.random, precision: int | None = None, reflect: bool = True, spec_augment: SpecAugment | None = None):
+                  rng=np.random, precision: int | None = None, reflect: bool = True, spec_augment: SpecAugment | None = None,
+                  tempo_gain: TempoGain | None = None):
     """`_collate_fn` (utils/data_loader.py:182-214) over waveforms: what a DataLoader over the reference's
     `SpectrogramDataset` yields, computed on the device.
 
@@ -313,7 +447,10 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     audio_conf["noise_dir"] set, noise is drawn from `noise_bank` (ValueError without one) in batch order, before
     sorting, as `__getitem__` draws it.  Each spectrogram is normalised over the whole utterance, then cut to
     `src_max_len` frames (:131).  `spec_augment`: a SpecAugment applied to the sorted batch after the cut
-    (SpecAugment.apply, which advances its counter); None leaves the features as they are.
+    (SpecAugment.apply, which advances its counter); None leaves the features as they are.  `tempo_gain`: a TempoGain
+    (the reference's `augment=True`): each utterance draws its tempo and gain, then its noise for the stretched length,
+    in batch order as `__getitem__` draws them, and the batch is stretched on the device (one `tempo_gain` launch)
+    before the features; the frame counts are those of the stretched utterances.  None: no stretch and no such draw.
 
     Returns (inputs [B,1,F,T] fp32 on the current CUDA device, targets [B,max_tgt] int64, input_percentages [B] fp32,
     input_sizes [B] int32, target_sizes [B] int32), the last four on the host, sorted by frame count, longest first
@@ -325,14 +462,29 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
         raise ValueError(f"src_max_len={src_max_len}")
     waves = [np.asarray(w.detach().cpu() if isinstance(w, torch.Tensor) else w, dtype=np.float32).reshape(-1) for w, _ in batch]
     lens = [len(w) for w in waves]
+    noisy = audio_conf.get("noise_dir") is not None
+    if noisy and noise_bank is None:
+        raise ValueError("audio_conf['noise_dir'] is set but no noise_bank was given")
     draws = None
-    if audio_conf.get("noise_dir") is not None:
-        if noise_bank is None:
-            raise ValueError("audio_conf['noise_dir'] is set but no noise_bank was given")
-        draws = noise_bank.draw(lens, audio_conf["noise_prob"], audio_conf["noise_levels"], rng)
-    frames = [min(1 + n // hop, src_max_len) for n in lens]
+    if tempo_gain is None:
+        if noisy:
+            draws = noise_bank.draw(lens, audio_conf["noise_prob"], audio_conf["noise_levels"], rng)
+        out_lens = lens
+    else:
+        TempoGain.geometry(sr)                        # a rate without a valid geometry fails before any draw
+        stretch, rows, out_lens = [], [], []
+        for n in lens:                                # per utterance: tempo and gain, then the noise of the stretched length
+            t, gain_db = tempo_gain.draw_one(rng)
+            m = TempoGain.out_length(n, t)
+            stretch.append((t, TempoGain.linear_gain(gain_db)))
+            out_lens.append(m)
+            if noisy:
+                rows.append(noise_bank.clips.draw_one(m, audio_conf["noise_prob"], audio_conf["noise_levels"], rng))
+        if noisy:
+            draws = noise_bank._draws(rows)
+    frames = [min(1 + n // hop, src_max_len) for n in out_lens]
     order = sorted(range(len(batch)), key=frames.__getitem__, reverse=True)          # sorted(..., reverse=True) is stable
-    B, Lmax = len(batch), max(1, max(lens))
+    B, Lmax = len(batch), max(1, max(out_lens))
     slens = np.array([lens[i] for i in order], dtype=np.int32)
     offsets = np.concatenate([[0], np.cumsum(slens, dtype=np.int64)[:-1]])
     host = torch.empty(max(1, int(slens.sum())), dtype=torch.float32, pin_memory=True)   # back to back, uploaded without a sync
@@ -340,11 +492,16 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     for r, i in enumerate(order):
         h[offsets[r]:offsets[r] + lens[i]] = waves[i]
     device = torch.device("cuda", torch.cuda.current_device())
-    dev_noise = None if draws is None else noise_bank._device_args(draws.take(order), slens, device)
+    wave, wave_offsets, wave_lens = host.to(device, non_blocking=True), _pinned_to(offsets, device), _pinned_to(slens, device)
+    if tempo_gain is not None:
+        wave, wave_offsets, wave_lens, _, _ = _tempo_gain(
+            wave, wave_offsets, wave_lens, np.array([stretch[i][0] for i in order], np.float64),
+            np.array([stretch[i][1] for i in order], np.float32), np.array([out_lens[i] for i in order], np.int32), sr)
+    sout = np.array([out_lens[i] for i in order], dtype=np.int64)
+    dev_noise = None if draws is None else noise_bank._device_args(draws.take(order), sout, device)
     t_max = frames[order[0]]
-    inputs, _ = _features(host.to(device, non_blocking=True), _pinned_to(slens, device), t_max, n_fft, hop, normalize, reflect,
-                          precision, audio_conf.get("window", "hamming"), False, dev_noise, src_max_len,
-                          offsets=_pinned_to(offsets, device), Lmax=Lmax)
+    inputs, _ = _features(wave, wave_lens, t_max, n_fft, hop, normalize, reflect, precision, audio_conf.get("window", "hamming"),
+                          False, dev_noise, src_max_len, offsets=wave_offsets, Lmax=Lmax)
     targets_list = [batch[i][1] for i in order]
     max_tgt = max(len(t) for t in targets_list)
     targets = torch.zeros(B, max_tgt, dtype=torch.int64)

@@ -15,6 +15,13 @@ SpecAugment is opt-in per dataset: a SpectrogramDataset with a `spec_augment` at
 applied to every batch after the features, on the device.  Building the loader restarts the policy's batch counter at
 0; the counter then advances once per batch, across epochs.  A dataset without the attribute yields exactly what it
 yields without this feature, and the reference's random draws are untouched either way.
+
+Tempo and gain perturbation is opt-in per dataset too: a SpectrogramDataset with `augment=True` and a `tempo_gain`
+attribute (a features.TempoGain) has its workers read the audio with the reference's `load_audio` and make
+`load_randomly_augmented_audio`'s two draws with `TempoGain.draw_one`, instead of running sox; the noise draw and the
+frame count use the stretched length, and each batch is stretched on the device (one `b200asr_tempo_gain` launch) before
+its features.  An `augment=True` dataset without the attribute keeps the reference's sox path; the attribute on an
+`augment=False` dataset is a ValueError when the loader is built.
 """
 from __future__ import annotations
 
@@ -32,19 +39,26 @@ from . import features
 
 class Item(NamedTuple):
     """One utterance as a worker returns it: the waveform (fp32), the noise draw as (clip index, first sample in the
-    bank, level) -- (-1, -1, NaN) without noise --, the transcript ids and the frame count after the src_max_len cut."""
+    bank, level) -- (-1, -1, NaN) without noise --, the transcript ids and the frame count after the src_max_len cut.
+    With a dataset's tempo_gain: the tempo, the linear gain fp32(10^(gain_db / 20)) and the stretched length `out_length`
+    that `wave` (the unstretched audio) becomes on the device; out_length -1 (the default) when nothing is stretched."""
     wave: np.ndarray
     noise_clip: int
     noise_start: int
     noise_level: float
     ids: list
     frames: int
+    tempo: float = 1.0
+    g: float = 1.0
+    out_length: int = -1
 
 
 class PackedBatch(NamedTuple):
     """A batch as the workers collate it, sorted as `_collate_fn` sorts (frames, longest first, stable): the waveforms
     back to back (`wave`, at least one sample) at int64 `offsets` with int32 `lengths`; per utterance the noise clip,
-    start (int64, -1 without noise) and level (fp32); `_collate_fn`'s four host tensors; the src_max_len of the cut."""
+    start (int64, -1 without noise) and level (fp32); `_collate_fn`'s four host tensors; the src_max_len of the cut.
+    With a dataset's tempo_gain: per utterance the tempo (float64), linear gain (fp32) and stretched length (int32) the
+    waveforms are stretched with before their features; None (the default) when nothing is stretched."""
     wave: torch.Tensor
     offsets: torch.Tensor
     lengths: torch.Tensor
@@ -56,6 +70,9 @@ class PackedBatch(NamedTuple):
     input_sizes: torch.Tensor
     target_sizes: torch.Tensor
     src_max_len: int
+    tempo: torch.Tensor | None = None
+    g: torch.Tensor | None = None
+    out_lengths: torch.Tensor | None = None
 
 
 def _data_loader():
@@ -78,19 +95,28 @@ class PackedItems(Dataset):
         ds, DL = self.dataset, _data_loader()
         ids = ds.ids_list[random.randint(0, len(ds.ids_list) - 1)]            # __getitem__ (:127-130)
         audio_path, transcript_path = ids[index % len(ids)][:2]
-        if ds.augment:                                                        # parse_audio (:61-70)
+        policy = getattr(ds, "tempo_gain", None) if ds.augment else None
+        stretch = ()
+        if policy is not None:                                                # the stretch is made on the device
+            y = DL.load_audio(audio_path)
+            tempo, gain_db = policy.draw_one(np.random)                      # load_randomly_augmented_audio's draws
+        elif ds.augment:                                                      # parse_audio (:61-70)
             y = DL.load_randomly_augmented_audio(audio_path, ds.sample_rate)
         else:
             y = DL.load_audio(audio_path)
         y = np.ascontiguousarray(y, dtype=np.float32).reshape(-1)
+        n = len(y)
+        if policy is not None:
+            n = policy.out_length(n, tempo)
+            stretch = (tempo, float(policy.linear_gain(gain_db)), n)
         clip, start, level = -1, -1, float("nan")
         if ds.noiseInjector:
             if self.clips is None:
                 raise RuntimeError("PackedItems: the dataset injects noise but no noise clips were given")
-            _, clip, level, _, start = self.clips.draw_one(len(y), ds.noise_prob, ds.noiseInjector.noise_levels, np.random)
+            _, clip, level, _, start = self.clips.draw_one(n, ds.noise_prob, ds.noiseInjector.noise_levels, np.random)
         transcript = ds.parse_transcript(transcript_path)
         src_max_len = importlib.import_module("utils.constant").args.src_max_len      # read at call time, as :131
-        return Item(y, clip, start, level, transcript, min(1 + len(y) // self.hop, src_max_len))
+        return Item(y, clip, start, level, transcript, min(1 + n // self.hop, src_max_len), *stretch)
 
 
 def collate_items(items) -> PackedBatch:
@@ -105,6 +131,14 @@ def collate_items(items) -> PackedBatch:
     targets = torch.zeros(B, max_tgt, dtype=torch.int64)
     for r, it in enumerate(items):
         targets[r, :len(it.ids)] = torch.tensor(list(it.ids), dtype=torch.int32)
+    stretched = [it.out_length >= 0 for it in items]
+    if any(stretched) and not all(stretched):
+        raise ValueError("collate_items: a batch mixes stretched and unstretched utterances")
+    stretch = {}
+    if all(stretched):
+        stretch = dict(tempo=torch.tensor([it.tempo for it in items], dtype=torch.float64),
+                       g=torch.tensor([it.g for it in items], dtype=torch.float32),
+                       out_lengths=torch.tensor([it.out_length for it in items], dtype=torch.int32))
     return PackedBatch(
         wave=torch.from_numpy(wave),
         offsets=torch.from_numpy(np.concatenate([[0], np.cumsum(lengths)[:-1]]).astype(np.int64)),
@@ -116,7 +150,7 @@ def collate_items(items) -> PackedBatch:
         input_percentages=torch.tensor([it.frames / float(t_max) for it in items], dtype=torch.float32),
         input_sizes=torch.tensor([it.frames for it in items], dtype=torch.int32),
         target_sizes=torch.tensor([len(it.ids) for it in items], dtype=torch.int32),
-        src_max_len=int(importlib.import_module("utils.constant").args.src_max_len))
+        src_max_len=int(importlib.import_module("utils.constant").args.src_max_len), **stretch)
 
 
 def _window_name(ds, DL) -> str:
@@ -172,13 +206,17 @@ class PackedLoader:
         ds = self.items.dataset
         device = torch.device("cuda", torch.cuda.current_device())
         up = lambda t: t.to(device, non_blocking=True)          # noqa: E731
+        sr = ds.sample_rate
+        wave, offsets, lengths_d = up(pb.wave), up(pb.offsets), up(pb.lengths)
         lengths = pb.lengths.numpy()
+        if pb.out_lengths is not None:                          # the stretched waveforms replace the read ones
+            wave, offsets, lengths_d, _, _ = features._tempo_gain(wave, offsets, lengths_d, pb.tempo, pb.g, pb.out_lengths, sr)
+            lengths = pb.out_lengths.numpy()
         noise = None
         if self.bank is not None:
             noise = self.bank.device_args(pb.noise_clip.numpy(), pb.noise_start, pb.noise_level, lengths, device)
-        sr = ds.sample_rate
         inputs, _ = features.stft_features_packed(
-            up(pb.wave), up(pb.offsets), up(pb.lengths), max(1, int(lengths.max())), int(pb.input_sizes[0]), sr,
+            wave, offsets, lengths_d, max(1, int(lengths.max())), int(pb.input_sizes[0]), sr,
             ds.window_size, ds.window_stride, normalize=ds.normalize, window=_window_name(ds, _data_loader()), noise=noise,
             max_frames=pb.src_max_len)
         augment = getattr(ds, "spec_augment", None)
@@ -205,6 +243,12 @@ class _Batches:
         return self.packed.batch(next(self.it))
 
 
+def _check_tempo_gain(ds):
+    if getattr(ds, "tempo_gain", None) is not None and not getattr(ds, "augment", False):
+        raise ValueError("the dataset carries tempo_gain but was built with augment=False: the reference would not "
+                         "perturb its tempo and gain")
+
+
 def audio_loader_init(self, *args, **kwargs):
     """AudioDataLoader.__init__ after install(): the reference's own construction (so `dataset`, `sampler`, `len()` are
     its), plus a PackedLoader unless the dataset is not a SpectrogramDataset or the caller passed a collate_fn."""
@@ -212,6 +256,7 @@ def audio_loader_init(self, *args, **kwargs):
     original(type(self), "__init__")(self, *args, **kwargs)
     arguments = inspect.signature(DataLoader.__init__).bind(self, *args, **kwargs).arguments
     arguments.pop("self")
+    _check_tempo_gain(self.dataset)
     eligible = isinstance(self.dataset, _data_loader().SpectrogramDataset) and arguments.get("collate_fn") is None
     self._b200asr_packed = PackedLoader(self, dict(arguments)) if eligible else None
 
@@ -221,9 +266,10 @@ def audio_loader_iter(self):
     (original(AudioDataLoader, "__iter__")) for a loader without one, without noise clips or with clips at another rate."""
     packed = self.__dict__.get("_b200asr_packed")
     if packed is None or not packed.prepare():
-        if getattr(self.dataset, "spec_augment", None) is not None:     # the reference's iterator would drop it silently
-            raise RuntimeError("the dataset carries spec_augment, which only the device front end applies; this loader "
-                               "runs the reference's own iterator (a collate_fn was given, or the noise clips need sox)")
+        for attr in ("spec_augment", "tempo_gain"):                      # the reference's iterator would drop it silently
+            if getattr(self.dataset, attr, None) is not None:
+                raise RuntimeError(f"the dataset carries {attr}, which only the device front end applies; this loader "
+                                   "runs the reference's own iterator (a collate_fn was given, or the noise clips need sox)")
         from .install import original
         return original(type(self), "__iter__")(self)
     return _Batches(packed)

@@ -670,6 +670,45 @@ int b200asr_stft_features_packed(const float* wave, const long long* offsets, co
                                  const long long* noise_start, const float* noise_level, int max_frames, int precision,
                                  b200asr_stream_t stream);
 
+/* Tempo and gain perturbation of a packed batch of waveforms: WSOLA (waveform-similarity overlap-add), modelled on sox's
+ * `tempo` effect with its default profile (linear search; 82 ms segment, 82/5.587 ms search, 82/6.833 ms overlap), then
+ * `gain` and the 16-bit output of the reference's `sox ... -b 16 -e si ... tempo T gain G` (utils/audio.py:35-47).  Parity
+ * with sox itself is not claimed (sox may add TPDF dither when it writes 16 bits); the algorithm below is the contract.
+ *
+ * Utterance b: x = the in_lengths[b] fp32 samples at in + in_offsets[b], read as x~, x extended to the right with zeros
+ * (nothing outside [in_offsets[b], in_offsets[b] + in_lengths[b]) is read); tempo[b] (float64) and the linear gain g[b]
+ * (fp32, the caller's fp32(10^(gain_db / 20)) computed in float64); its output is the out_lengths[b] samples at
+ * out + out_offsets[b].  The geometry is the caller's (the host layer computes it from the sample rate sr in float64:
+ * segment = floor(sr * 82 / 1000 + 0.5), search = floor(sr * (82 / 5.587) / 1000 + 0.5), overlap = floor(max(sr *
+ * (82 / 6.833) / 1000 + 4.5, 16)) rounded down to a multiple of 8, minus 8 if 2 * overlap > segment; at 16 kHz (1312, 235,
+ * 192)).  step = segment - overlap; the caller's out_lengths[b] = floor(n / tempo + 0.5) and K_b = ceil(out_lengths[b] /
+ * step) segments.
+ *   Segment k: input start S_k = floor(tempo * (k * step) + 0.5) in float64 (k * step an exact integer), independent of any
+ *   pick.  Pick p_0 = floor(search / 2); for k >= 1, with prev_j = x~[S_{k-1} + p_{k-1} + step + j] (j < overlap), p_k is the
+ *   smallest i in [0, search) minimising D(i) = sum_j (x~[S_k + i + j] - prev_j)^2 computed in float64 (a NaN D counts as
+ *   +inf).  On inputs from 16-bit files (k / 32768) every term and partial sum of D is exact, so the picks do not depend
+ *   on the summation order.  Segment k writes y[k * step + j] for j < step: x~[S_k + p_k + j], except for k >= 1 and
+ *   j < overlap the crossfade fp32(fp32(prev_j * fp32(1 - f_j)) + fp32(x~[S_k + p_k + j] * f_j)), f_j = fp32(j * fp32(1 /
+ *   overlap)), every operation rounded on its own (no FMA).
+ *   Output: v = fp32(y * g), written as clamp(rint(v * 32768), -32768, 32767) / 32768 (half to even; NaN stays NaN) --
+ *   what load_audio returns for a 16-bit file; gains above 0 dB clip loud utterances.  Samples k * step + j >=
+ *   out_lengths[b] are not written.
+ * picks, pick_offsets: NULL together, or p_k written to picks[pick_offsets[b] + k] for k < K_b (int32 / int64 device arrays).
+ *
+ * One launch, one CTA per utterance walking its K_b segments in order (the next window prefetched while one is searched).
+ * Rejections, which launch and write nothing: a NULL pointer other than picks / pick_offsets, or exactly one of those
+ * two NULL (B200ASR_BAD_ARG); in, in_lengths, g, out, out_lengths or picks not 4-byte, in_offsets, tempo, out_offsets or
+ * pick_offsets not 8-byte aligned (B200ASR_BAD_ALIGN); B < 1, overlap < 8, 2 * overlap > segment, search < 1, or a
+ * geometry whose 8 (3 overlap + search - 1) + 8 (search + segment - 1) bytes of shared memory exceed 226 KB
+ * (B200ASR_BAD_SHAPE).  The per-utterance arrays are device data, which the library does not read on the host: an
+ * utterance with a non-finite or non-positive tempo, a negative in_offsets or a negative in_lengths gets NaN for its
+ * out_lengths[b] samples and -1 for its picks; one with a negative out_offsets or out_lengths[b] <= 0 writes nothing (nor
+ * does a negative pick_offsets write picks).  out must not overlap in. */
+int b200asr_tempo_gain(const float* in, const long long* in_offsets, const int* in_lengths, const double* tempo,
+                       const float* g, float* out, const long long* out_offsets, const int* out_lengths, int* picks,
+                       const long long* pick_offsets, int B, int segment, int search, int overlap,
+                       b200asr_stream_t stream);
+
 /* SpecAugment (Park et al. 2019, "SpecAugment: A Simple Data Augmentation Method for Automatic Speech Recognition") over a
  * batch of the front end's output: in, out [B,1,F,T] fp32 (the layout above), frames [B] int32 (device) = each
  * utterance's frame count after the src_max_len cut (input_sizes), read as T_b = min(max(frames[b], 0), T).  Applied in
