@@ -6,8 +6,8 @@ needs the built library and an H100.
 """
 from . import _lib, lm_train
 from .config import ASRConfig, BASELINE_CONFIGS
-from .features import (NoiseBank, NoiseClips, SpecAugment, TempoGain, collate_waves, spectrogram_batch, stft_features_packed,
-                       tempo_gain)
+from .features import (NoiseBank, NoiseClips, SpecAugment, SpeedPerturb, TempoGain, collate_waves, resample,
+                       spectrogram_batch, stft_features_packed, tempo_gain)
 from .install import install, original, uninstall
 from .metrics import LabelTable, calculate_loss, calculate_metrics, edit_counts, loss_and_stats
 from .modules import (LM, Decoder, DecoderLayer, Encoder, EncoderLayer, MultiHeadAttention, PositionalEncoding,
@@ -19,4 +19,4 @@ from .parallel import DataParallelStep, HostBatchPrefetcher, shard_batch
 __all__ = ["ASRConfig", "BASELINE_CONFIGS", "install", "uninstall", "original", "calculate_loss", "calculate_metrics",
            "loss_and_stats", "LabelTable", "edit_counts","Transformer", "Encoder", "Decoder", "EncoderLayer", "DecoderLayer", "MultiHeadAttention",
            "ScaledDotProductAttention", "PositionwiseFeedForwardWithConv", "PositionalEncoding", "build_model", "RNNModel", "LM",
-           "precision", "manual_seed", "attention_maps", "spectrogram_batch", "NoiseBank", "NoiseClips", "SpecAugment", "TempoGain", "tempo_gain", "collate_waves", "stft_features_packed","FlatParams", "FusedAdam", "NoamOpt", "adam_step", "clip_grad_norm_", "DataParallelStep", "HostBatchPrefetcher", "shard_batch", "lm_train"]
+           "precision", "manual_seed", "attention_maps", "spectrogram_batch", "NoiseBank", "NoiseClips", "SpecAugment", "TempoGain", "tempo_gain", "SpeedPerturb", "resample", "collate_waves", "stft_features_packed","FlatParams", "FusedAdam", "NoamOpt", "adam_step", "clip_grad_norm_", "DataParallelStep", "HostBatchPrefetcher", "shard_batch", "lm_train"]

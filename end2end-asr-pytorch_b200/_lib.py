@@ -60,6 +60,7 @@ SIGNATURES = {
     "b200asr_spec_augment_draws_ints": (_sz, [_i, _i]),
     "b200asr_spec_augment": (_i, [_vp] * 4 + [_i] * 7 + [_f, _i, C.c_ulonglong, C.c_ulonglong, _vp]),
     "b200asr_tempo_gain": (_i, [_vp] * 10 + [_i] * 4 + [_vp]),
+    "b200asr_resample_packed": (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _i, _i, _vp]),
     "b200asr_conv3x3_c1_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_c1_bwd_weight": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b200asr_conv3x3_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),

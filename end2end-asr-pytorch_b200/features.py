@@ -13,11 +13,15 @@ whole batch is a single 3xTF32 tensor-core GEMM over overlapping frame rows.
 and makes the reference's random draws (host data: DataLoader workers draw with it); `NoiseBank` adds the clips on the
 device.  `SpecAugment` is an opt-in augmentation policy both helpers (and loader.py) apply to their output on the device;
 `TempoGain` (with `tempo_gain`) is the reference's tempo and gain perturbation, which collate_waves (and loader.py) apply to
-the waveforms before the features.  loader.py feeds the reference's AudioDataLoader from here.
+the waveforms before the features.  `SpeedPerturb` (with `resample`, a polyphase resampler restating
+scipy.signal.resample_poly) is speed perturbation, applied after the tempo and gain; `NoiseBank` resamples noise clips
+at other rates with the same kernel (loader.py does so for a dataset with `resample_noise = True`).  loader.py feeds the reference's AudioDataLoader from here.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
+from fractions import Fraction
+from math import gcd
 from typing import Sequence
 
 import numpy as np
@@ -56,15 +60,20 @@ class NoiseDraws:
 
 class NoiseClips:
     """Where the noise clips of `NoiseInjection` (utils/data_loader.py:147-179) lie in a `NoiseBank`: their lengths in
-    samples, their offsets when back to back, and their sample rate.  Host data that pickles, so DataLoader workers make
-    the reference's draws with it (loader.py) while the samples stay on the device."""
+    samples, their offsets when back to back, and their sample rate; and each clip's own duration in seconds, which the
+    draws use as the reference uses get_audio_length (lengths / sample_rate unless a clip was resampled).  Host data that
+    pickles, so DataLoader workers make the reference's draws with it (loader.py) while the samples stay on the device."""
 
-    def __init__(self, lengths, sample_rate: int):
+    def __init__(self, lengths, sample_rate: int, durations=None):
         self.lengths = np.asarray(lengths, dtype=np.int64).reshape(-1)
         if len(self.lengths) == 0:
             raise ValueError("NoiseBank needs at least one clip")
         self.offsets = np.concatenate([[0], np.cumsum(self.lengths)[:-1]]).astype(np.int64)
         self.sample_rate = int(sample_rate)
+        self.durations = self.lengths / self.sample_rate if durations is None else \
+            np.asarray(durations, dtype=np.float64).reshape(-1)
+        if len(self.durations) != len(self.lengths):
+            raise ValueError(f"{len(self.durations)} durations for {len(self.lengths)} clips")
 
     def __len__(self):
         return len(self.lengths)
@@ -75,7 +84,7 @@ class NoiseClips:
         `rng` is np.random (the reference's global state) or a RandomState.  Returns (add, clip, level, rand, start): clip
         -1, level and rand NaN, start -1 without noise.
 
-        The segment start is noise_start = rand * (clip_len / sr - n / sr) seconds, in float64 as :169-172.  The reference
+        The segment start is noise_start = rand * (duration - n / sr) seconds, in float64 as :169-172.  The reference
         then cuts the segment with sox `trim` (utils/audio.py:21-32); that cut is not pinned here but restated as the
         sample round(noise_start * sr), clamped so that the n samples fit in the clip; `start` is that sample's index in
         the bank.  A clip shorter than the utterance, where the reference fails its assert (:175), raises ValueError."""
@@ -88,7 +97,7 @@ class NoiseClips:
         clip_len = int(self.lengths[c])
         if clip_len < n:
             raise ValueError(f"noise clip {c} has {clip_len} samples, fewer than an utterance's {n}")
-        noise_start = rand * (clip_len / self.sample_rate - n / self.sample_rate)
+        noise_start = rand * (float(self.durations[c]) - n / self.sample_rate)
         return 1, c, level, rand, int(self.offsets[c]) + min(max(round(noise_start * self.sample_rate), 0), clip_len - n)
 
     def check(self, clip, start, lengths):
@@ -106,15 +115,35 @@ class NoiseClips:
 class NoiseBank:
     """Noise clips for `NoiseInjection` (utils/data_loader.py:147-179), back to back in one device buffer.
 
-    `clips` are 1-D fp32 waveforms at `sample_rate`, in the order `librosa.util.find_files(noise_dir)` lists them (sorted
-    paths): `draw` picks clips by index, so that order is what makes its choices the reference's.  Reading and resampling
-    the files is the caller's job.  `clips` (a NoiseClips) is the host side the draws need."""
+    `clips` are 1-D fp32 waveforms, in the order `librosa.util.find_files(noise_dir)` lists them (sorted paths): `draw`
+    picks clips by index, so that order is what makes its choices the reference's.  `rates` gives each clip's integer
+    sample rate (None: all at `sample_rate`).  Clips at another rate are resampled to `sample_rate` on the device, all in
+    one `resample` launch with quantize16 -- the reference's `sox ... -r sr -b 16` -- and keep their own duration
+    (samples / rate) for the draws; ValueError for a rate whose ratio to `sample_rate` exceeds RESAMPLE_MAX_RATE in
+    lowest terms.  `clips` (a NoiseClips) is the host side the draws need."""
 
-    def __init__(self, clips, sample_rate: int, device=None):
+    def __init__(self, clips, sample_rate: int, device=None, rates=None):
         arrays = [np.asarray(c.detach().cpu() if isinstance(c, torch.Tensor) else c, dtype=np.float32).reshape(-1) for c in clips]
-        self.clips = NoiseClips([len(a) for a in arrays], sample_rate)
+        sr = int(sample_rate)
+        rates = [sr] * len(arrays) if rates is None else [int(r) for r in rates]
+        if len(rates) != len(arrays) or min(rates, default=1) < 1:
+            raise ValueError(f"NoiseBank: rates {rates!r} for {len(arrays)} clips")
+        other = [i for i, r in enumerate(rates) if r != sr]
+        ratios = {i: resample_ratio(sr, rates[i]) for i in other}
+        lengths = [resample_out_length(len(a), *ratios[i]) if i in ratios else len(a) for i, a in enumerate(arrays)]
+        self.clips = NoiseClips(lengths, sr, [len(a) / r for a, r in zip(arrays, rates)])
         device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.bank = torch.from_numpy(np.concatenate(arrays)).to(device)
+        host = np.zeros(sum(lengths), np.float32)
+        for i, a in enumerate(arrays):
+            if i not in ratios:
+                host[self.clips.offsets[i]:self.clips.offsets[i] + len(a)] = a
+        self.bank = torch.from_numpy(host).to(device)
+        if any(lengths[i] for i in other):         # written in place into their slots of the bank
+            src = [arrays[i] for i in other]
+            src_off = np.concatenate([[0], np.cumsum([len(a) for a in src])[:-1]]).astype(np.int64)
+            _resample(torch.from_numpy(np.concatenate(src + [np.zeros(1, np.float32)])).to(device), src_off,
+                      [len(a) for a in src], [ratios[i][0] for i in other], [ratios[i][1] for i in other], True,
+                      out=self.bank, out_offsets=self.clips.offsets[other])
 
     sample_rate = property(lambda self: self.clips.sample_rate)
     lengths = property(lambda self: self.clips.lengths)
@@ -354,6 +383,155 @@ def tempo_gain(wave: torch.Tensor, offsets, lengths, tempo, gain_db, sample_rate
     return (out, out_off, out_len, pk, pk_off) if picks else (out, out_off, out_len)
 
 
+RESAMPLE_MAX_RATE = 1000
+
+
+def resample_ratio(up, down) -> tuple[int, int]:
+    """(up, down) in lowest terms; ValueError unless both are integers >= 1 and the larger is at most RESAMPLE_MAX_RATE."""
+    for v in (up, down):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+            raise ValueError(f"resample: up={up!r}, down={down!r} must be integers >= 1")
+    g = gcd(int(up), int(down))
+    up, down = int(up) // g, int(down) // g
+    if max(up, down) > RESAMPLE_MAX_RATE:
+        raise ValueError(f"resample: {up}/{down} exceeds {RESAMPLE_MAX_RATE} in lowest terms")
+    return up, down
+
+
+def resample_out_length(n: int, up: int, down: int) -> int:
+    """ceil(n * up / down): resample_poly's output length for a reduced ratio."""
+    return -(-int(n) * int(up) // int(down))
+
+
+def resample_filter(up: int, down: int) -> np.ndarray:
+    """resample_poly's default filter for a reduced ratio, in float64: firwin(2 half + 1, 1 / max(up, down),
+    window=('kaiser', 5.0)) * up, half = 10 max(up, down), restated with numpy (np.i0 for the Bessel function, which can
+    differ from scipy.special.i0 in the last bit)."""
+    mr = max(up, down)
+    numtaps, fc = 2 * 10 * mr + 1, 1.0 / mr
+    m = np.arange(numtaps, dtype=np.float64) - 0.5 * (numtaps - 1)
+    h = fc * np.sinc(fc * m)
+    n = np.arange(numtaps, dtype=np.float64)
+    alpha = (numtaps - 1) / 2.0
+    h *= np.i0(5.0 * np.sqrt(1 - ((n - alpha) / alpha) ** 2.0)) / np.i0(np.float64(5.0))
+    h /= np.sum(h)
+    return h * up
+
+
+def resample_taps(up: int, down: int) -> np.ndarray:
+    """The kernel's taps for a reduced ratio (up / down != 1): resample_filter split per phase, [up, K] fp32 with
+    taps[p, m] = h[p + m up] and zeros past the filter, K = ceil((2 half + 1) / up)."""
+    h = resample_filter(up, down)
+    K = -(-len(h) // up)
+    return np.pad(h, (0, up * K - len(h))).reshape(K, up).T.astype(np.float32)
+
+
+_TAPS: dict = {}            # (device, up, down) -> the ratio's taps on that device, uploaded once
+
+
+def _device_taps(up: int, down: int, device) -> torch.Tensor:
+    key = (str(device), up, down)
+    if key not in _TAPS:
+        _TAPS[key] = torch.from_numpy(np.ascontiguousarray(resample_taps(up, down))).to(device)
+    return _TAPS[key]
+
+
+_RESAMPLE_ITEM = np.dtype([("in_offset", "<i8"), ("out_offset", "<i8"), ("taps", "<u8"), ("in_length", "<i4"),
+                           ("up", "<i4"), ("down", "<i4"), ("reserved", "<i4")])     # b200asr_resample_item
+
+
+def _resample(wave, offsets, lengths, ups, downs, quantize16, out=None, out_offsets=None):
+    """One b200asr_resample_packed launch.  wave on the device; offsets, lengths and the reduced ratios host data.  The
+    outputs go back to back in batch order into a new buffer, or into `out` at the host `out_offsets`.  Returns (out,
+    out_offsets, out_lengths), the last two int64 host arrays."""
+    device = wave.device
+    host = lambda a: np.asarray(a.numpy() if isinstance(a, torch.Tensor) else a, dtype=np.int64).reshape(-1)  # noqa: E731
+    offsets, lengths, ups, downs = host(offsets), host(lengths), host(ups), host(downs)
+    B = len(lengths)
+    out_lengths = np.array([resample_out_length(n, u, d) for n, u, d in zip(lengths, ups, downs)], dtype=np.int64)
+    if out is None:
+        out_offsets = np.concatenate([[0], np.cumsum(out_lengths)[:-1]]).astype(np.int64)
+        out = torch.empty(max(1, int(out_lengths.sum())), device=device, dtype=torch.float32)
+    items = np.zeros(B, _RESAMPLE_ITEM)
+    items["in_offset"], items["out_offset"], items["in_length"] = offsets, host(out_offsets), lengths
+    items["up"], items["down"] = ups, downs
+    items["taps"] = [0 if u == d == 1 else _device_taps(int(u), int(d), device).data_ptr() for u, d in zip(ups, downs)]
+    items_d = _pinned_to(items.view(np.uint8), device)      # held until the launch: a freed block would be reused
+    L.check(ops._lib().b200asr_resample_packed(L.ptr(wave), wave.numel(), L.ptr(out), out.numel(), items.ctypes.data,
+                                               L.ptr(items_d), B, int(bool(quantize16)), ops._stream()), "resample_packed")
+    return out, host(out_offsets), out_lengths
+
+
+def resample(wave: torch.Tensor, offsets, lengths, up, down, quantize16: bool = False):
+    """scipy.signal.resample_poly(x, up[b], down[b]) with its defaults for every utterance of a packed batch, in fp32 (the
+    algorithm and the summation order: include/b200asr.h).  Utterance b is the lengths[b] samples of the 1-D CUDA fp32
+    `wave` from offsets[b] on; offsets, lengths and the per-utterance `up` and `down` (reduced here; at most
+    RESAMPLE_MAX_RATE in lowest terms) are host data, uploaded through pinned memory, so there is no host
+    synchronisation.  A ratio of 1 copies.  quantize16=True rounds the outputs to the 16-bit grid as `sox -b 16` writes
+    them (round to nearest, clamped, no dither).  One launch.
+
+    Returns (out, out_offsets, out_lengths): the ceil(n up / down) outputs of every utterance back to back in batch order
+    (a 1-D CUDA fp32 tensor, at least one element), their int64 offsets and int32 lengths on the device."""
+    ops._need_cuda(wave)
+    for name, a in (("offsets", offsets), ("lengths", lengths)):
+        if isinstance(a, torch.Tensor) and a.is_cuda:
+            raise ValueError(f"resample: {name} must be host data (the launch is checked on the host)")
+    lens = np.asarray(lengths.numpy() if isinstance(lengths, torch.Tensor) else lengths, dtype=np.int64).reshape(-1)
+    offs = np.asarray(offsets.numpy() if isinstance(offsets, torch.Tensor) else offsets, dtype=np.int64).reshape(-1)
+    up, down = np.asarray(up).reshape(-1), np.asarray(down).reshape(-1)
+    B = len(lens)
+    if not B or len(offs) != B or len(up) != B or len(down) != B:
+        raise ValueError(f"resample: {B} lengths, {len(offs)} offsets, {len(up)} ups and {len(down)} downs")
+    ratios = [resample_ratio(u.item(), d.item()) for u, d in zip(up, down)]
+    out, out_off, out_len = _resample(ops._f32c(wave), offs, lens, [r[0] for r in ratios], [r[1] for r in ratios], quantize16)
+    device = wave.device
+    return out, _pinned_to(out_off, device), _pinned_to(out_len.astype(np.int32), device)
+
+
+class SpeedPerturb:
+    """Speed perturbation (Ko et al. 2015, "Audio augmentation for speech recognition"): per utterance a factor drawn
+    uniformly from `factors` resamples the waveform by up / down = 1 / factor, which changes its tempo and pitch together
+    (a factor 1.1 plays 10 % faster: 10 / 11 as many samples).  The resampling is `resample` (scipy.signal.resample_poly
+    restated, include/b200asr.h); a factor of 1 copies.  Each factor is taken as the exact decimal Fraction(str(f)).
+
+    A SpeedPerturb holds plain numbers, so it pickles (DataLoader workers receive it with the dataset it is attached to)."""
+
+    def __init__(self, factors=(0.9, 1.0, 1.1)):
+        try:
+            fs = list(factors)
+        except TypeError:
+            raise ValueError(f"SpeedPerturb: factors={factors!r} is not a sequence") from None
+        if not fs:
+            raise ValueError("SpeedPerturb: no factors")
+        for f in fs:
+            if isinstance(f, bool) or not isinstance(f, (int, float, np.integer, np.floating)) or not np.isfinite(f) or f <= 0:
+                raise ValueError(f"SpeedPerturb: factor {f!r} must be a finite number > 0")
+            up, down = self.ratio(f)
+            if max(up, down) > RESAMPLE_MAX_RATE:
+                raise ValueError(f"SpeedPerturb: factor {f!r} gives the ratio {up}/{down}, beyond {RESAMPLE_MAX_RATE} in "
+                                 "lowest terms")
+        self.factors = tuple(float(f) for f in fs)
+
+    def __repr__(self):
+        return f"SpeedPerturb(factors={self.factors})"
+
+    def draw_one(self, rng=np.random) -> float:
+        """One rng.choice over the factors (`rng` is np.random, the worker's global state, or a RandomState); returns the
+        factor drawn."""
+        return self.factors[int(rng.choice(len(self.factors)))]
+
+    @staticmethod
+    def ratio(f) -> tuple[int, int]:
+        """(up, down) = 1 / Fraction(str(f)) in lowest terms: (10, 11) for 1.1, (10, 9) for 0.9, (1, 1) for 1.0."""
+        r = 1 / Fraction(str(f))
+        return r.numerator, r.denominator
+
+    @staticmethod
+    def out_length(n: int, f) -> int:
+        """Samples of an utterance of `n` samples at factor f: ceil(n up / down)."""
+        return resample_out_length(n, *SpeedPerturb.ratio(f))
+
+
 def _geometry(sample_rate, window_size, window_stride):
     return int(sample_rate * window_size), int(sample_rate * window_stride)
 
@@ -438,7 +616,7 @@ def spectrogram_batch(waves: Sequence[torch.Tensor] | torch.Tensor, lengths: tor
 
 def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBank | None = None, normalize: bool = True,
                   rng=np.random, precision: int | None = None, reflect: bool = True, spec_augment: SpecAugment | None = None,
-                  tempo_gain: TempoGain | None = None):
+                  tempo_gain: TempoGain | None = None, speed_perturb: SpeedPerturb | None = None):
     """`_collate_fn` (utils/data_loader.py:182-214) over waveforms: what a DataLoader over the reference's
     `SpectrogramDataset` yields, computed on the device.
 
@@ -451,6 +629,9 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     (the reference's `augment=True`): each utterance draws its tempo and gain, then its noise for the stretched length,
     in batch order as `__getitem__` draws them, and the batch is stretched on the device (one `tempo_gain` launch)
     before the features; the frame counts are those of the stretched utterances.  None: no stretch and no such draw.
+    `speed_perturb`: a SpeedPerturb: each utterance draws its factor after its tempo and gain and before its noise, the
+    noise is drawn for the resampled length, and the batch is resampled on the device (one `resample` launch) after the
+    stretch and before the features.  None: no resampling and no such draw.
 
     Returns (inputs [B,1,F,T] fp32 on the current CUDA device, targets [B,max_tgt] int64, input_percentages [B] fp32,
     input_sizes [B] int32, target_sizes [B] int32), the last four on the host, sorted by frame count, longest first
@@ -465,23 +646,22 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     noisy = audio_conf.get("noise_dir") is not None
     if noisy and noise_bank is None:
         raise ValueError("audio_conf['noise_dir'] is set but no noise_bank was given")
-    draws = None
-    if tempo_gain is None:
-        if noisy:
-            draws = noise_bank.draw(lens, audio_conf["noise_prob"], audio_conf["noise_levels"], rng)
-        out_lens = lens
-    else:
+    if tempo_gain is not None:
         TempoGain.geometry(sr)                        # a rate without a valid geometry fails before any draw
-        stretch, rows, out_lens = [], [], []
-        for n in lens:                                # per utterance: tempo and gain, then the noise of the stretched length
+    stretch, speed, rows, out_lens = [], [], [], []
+    for n in lens:                                    # per utterance: tempo and gain, speed, then the noise of the final length
+        if tempo_gain is not None:
             t, gain_db = tempo_gain.draw_one(rng)
-            m = TempoGain.out_length(n, t)
-            stretch.append((t, TempoGain.linear_gain(gain_db)))
-            out_lens.append(m)
-            if noisy:
-                rows.append(noise_bank.clips.draw_one(m, audio_conf["noise_prob"], audio_conf["noise_levels"], rng))
+            n = TempoGain.out_length(n, t)
+            stretch.append((t, TempoGain.linear_gain(gain_db), n))
+        if speed_perturb is not None:
+            up, down = speed_perturb.ratio(speed_perturb.draw_one(rng))
+            n = resample_out_length(n, up, down)
+            speed.append((up, down))
+        out_lens.append(n)
         if noisy:
-            draws = noise_bank._draws(rows)
+            rows.append(noise_bank.clips.draw_one(n, audio_conf["noise_prob"], audio_conf["noise_levels"], rng))
+    draws = noise_bank._draws(rows) if noisy else None
     frames = [min(1 + n // hop, src_max_len) for n in out_lens]
     order = sorted(range(len(batch)), key=frames.__getitem__, reverse=True)          # sorted(..., reverse=True) is stable
     B, Lmax = len(batch), max(1, max(out_lens))
@@ -494,9 +674,15 @@ def collate_waves(batch, audio_conf: dict, src_max_len: int, noise_bank: NoiseBa
     device = torch.device("cuda", torch.cuda.current_device())
     wave, wave_offsets, wave_lens = host.to(device, non_blocking=True), _pinned_to(offsets, device), _pinned_to(slens, device)
     if tempo_gain is not None:
+        tlens = np.array([stretch[i][2] for i in order], np.int32)
         wave, wave_offsets, wave_lens, _, _ = _tempo_gain(
             wave, wave_offsets, wave_lens, np.array([stretch[i][0] for i in order], np.float64),
-            np.array([stretch[i][1] for i in order], np.float32), np.array([out_lens[i] for i in order], np.int32), sr)
+            np.array([stretch[i][1] for i in order], np.float32), tlens, sr)
+        offsets, slens = np.concatenate([[0], np.cumsum(tlens, dtype=np.int64)[:-1]]), tlens
+    if speed_perturb is not None:
+        wave, offsets, slens = _resample(wave, offsets, slens, [speed[i][0] for i in order], [speed[i][1] for i in order],
+                                         False)
+        wave_offsets, wave_lens = _pinned_to(offsets, device), _pinned_to(slens.astype(np.int32), device)
     sout = np.array([out_lens[i] for i in order], dtype=np.int64)
     dev_noise = None if draws is None else noise_bank._device_args(draws.take(order), sout, device)
     t_max = frames[order[0]]

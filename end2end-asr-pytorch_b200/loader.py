@@ -22,12 +22,26 @@ attribute (a features.TempoGain) has its workers read the audio with the referen
 frame count use the stretched length, and each batch is stretched on the device (one `b200asr_tempo_gain` launch) before
 its features.  An `augment=True` dataset without the attribute keeps the reference's sox path; the attribute on an
 `augment=False` dataset is a ValueError when the loader is built.
+
+Speed perturbation is opt-in per dataset as well, with or without `augment`: a SpectrogramDataset with a `speed_perturb`
+attribute (a features.SpeedPerturb) has its workers draw each utterance's factor from np.random after the item's own
+`--augment` draws and before its noise draws (an extra draw the reference does not make, so every later draw of that
+worker shifts); the noise draw and the frame count use the resampled length, and each batch is resampled on the device
+(one `b200asr_resample_packed` launch) after its tempo and gain and before its features.
+
+Resampling noise clips on the device is opt-in per dataset: a noise clip at another sample rate than the dataset's
+makes the installed loader run the reference's own loader (which resamples the segment it cuts with sox, in the worker,
+per utterance), unless the SpectrogramDataset has `resample_noise = True`.  Then every such clip is resampled once, when
+the clips are read, on the device (16-bit output, as sox's `-r sr -b 16` writes it), and the device path serves the
+dataset; only a clip whose rate cannot be inferred from its duration and sample count, or whose ratio to the dataset's
+rate the resampler does not take, still runs the reference's loader.
 """
 from __future__ import annotations
 
 import importlib
 import inspect
 import random
+from math import gcd
 from typing import NamedTuple
 
 import numpy as np
@@ -53,12 +67,20 @@ class Item(NamedTuple):
     out_length: int = -1
 
 
+# An Item of a dataset with speed_perturb: the Item's fields, then the ratio (up, down) of the factor drawn and the length
+# `speed_length` the (stretched) waveform is resampled to on the device.
+ResampledItem = NamedTuple("ResampledItem", list(Item.__annotations__.items()) + [("up", int), ("down", int),
+                                                                                   ("speed_length", int)])
+
+
 class PackedBatch(NamedTuple):
     """A batch as the workers collate it, sorted as `_collate_fn` sorts (frames, longest first, stable): the waveforms
     back to back (`wave`, at least one sample) at int64 `offsets` with int32 `lengths`; per utterance the noise clip,
     start (int64, -1 without noise) and level (fp32); `_collate_fn`'s four host tensors; the src_max_len of the cut.
     With a dataset's tempo_gain: per utterance the tempo (float64), linear gain (fp32) and stretched length (int32) the
-    waveforms are stretched with before their features; None (the default) when nothing is stretched."""
+    waveforms are stretched with before their features; None (the default) when nothing is stretched.  With a dataset's
+    speed_perturb: per utterance the ratio (up, down, int32) and the resampled length (int32); None when nothing is
+    resampled."""
     wave: torch.Tensor
     offsets: torch.Tensor
     lengths: torch.Tensor
@@ -73,6 +95,9 @@ class PackedBatch(NamedTuple):
     tempo: torch.Tensor | None = None
     g: torch.Tensor | None = None
     out_lengths: torch.Tensor | None = None
+    up: torch.Tensor | None = None
+    down: torch.Tensor | None = None
+    speed_lengths: torch.Tensor | None = None
 
 
 def _data_loader():
@@ -109,6 +134,11 @@ class PackedItems(Dataset):
         if policy is not None:
             n = policy.out_length(n, tempo)
             stretch = (tempo, float(policy.linear_gain(gain_db)), n)
+        speed = getattr(ds, "speed_perturb", None)
+        if speed is not None:                                                 # resampled on the device
+            up, down = speed.ratio(speed.draw_one(np.random))
+            n = features.resample_out_length(n, up, down)
+            stretch = (stretch or tuple(Item._field_defaults.values())) + (up, down, n)     # no stretch: its defaults
         clip, start, level = -1, -1, float("nan")
         if ds.noiseInjector:
             if self.clips is None:
@@ -116,7 +146,8 @@ class PackedItems(Dataset):
             _, clip, level, _, start = self.clips.draw_one(n, ds.noise_prob, ds.noiseInjector.noise_levels, np.random)
         transcript = ds.parse_transcript(transcript_path)
         src_max_len = importlib.import_module("utils.constant").args.src_max_len      # read at call time, as :131
-        return Item(y, clip, start, level, transcript, min(1 + n // self.hop, src_max_len), *stretch)
+        return (Item if speed is None else ResampledItem)(y, clip, start, level, transcript, min(1 + n // self.hop, src_max_len),
+                                                           *stretch)
 
 
 def collate_items(items) -> PackedBatch:
@@ -134,11 +165,18 @@ def collate_items(items) -> PackedBatch:
     stretched = [it.out_length >= 0 for it in items]
     if any(stretched) and not all(stretched):
         raise ValueError("collate_items: a batch mixes stretched and unstretched utterances")
+    resampled = [isinstance(it, ResampledItem) for it in items]
+    if any(resampled) and not all(resampled):
+        raise ValueError("collate_items: a batch mixes resampled and unresampled utterances")
     stretch = {}
     if all(stretched):
         stretch = dict(tempo=torch.tensor([it.tempo for it in items], dtype=torch.float64),
                        g=torch.tensor([it.g for it in items], dtype=torch.float32),
                        out_lengths=torch.tensor([it.out_length for it in items], dtype=torch.int32))
+    if all(resampled):
+        stretch.update(up=torch.tensor([it.up for it in items], dtype=torch.int32),
+                       down=torch.tensor([it.down for it in items], dtype=torch.int32),
+                       speed_lengths=torch.tensor([it.speed_length for it in items], dtype=torch.int32))
     return PackedBatch(
         wave=torch.from_numpy(wave),
         offsets=torch.from_numpy(np.concatenate([[0], np.cumsum(lengths)[:-1]]).astype(np.int64)),
@@ -151,6 +189,20 @@ def collate_items(items) -> PackedBatch:
         input_sizes=torch.tensor([it.frames for it in items], dtype=torch.int32),
         target_sizes=torch.tensor([len(it.ids) for it in items], dtype=torch.int32),
         src_max_len=int(importlib.import_module("utils.constant").args.src_max_len), **stretch)
+
+
+def clip_rate(n: int, duration: float, sample_rate: int) -> int | None:
+    """A noise clip's integer sample rate from its sample count `n` and its duration in seconds (get_audio_length):
+    `sample_rate` when round(duration * sample_rate) == n, else r = round(n / duration) when round(duration * r) == n;
+    None when neither holds (or the duration is not a positive finite number)."""
+    if not np.isfinite(duration):
+        return None
+    if round(duration * sample_rate) == n:
+        return int(sample_rate)
+    if duration <= 0:
+        return None
+    r = int(round(n / duration))
+    return r if r >= 1 and round(duration * r) == n else None
 
 
 def _window_name(ds, DL) -> str:
@@ -177,8 +229,10 @@ class PackedLoader:
     def prepare(self) -> bool:
         """Read the noise clips into a NoiseBank on the current device, once, before any worker starts.  False when the
         reference's loader has to run: noise_dir holds no clips (the reference then fails only on a draw that adds
-        noise, never at noise_prob 0), or a clip whose duration (get_audio_length) does not give its sample count at the
-        dataset's sample rate would be resampled by sox, which is not restated here."""
+        noise, never at noise_prob 0), or a clip's duration (get_audio_length) does not give its sample count at the
+        dataset's sample rate, so that sox would resample it -- unless the dataset has `resample_noise = True`: then a clip
+        at another rate (clip_rate) is resampled to the dataset's rate on the device, and only a clip whose rate cannot
+        be inferred, or whose ratio to the dataset's rate is beyond the resampler's, runs the reference's loader."""
         ds = self.items.dataset
         if self.reference or not ds.noiseInjector:
             return not self.reference
@@ -187,14 +241,17 @@ class PackedLoader:
                 self.reference = True
                 return False
             DL, sr = _data_loader(), ds.sample_rate
-            clips = []
+            resample = getattr(ds, "resample_noise", False)
+            clips, rates = [], []
             for path in ds.noiseInjector.paths:
                 y = np.asarray(DL.load_audio(path), dtype=np.float32).reshape(-1)
-                if round(DL.get_audio_length(path) * sr) != len(y):
+                r = clip_rate(len(y), DL.get_audio_length(path), sr)
+                if r is None or (r != sr and not resample) or max(sr, r) // gcd(int(sr), r) > features.RESAMPLE_MAX_RATE:
                     self.reference = True
                     return False
                 clips.append(y)
-            self.bank = features.NoiseBank(clips, sr)
+                rates.append(r)
+            self.bank = features.NoiseBank(clips, sr, rates=rates)
             self.items.clips = self.bank.clips
         device = torch.device("cuda", torch.cuda.current_device())
         if self.bank.bank.device != device:
@@ -209,9 +266,14 @@ class PackedLoader:
         sr = ds.sample_rate
         wave, offsets, lengths_d = up(pb.wave), up(pb.offsets), up(pb.lengths)
         lengths = pb.lengths.numpy()
+        offsets_h = pb.offsets.numpy()
         if pb.out_lengths is not None:                          # the stretched waveforms replace the read ones
             wave, offsets, lengths_d, _, _ = features._tempo_gain(wave, offsets, lengths_d, pb.tempo, pb.g, pb.out_lengths, sr)
             lengths = pb.out_lengths.numpy()
+            offsets_h = np.concatenate([[0], np.cumsum(lengths, dtype=np.int64)[:-1]])
+        if pb.speed_lengths is not None:                        # then the resampled ones replace those
+            wave, offsets_h, lengths = features._resample(wave, offsets_h, lengths, pb.up.numpy(), pb.down.numpy(), False)
+            offsets, lengths_d = features._pinned_to(offsets_h, device), features._pinned_to(lengths.astype(np.int32), device)
         noise = None
         if self.bank is not None:
             noise = self.bank.device_args(pb.noise_clip.numpy(), pb.noise_start, pb.noise_level, lengths, device)
@@ -263,13 +325,16 @@ def audio_loader_init(self, *args, **kwargs):
 
 def audio_loader_iter(self):
     """AudioDataLoader.__iter__ after install(): device batches from the PackedLoader, or the reference's iterator
-    (original(AudioDataLoader, "__iter__")) for a loader without one, without noise clips or with clips at another rate."""
+    (original(AudioDataLoader, "__iter__")) for a loader without one, without noise clips or with a clip at another rate
+    that the dataset does not resample on the device (PackedLoader.prepare)."""
     packed = self.__dict__.get("_b200asr_packed")
     if packed is None or not packed.prepare():
-        for attr in ("spec_augment", "tempo_gain"):                      # the reference's iterator would drop it silently
+        for attr in ("spec_augment", "tempo_gain", "speed_perturb"):     # the reference's iterator would drop it silently
             if getattr(self.dataset, attr, None) is not None:
                 raise RuntimeError(f"the dataset carries {attr}, which only the device front end applies; this loader "
-                                   "runs the reference's own iterator (a collate_fn was given, or the noise clips need sox)")
+                                   "runs the reference's own iterator (a collate_fn was given, or a noise clip is at "
+                                   "another sample rate: set the dataset's resample_noise = True to resample it on the "
+                                   "device)")
         from .install import original
         return original(type(self), "__iter__")(self)
     return _Batches(packed)

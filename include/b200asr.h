@@ -709,6 +709,46 @@ int b200asr_tempo_gain(const float* in, const long long* in_offsets, const int* 
                        const long long* pick_offsets, int B, int segment, int search, int overlap,
                        b200asr_stream_t stream);
 
+/* One utterance of b200asr_resample_packed: its in_length samples start at in + in_offset, its outputs at out + out_offset;
+ * up / down is its ratio in lowest terms; taps is a device array of the ratio's phase-split filter (below), NULL allowed
+ * for up == down == 1.  40 bytes, 8-byte aligned. */
+typedef struct {
+  long long in_offset;
+  long long out_offset;
+  const float* taps;
+  int in_length;
+  int up;
+  int down;
+  int reserved;
+} b200asr_resample_item;
+
+/* Polyphase resampling of a packed batch of waveforms: utterance b becomes scipy.signal.resample_poly(x, up, down) with
+ * its defaults, computed in fp32.  That function is the contract, restated here:
+ *   up / down in lowest terms (the caller reduces by the gcd).  up == down == 1: y = x, copied, not filtered.  Otherwise
+ *   half = 10 max(up, down) and h = firwin(2 half + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up: the windowed
+ *   sinc h_k = w_k sin(pi f (k - half)) / (pi (k - half)) (f for k = half), w the symmetric Kaiser window of beta 5,
+ *   scaled to unit sum, then times up, designed in float64 and rounded once to fp32.  x is zero outside [0, n) (scipy's
+ *   padtype='constant'), and with scipy's delay compensation the n_out = ceil(n up / down) outputs are
+ *     y[i] = sum_j h[i down + half - j up] x[j]    over 0 <= i down + half - j up <= 2 half.
+ *   taps, phase-split: with K = ceil((2 half + 1) / up), taps[p K + m] = fp32(h[p + m up]) for p < up, m < K (0 past
+ *   2 half).  Output i, with c = i down + half, p = c mod up and j0 = floor(c / up), is the fp32 sum
+ *   s = fma(taps[p K + m], x[j0 - m], s) over m = 0, 1, ... while p + m up <= 2 half, from s = 0, in that order: the
+ *   bits do not depend on the batch, the launch or the run.
+ *   quantize16 = 1 writes clamp(rint(y * 32768), -32768, 32767) / 32768 instead (half to even, no dither; NaN stays
+ *   NaN), the grid `sox ... -b 16 -e si` writes; 0 writes y.
+ * items: B host descriptors, read and checked before launch; items_dev: a device copy of the same B descriptors, which the
+ * kernel reads (the library does not compare them).  in_size / out_size: floats in the in / out buffers.
+ *
+ * One launch: CTA (chunk, utterance) stages the input window of up to 2048 consecutive outputs in shared memory.
+ * Rejections, which launch and write nothing: a NULL in, out, items or items_dev, a quantize16 other than 0 or 1, out
+ * overlapping in, or a NULL or misaligned taps where up / down != 1 (B200ASR_BAD_ARG); in or out not 4-byte, items_dev
+ * not 8-byte aligned (B200ASR_BAD_ALIGN); B < 1, a negative in_size or out_size, up or down outside [1, 1000] or not
+ * coprime, an input outside [0, in_size), an output outside [0, out_size), or two outputs that overlap
+ * (B200ASR_BAD_SHAPE).  A batch whose outputs are all empty launches nothing. */
+int b200asr_resample_packed(const float* in, long long in_size, float* out, long long out_size,
+                            const b200asr_resample_item* items, const b200asr_resample_item* items_dev, int B,
+                            int quantize16, b200asr_stream_t stream);
+
 /* SpecAugment (Park et al. 2019, "SpecAugment: A Simple Data Augmentation Method for Automatic Speech Recognition") over a
  * batch of the front end's output: in, out [B,1,F,T] fp32 (the layout above), frames [B] int32 (device) = each
  * utterance's frame count after the src_max_len cut (input_sizes), read as T_b = min(max(frames[b], 0), T).  Applied in
